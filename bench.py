@@ -5,7 +5,7 @@
 
 metric   : StyleGAN2-256 images/sec (BASELINE.json), synthetic random z, seeded random weights
 workload : SeqStyleGAN2(256, mconv='seq') generator forward, batch=32 per GPU, fp32 in/out,
-           conv operands 3-term split bf16 on tcgen05 tensor cores (fp32 accumulate)
+           conv operands 3-term split bf16 on wgmma tensor cores (fp32 accumulate)
 step     : one batch of 32 latents through the whole generator -> 32 images (per GPU)
 value    : images/s with z resident in HBM, CUDA-event timed, max over ranks, whole job
 e2e      : same through the public API with HOST buffers: pinned z -> H2D, model(z), D2H of
@@ -20,7 +20,10 @@ extra    : the other BASELINE.json configs as stated —
              uint8 NHWC out, pipelined D2H;
            config 2: fused StyledConv forward + backward over all 13 layer shapes (N = 1 only)
 roofline : dominant kernel = conv_tc (implicit-GEMM styled conv); achieved = algorithmic conv
-           FLOPs / summed CUDA-event kernel time, against the MEASURED bf16 tensor peak
+           FLOPs / summed CUDA-event kernel time, against the dense bf16 tensor peak
+outputs  : --dump-outputs DIR writes the images of the last timed step (rank 0) as
+           DIR/images.npy (float32 [32, 3, 256, 256], 25 MB); z and weights are seeded, so two
+           builds run with the same arguments can be compared output for output
 cpu_baseline / --impl reference: the CPU oracle port of the reference's PyTorch path
            (oracle/sg2_oracle.py; the Python reference itself cannot travel to the GPU box)
            timed on the host cores on a bounded sample (batch 2).
@@ -89,7 +92,7 @@ def measured_peaks():
         return dict(tflops=float(d.get('bf16_tflops_sustained', d.get('bf16_tflops', 1590.0))),
                     hbm=float(d.get('hbm_gbs', 6650.0)), source='measured (MEASURED_PEAKS.json, '
                     'sustained bf16 GEMM)')
-    return dict(tflops=1400.0, hbm=6650.0, source='fallback (B200_PROFILING.md)')
+    return dict(tflops=989.0, hbm=3350.0, source='H100 SXM data sheet (dense bf16, HBM3), not measured')
 
 
 class ClockSampler(object):
@@ -254,6 +257,8 @@ def main():
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-graph', action='store_true',
                     help='time eager module calls instead of the CUDA-graph replay')
+    ap.add_argument('--dump-outputs', metavar='DIR',
+                    help='write the images of the last timed step (rank 0) to DIR/images.npy')
     args = ap.parse_args()
     if args.impl == 'reference':
         return run_reference(args)
@@ -283,7 +288,7 @@ def main():
     z_all = zdataset.standard_z_sample(BATCH * n_batches * world, 512, seed=1)
     z_mine = z_all[rank * BATCH * n_batches:(rank + 1) * BATCH * n_batches].contiguous()
     z_dev = z_mine.to(device)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=device)   # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=device)   # > 50 MB L2
 
     def barrier():
         if world > 1:
@@ -347,6 +352,8 @@ def main():
         e1.record()
         barrier()
         ms_dev = max_over_ranks(e0.elapsed_time(e1))
+        # a graph replay returns its static output buffer: copy it before anything replays again
+        last_images = img.float().cpu() if args.dump_outputs and rank == 0 else None
         launches = launches_per_step * K          # a graph replay launches the same kernels
         # per-kernel CUDA-event timing of the dominant kernel: eager replay of the same steps
         # (events cannot be read back from inside a graph), CPU running ahead of the GPU
@@ -443,22 +450,7 @@ def main():
 
     if rank == 0:
         peaks = measured_peaks()
-        # DRAM bytes per launch of the dominant kernel class: ncu (dram__bytes_read.sum +
-        # dram__bytes_write.sum) over every conv launch of one forward of THIS command, digested
-        # by tools/dram_summary.py into profiles/ (a profiler cannot run inside the timed bench)
-        traffic, traffic_note = None, None
-        prof = os.path.join(ROOT, 'profiles', 'r2_dram_per_launch.json')
-        if os.path.exists(prof):
-            try:
-                with open(prof) as f:
-                    dj = json.load(f)
-                ent = dj['kernels']['conv (conv_tc + upconv_fused)']
-                traffic = ent['dram_bytes_per_launch']
-                traffic_note = ('mean over the %d styled-conv launches of one forward, %s; '
-                                'algorithmic bytes per launch %.3g' % (
-                                    ent['launches'], dj['source'], ent['algorithmic_bytes_per_launch']))
-            except Exception:
-                traffic = None
+        traffic, traffic_note = None, 'not measured'
         achieved = (conv_flops / 1e12) / (conv_ms / 1e3) if conv_ms > 0 else 0.0
         line = {
             'metric': METRIC, 'value': value, 'unit': 'images/s', 'n_gpus': world, 'steps': K,
@@ -485,10 +477,9 @@ def main():
                                      'value is the %s' % (ms_eager / K, 'CUDA-graph replay of the '
                                      'same module call' if use_graph else 'eager call'),
                          'peak_source': peaks['source'],
-                         'note': 'algorithmic FLOPs (1x) against the cuBLAS-measured sustained bf16 '
-                                 'peak; the 3-term split issues 3x the MMAs, so frac ~ 1/3 means the '
-                                 'tensor pipe is as busy as in a cuBLAS GEMM; tensor-pipe utilisation '
-                                 'per layer is in profiles/'},
+                         'note': 'algorithmic FLOPs (1x) against the bf16 peak; the 3-term split '
+                                 'issues 3x the MMAs, so frac ~ 1/3 means the tensor pipe is as busy '
+                                 'as in a single-pass bf16 GEMM at that peak'},
             'e2e': {'value': e2e_value, 'unit': 'images/s', 'ms_per_step': ms_e2e / K,
                     'h2d_bytes_per_step': BATCH * 512 * 4,
                     'd2h_bytes_per_step': BATCH * 3 * SIZE * SIZE * 4},
@@ -504,11 +495,7 @@ def main():
                 'conv_transpose + 4x4 blur + demod + noise + bias + leaky-ReLU + next-layer planes in one '
                 'launch; FLOPs counted for the conv_transpose only)', 'kernel_launches': up_launches,
                 'kernel_ms_per_step': up_ms / K,
-                'note': 'layer 13 is epilogue-bound (SIMT FIR + activation behind the MMAs: 5.2k cycles '
-                        'per row step against 3.7k of MMAs), layers 9/11 wait for the MMAs half of the '
-                        'time (3-term split: frac <= 1/3), tools/prof_upconv.py + DESIGN.md §6; the '
-                        'round-1 pair (conv_transpose GEMM + SIMT blur) moved 2.3x the DRAM bytes of the '
-                        'layer pair'}
+                'note': '3-term split: frac <= 1/3; the conv_transpose output never leaves the SM'}
         if cov is not None and 'samples_per_s' in cov:
             # second half of BASELINE.json's metric: key-covariance samples/s (config 3)
             cov_tf = cov['samples_per_s'] * GFLOP_PER_COV_SAMPLE / 1e3
@@ -525,6 +512,10 @@ def main():
             line['cpu_baseline'] = {'value': None, 'unit': 'images/s', 'cores': os.cpu_count(),
                                     'kind': 'port', 'sample': 'measured at N=1 only'}
         print(json.dumps(line), flush=True)
+    if last_images is not None:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, 'images.npy'), last_images.numpy())
     if world > 1:
         dist.destroy_process_group()
     return 0
@@ -615,11 +606,8 @@ def bench_config4(model, device):
                 'fp32_TFLOPs': flop_it * its / 1e12,
                 'hbm_equivalent_GBps_if_state_streamed': state_bytes * its / 1e9,
                 'note': 'W[o] lives in shared memory for all iterations, m/v stream through L2; '
-                        'the key crop is re-read from L2 by every 4-channel CTA twice per iteration. '
-                        'ncu (profiles/r2_ncu_insert_before_details.txt): DRAM 0.03 %, L2 3.8 %, L2 hit '
-                        '99.4 %, issue slots 46 %, 8 warps/SM at 255 registers: latency-bound '
-                        '(stall_wait / long_scoreboard on the L2 key loads), 128 of 148 SMs busy '
-                        '(512 output channels / 4 per CTA)'}}
+                        'the key crop is re-read from L2 by every 4-channel CTA twice per iteration; '
+                        '128 CTAs (512 output channels / 4 per CTA) on the 132 SMs'}}
 
 
 def bench_config5(model, device, world, barrier, max_over_ranks, nimgs):

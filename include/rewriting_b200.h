@@ -74,7 +74,7 @@ int rw_prep_weights(const float* w, int Cout, int Cin, float scale, int transpos
 int rw_demod(const float* style, const float* wsq, int B, int Cout, int Cin, float eps,
              float* demod, rw_stream_t stream);
 
-/* ---- fused modulated 3x3 convolution (tcgen05) ---- */
+/* ---- fused modulated 3x3 convolution (wgmma) ---- */
 /* out[b,o,y,x] = act( conv3x3(k, scale*W)[b,o,y,x] * scale_bo[b,o] + noise_w[0]*noise[b,y*W+x] + bias[o] )
  * scale_bo / noise / bias may be NULL; noise_w is a DEVICE scalar (the nn.Parameter's storage,
  * so no host sync per layer); act: 0 none, 1 leaky_relu(0.2)*sqrt(2). */
@@ -179,7 +179,7 @@ int rw_upfirdn2d(const float* in, const float* kernel, int major, int in_h, int 
                  int kw, int up_x, int up_y, int down_x, int down_y, int pad_x0, int pad_x1,
                  int pad_y0, int pad_y1, float* out, int out_h, int out_w, rw_stream_t stream);
 
-/* ---- key second moment / weight gradient (tcgen05 col-GEMM) ---- */
+/* ---- key second moment / weight gradient (wgmma col-GEMM) ---- */
 size_t rw_gram_workspace_bytes(int Cm, int Cn, long long rows, int ntaps);
 /* mom2[C,C] += sum_r a_r a_r^T over `rows` rows of the hi/lo planes [rows][C] */
 int rw_second_moment_accum(const void* hi, const void* lo, long long rows, int C, float* mom2,
@@ -302,7 +302,7 @@ int rw_debug_colgemm(const void* a_hi, const void* a_lo, const void* b_hi, const
                      void* workspace, size_t workspace_bytes, rw_stream_t stream);
 
 /* rw_modconv_up_fused instrumented with clock64(): prof_out[grid][8 epilogue warps][16] = cycles in
- * {wait for the MMAs, TMEM drain, combine + mailbox + barrier, shuffles, edge-lane fix-ups,
+ * {wait for the MMAs, accumulator exchange, combine + mailbox + barrier, shuffles, edge-lane fix-ups,
  * horizontal FIR, vertical FIR + activation + stores}, the step count, and the last phase split into
  * {FIR + activation + bf16 split, wait for the staging slots, stmatrix + fence + pair barrier, TMA store issue} and
  * the third of those into {stmatrix, fence.proxy.async, pair barrier} */

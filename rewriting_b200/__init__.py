@@ -1,4 +1,4 @@
-"""rewriting_b200 — Blackwell-native hot path of davidbau/rewriting.
+"""rewriting_b200 — Hopper-native (H100) hot path of davidbau/rewriting.
 
 Layout: `csrc/` (CUDA kernels + C-ABI, built into librw_b200.so), `ops` (torch-facing
 wrappers / autograd), `utils/` and `rewrite/` (host-side mirror of the reference's operator,

@@ -1,4 +1,4 @@
-"""Build librw_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build librw_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
 The library is plain `extern "C"` (include/rewriting_b200.h); it is loaded with
 ctypes by rewriting_b200._cabi.  Nothing here links against torch.
@@ -13,7 +13,7 @@ CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'librw_b200.so')
 SOURCES = ['api.cu', 'conv_tc.cu', 'upconv_tc.cu', 'gram_tc.cu', 'simt.cu', 'bwd.cu', 'rewrite.cu']
 NVCC_FLAGS = [
-    '-gencode', 'arch=compute_100a,code=sm_100a',
+    '-gencode', 'arch=compute_90a,code=sm_90a',
     '-lineinfo', '-O3', '-std=c++17',
     '-Xcompiler', '-fPIC',
     '-cudart', 'shared',
@@ -65,7 +65,7 @@ def build(force=False, verbose=False):
     if failed:
         raise RuntimeError('nvcc compilation failed')
     cmd = [nvcc, '-shared', '-o', LIB] + objs + ['-cudart', 'shared',
-                                                  '-gencode', 'arch=compute_100a,code=sm_100a']
+                                                  '-gencode', 'arch=compute_90a,code=sm_90a']
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError('link failed:\n' + r.stdout)

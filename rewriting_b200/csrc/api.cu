@@ -30,11 +30,11 @@ int check_cuda(cudaError_t e, const char* what) {
 int device_sm_count() {
   static int cached[64] = {0};
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
   if (cached[dev] == 0) {
     int n = 0;
     if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
-      n = 148;
+      n = 132;
     cached[dev] = n;
   }
   return cached[dev];
@@ -153,7 +153,7 @@ int make_tmap_nd_bf16(CUtensorMap* out, const void* base, int rank, const uint64
 // split heuristic shared by the workspace query and the launches
 static int gram_splits(int tiles, long long rows, int ntaps) {
   const long long total_rb = (rows + 63) / 64;
-  const int sms = 148;
+  const int sms = device_sm_count();
   long long s = (sms + static_cast<long long>(tiles) * ntaps - 1) / (static_cast<long long>(tiles) * ntaps);
   if (s > total_rb) s = total_rb;
   if (s < 1) s = 1;

@@ -1,4 +1,4 @@
-// conv_tc.cu — tcgen05 implicit-GEMM over the padded-flat key layout ("row-GEMM").
+// conv_tc.cu — wgmma implicit-GEMM over the padded-flat key layout ("row-GEMM").
 //
 //   acc[p, o] = sum_{tap} sum_{i} KP[p + shift(tap), i] * Wt[o, tap, i]
 //
@@ -19,9 +19,8 @@
 // each term optional, so the same kernel serves the un-fused `dconv` leaf of a
 // nethook-split layer, the conv_transpose phases of an up layer and dgrad.
 //
-// Warp roles (192 threads): warp0 = TMA producer, warp1 = MMA issuer (+TMEM
-// alloc), warps 2..5 = epilogue (TMEM -> regs -> global).  Persistent CTAs,
-// 3-stage smem ring, double-buffered TMEM accumulators.
+// Warp roles (288 threads): warpgroups 0 and 1 each issue wgmma for 64 of the tile's 128 rows and
+// run the epilogue on their register accumulators; warp 8 is the TMA producer.  Persistent CTAs, 3-stage shared-memory ring.
 #include <cstdlib>
 #include <cstring>
 
@@ -33,56 +32,29 @@ namespace rw {
 namespace {
 
 constexpr int BM = 128;
+constexpr int BN = 128;
 constexpr int BK = 64;            // bf16 elements per k-block = one 128B swizzle row
-constexpr int UMMA_K = 16;
+constexpr int MMA_K = 16;
 constexpr int kStages = 3;
-// warp 0 = TMA producer, warp 1 = MMA issuer, warps 2..9 = epilogue: two warps per TMEM lane
-// quarter, each owning 64 of the tile's 128 columns (64 fp32 running sums per thread: no spills,
-// and twice the epilogue throughput for the short-K phase tiles of the upsampling layers)
-constexpr int kNumThreads = 320;
-constexpr int kEpiWarps = 8;
-constexpr int kEpiCols = 64;
-// The tensor core's fp32 accumulate truncates (round-toward-zero) on every MMA: measured
-// relative bias ~ -2^-25 per accumulation (profiles/r1_precision_probe.json), i.e. 1.6e-5
-// after the 864 accumulations of a K=4608 tile.  So a TMEM accumulator only ever holds a
-// CHUNK of kChunkKB k-blocks (K=512: 96 accumulations); the epilogue warps add the chunks in
-// fp32 registers with round-to-nearest.  kNumAcc TMEM buffers form a ring between the MMA
-// issuer and the epilogue.
-// (kChunkKB must stay a compile-time constant: a run-time chunk bound cost 15 % in this kernel —
-//  measured chunk 8 -> pixel error 5.2e-4, chunk 16 -> 8.1e-4, >= 36 fails the 1e-3 bound)
+constexpr int kNumThreads = 288;   // two consumer warpgroups + the producer warp
+constexpr int kTmaWarp = 8;
+// The tensor core's fp32 accumulate truncates (round-toward-zero) on every MMA, a relative bias of
+// ~ -2^-25 per accumulation, i.e. 1.6e-5 after the 864 accumulations of a K=4608 tile.  So the
+// wgmma accumulator only ever holds a CHUNK of kChunkKB k-blocks (K=512: 96 accumulations); the
+// chunks are added in fp32 registers with round-to-nearest.
+// (chunk 8 -> pixel error 5.2e-4, chunk 16 -> 8.1e-4, >= 36 fails the 1e-3 bound)
 constexpr int kChunkKB = 8;
-// Measured (tools/cuda/mma_rate.cu, profiles/r1_mma_rate.txt): an M=128,K=16 bf16 MMA costs
-// 75 cycles for N <= 128 and 128 cycles for N = 256.  Issuing A_hi x [B_hi ; B_lo] as one N=256
-// instruction (203 instead of 225 cycles per k-step) was tried and changed nothing: the kernel
-// is bound by the depth of the TMA pipeline (bytes in flight vs L2 latency), not by the tensor
-// pipe, so the simpler three N=128 products are kept.
-template <int CG> struct AccGeom {
-  static constexpr int kAccCols = 128;                     // TMEM columns per accumulator
-  static constexpr int kNumAcc = 512 / kAccCols;           // ring depth
-};
 
-// CG = cta_group: 1 = one CTA per 128-row tile; 2 = CTA pair, 256-row tile, each CTA stages its
-// own 128 A rows and HALF of the B (weight) tile -> 25 % less shared-memory traffic per MMA,
-// which is what bounds the 1-CTA kernel (A 4 KB + B 4 KB read per 64-cycle MMA = 125 B/cycle).
-template <int BN, int CG>
 struct ConvSmem {
-  static constexpr int kStagesN = (CG == 2) ? 4 : kStages;
   static constexpr int kABytes = BM * BK * 2;          // one plane
-  static constexpr int kBBytes = (BN / CG) * BK * 2;   // one plane (this CTA's share)
+  static constexpr int kBBytes = BN * BK * 2;          // one plane
   static constexpr int kStageBytes = 2 * kABytes + 2 * kBBytes;
-  // per-epilogue-warp transpose scratch: 32 rows x (64 B + 16 B pad)
-  static constexpr int kScratchRow = 80;
-  static constexpr int kScratchBytes = kEpiWarps * 32 * kScratchRow;
-  static constexpr int kTotal = kStagesN * kStageBytes + kScratchBytes + 1024 /*align slack*/ +
-                                256 /*barriers*/;
+  static constexpr int kTotal = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
 struct Barriers {
-  uint64_t full[4];
-  uint64_t empty[4];
-  uint64_t tmem_full[4];
-  uint64_t tmem_empty[4];
-  uint32_t tmem_base;
+  uint64_t full[kStages];
+  uint64_t empty[kStages];
 };
 
 // tile -> (phase, mn).  Phases have very different tap counts (4/2/2/1 for a stride-2
@@ -98,11 +70,8 @@ __device__ __forceinline__ void decode_tile(int tile, int nphase, int nsched, in
 // EPI = 0: full fused epilogue (demod, noise, bias, leaky-ReLU, NCHW / channels-last store, next
 //          layer's planes, ToRGB partials — every feature a run-time switch).
 // EPI = 1: lean epilogue — optional per-(b,o) scale and the store, nothing else.  The up-path
-//          conv_transpose phases, dgrad and the plain row-GEMM use it: with 1-4 taps per tile the
-//          mainloop is short, and the generic epilogue's ~37 predicated instructions per column
-//          (2400 per tile and warp) made the MMA issuer wait for TMEM (ncu, layer 13: issuer
-//          spinning on tmem_empty, tensor pipe 52 %).
-template <int BN, int CG, int EPI>
+//          conv_transpose phases, dgrad and the plain row-GEMM use it.
+template <int EPI>
 __global__ void __launch_bounds__(kNumThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
                const __grid_constant__ CUtensorMap map_a_lo,
@@ -111,63 +80,42 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
-  using S = ConvSmem<BN, CG>;
-  constexpr int kSt = S::kStagesN;
-  constexpr int kNumAcc = AccGeom<CG>::kNumAcc;
-  constexpr int kAccCols = AccGeom<CG>::kAccCols;
-  static_assert(BN == 128, "accumulator geometry assumes 128-column tiles");
-  uint8_t* scratch_base = smem + kSt * S::kStageBytes;
-  Barriers* bars = reinterpret_cast<Barriers*>(scratch_base + S::kScratchBytes);
+  using S = ConvSmem;
+  Barriers* bars = reinterpret_cast<Barriers*>(smem + kStages * S::kStageBytes);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int cta_rank = (CG == 2) ? static_cast<int>(cluster_ctarank()) : 0;
-  const bool leader = (cta_rank == 0);
-  const int sched_id = blockIdx.x / CG;          // tile scheduler slot (one per CTA / CTA pair)
-  const int nsched = gridDim.x / CG;
+  const int nsched = gridDim.x;
 
-  const int m_tiles = (p.rows + BM * CG - 1) / (BM * CG);
+  const int m_tiles = (p.rows + BM - 1) / BM;
   const int n_tiles = p.Cout / BN;
   const int mn_tiles = m_tiles * n_tiles;
   const int num_tiles = mn_tiles * p.nphase;
   const int kb_per_tap = p.Cin / BK;
-  constexpr int chunk_kb = kChunkKB;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kTmaWarp && lane == 0) {
     tma_prefetch_desc(&map_a_hi);
     tma_prefetch_desc(&map_a_lo);
     tma_prefetch_desc(&map_w_hi);
     tma_prefetch_desc(&map_w_lo);
-    for (int s = 0; s < kSt; ++s) {
+    for (int s = 0; s < kStages; ++s) {
       mbar_init(&bars->full[s], 1);
-      mbar_init(&bars->empty[s], 1);
-    }
-    for (int s = 0; s < kNumAcc; ++s) {
-      mbar_init(&bars->tmem_full[s], 1);
-      mbar_init(&bars->tmem_empty[s], kEpiWarps * CG);   // epilogue warps of every CTA of the pair
+      mbar_init(&bars->empty[s], 2);      // one arrival per consumer warpgroup
     }
     fence_mbar_init();
   }
-  if (warp == 1) {
-    if constexpr (CG == 2) tmem_alloc_cg2<512>(&bars->tmem_base);
-    else tmem_alloc<512>(&bars->tmem_base);
-  }
-  tc_fence_before();
   __syncthreads();
-  if constexpr (CG == 2) cluster_sync_all();     // peer barriers are initialised
-  tc_fence_after();
-  const uint32_t tmem_base = bars->tmem_base;
 
-  if (warp == 0) {
+  if (warp == kTmaWarp) {
     // ------------------------------ TMA producer ------------------------------
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = sched_id; tile < num_tiles; tile += nsched) {
+      for (int tile = blockIdx.x; tile < num_tiles; tile += nsched) {
         int ph, mn;
         decode_tile(tile, p.nphase, nsched, ph, mn);
-        const int n0 = (mn % n_tiles) * BN + cta_rank * (BN / CG);
-        const int m0 = (mn / n_tiles) * BM * CG + cta_rank * BM;
+        const int n0 = (mn % n_tiles) * BN;
+        const int m0 = (mn / n_tiles) * BM;
         for (int t = 0; t < p.ph_ntaps[ph]; ++t) {
           const int arow = m0 + p.ph_shift[ph][t];
           const int wcol = p.ph_kofs[ph][t];
@@ -175,336 +123,218 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
           for (int kb = 0; kb < kb_per_tap; ++kb) {
             mbar_wait(&bars->empty[stage], phase ^ 1u);
             uint8_t* st = smem + stage * S::kStageBytes;
-            if constexpr (CG == 2) {
-              // both CTAs' bytes are credited to the leader's full barrier
-              if (leader) mbar_expect_tx(&bars->full[stage], 2 * S::kStageBytes);
-              tma_load_2d_cg2(st, &map_a_hi, &bars->full[stage], acol + kb * BK, arow);
-              tma_load_2d_cg2(st + S::kABytes, &map_a_lo, &bars->full[stage], acol + kb * BK, arow);
-              tma_load_2d_cg2(st + 2 * S::kABytes, &map_w_hi, &bars->full[stage], wcol + kb * BK, n0);
-              tma_load_2d_cg2(st + 2 * S::kABytes + S::kBBytes, &map_w_lo, &bars->full[stage],
-                              wcol + kb * BK, n0);
-            } else {
-              mbar_expect_tx(&bars->full[stage], S::kStageBytes);
-              tma_load_2d(st, &map_a_hi, &bars->full[stage], acol + kb * BK, arow);
-              tma_load_2d(st + S::kABytes, &map_a_lo, &bars->full[stage], acol + kb * BK, arow);
-              tma_load_2d(st + 2 * S::kABytes, &map_w_hi, &bars->full[stage], wcol + kb * BK, n0);
-              tma_load_2d(st + 2 * S::kABytes + S::kBBytes, &map_w_lo, &bars->full[stage],
-                          wcol + kb * BK, n0);
-            }
-            if (++stage == kSt) { stage = 0; phase ^= 1u; }
+            mbar_expect_tx(&bars->full[stage], S::kStageBytes);
+            tma_load_2d(st, &map_a_hi, &bars->full[stage], acol + kb * BK, arow);
+            tma_load_2d(st + S::kABytes, &map_a_lo, &bars->full[stage], acol + kb * BK, arow);
+            tma_load_2d(st + 2 * S::kABytes, &map_w_hi, &bars->full[stage], wcol + kb * BK, n0);
+            tma_load_2d(st + 2 * S::kABytes + S::kBBytes, &map_w_lo, &bars->full[stage],
+                        wcol + kb * BK, n0);
+            if (++stage == kStages) { stage = 0; phase ^= 1u; }
           }
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer --------------------------------
-    constexpr uint32_t idesc = make_idesc_bf16(BM * CG, BN, 0, 0);
-    int stage = 0;
-    uint32_t phase = 0;
-    uint32_t chunk = 0;     // running chunk counter of this CTA -> accumulator ring slot
-    // All 32 lanes run this loop with warp-uniform values so that descriptors live in uniform
-    // registers; one elected lane issues the tcgen05 instructions.  (Under a divergent
-    // `if (lane == 0)` the compiler wraps every MMA in an ELECT / R2UR.BROADCAST waterfall loop,
-    // which makes the single issuing thread the bottleneck: 12 MMAs of 75 cycles per k-block.)
-    if (leader) {
-      for (int tile = sched_id; tile < num_tiles; tile += nsched) {
-        int ph_m, mn_m;
-        decode_tile(tile, p.nphase, nsched, ph_m, mn_m);
-        const int num_kb = p.ph_ntaps[ph_m] * kb_per_tap;
-        for (int kb0 = 0; kb0 < num_kb; kb0 += chunk_kb, ++chunk) {
-          const int as = chunk % kNumAcc;
-          const uint32_t aphase = (chunk / kNumAcc) & 1u;
-          mbar_wait(&bars->tmem_empty[as], aphase ^ 1u);
-          tc_fence_after();
-          const uint32_t tmem_d = tmem_base + as * kAccCols;
-          const int kb_end = (kb0 + chunk_kb < num_kb) ? kb0 + chunk_kb : num_kb;
-          for (int kb = kb0; kb < kb_end; ++kb) {
-            mbar_wait(&bars->full[stage], phase);
-            tc_fence_after();
-            const uint32_t sa = smem_u32(smem + stage * S::kStageBytes);
-            const uint64_t da_hi = make_smem_desc(sa, 16, 1024, kSwizzle128B);
-            const uint64_t da_lo = make_smem_desc(sa + S::kABytes, 16, 1024, kSwizzle128B);
-            const uint64_t db_hi = make_smem_desc(sa + 2 * S::kABytes, 16, 1024, kSwizzle128B);
-            const uint64_t db_lo =
-                make_smem_desc(sa + 2 * S::kABytes + S::kBBytes, 16, 1024, kSwizzle128B);
-            if (elect_one()) {
+    return;
+  }
+
+  // ------------------------- MMA + epilogue (consumers) ------------------------
+  const int wg = threadIdx.x >> 7;            // 64-row half of the tile
+  const int g = lane >> 2, c = lane & 3;
+  const int img = p.Hp * p.Wp;
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += nsched) {
+    int ph, mn;
+    decode_tile(tile, p.nphase, nsched, ph, mn);
+    const int num_kb = p.ph_ntaps[ph] * kb_per_tap;
+    const int n_tile = mn % n_tiles;
+    const int n0 = n_tile * BN;
+    const int m0 = (mn / n_tiles) * BM;
+
+    float acc[64], d[64];
 #pragma unroll
-              for (int kk = 0; kk < BK / UMMA_K; ++kk) {
-                const uint64_t adv = static_cast<uint64_t>((kk * UMMA_K * 2) >> 4);
-                // smallest terms first, then the dominant hi*hi product
-                if constexpr (CG == 2) {
-                  umma_bf16_cg2(tmem_d, da_lo + adv, db_hi + adv, idesc, ((kb - kb0) | kk) != 0);
-                  umma_bf16_cg2(tmem_d, da_hi + adv, db_lo + adv, idesc, 1u);
-                  umma_bf16_cg2(tmem_d, da_hi + adv, db_hi + adv, idesc, 1u);
-                } else {
-                  umma_bf16(tmem_d, da_lo + adv, db_hi + adv, idesc, ((kb - kb0) | kk) != 0);
-                  umma_bf16(tmem_d, da_hi + adv, db_lo + adv, idesc, 1u);
-                  umma_bf16(tmem_d, da_hi + adv, db_hi + adv, idesc, 1u);
-                }
-              }
-              if constexpr (CG == 2) umma_commit_cg2_mc(&bars->empty[stage]);
-              else umma_commit(&bars->empty[stage]);
-              if (kb + 1 == kb_end) {
-                if constexpr (CG == 2) umma_commit_cg2_mc(&bars->tmem_full[as]);
-                else umma_commit(&bars->tmem_full[as]);
-              }
-            }
-            __syncwarp();
-            if (++stage == kSt) { stage = 0; phase ^= 1u; }
-          }
+    for (int j = 0; j < 64; ++j) acc[j] = 0.f;
+    for (int kb0 = 0; kb0 < num_kb; kb0 += kChunkKB) {
+      const int kb_end = (kb0 + kChunkKB < num_kb) ? kb0 + kChunkKB : num_kb;
+      for (int kb = kb0; kb < kb_end; ++kb) {
+        mbar_wait(&bars->full[stage], phase);
+        const uint32_t sa = smem_u32(smem + stage * S::kStageBytes);
+        const uint64_t da_hi = make_smem_desc(sa + wg * (S::kABytes / 2), 16, 1024);
+        const uint64_t da_lo = make_smem_desc(sa + S::kABytes + wg * (S::kABytes / 2), 16, 1024);
+        const uint64_t db_hi = make_smem_desc(sa + 2 * S::kABytes, 16, 1024);
+        const uint64_t db_lo = make_smem_desc(sa + 2 * S::kABytes + S::kBBytes, 16, 1024);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < BK / MMA_K; ++kk) {
+          const uint64_t adv = static_cast<uint64_t>((kk * MMA_K * 2) >> 4);
+          // smallest terms first, then the dominant hi*hi product
+          wgmma_m64n128<0, 0>(d, da_lo + adv, db_hi + adv, ((kb - kb0) | kk) != 0);
+          wgmma_m64n128<0, 0>(d, da_hi + adv, db_lo + adv, 1u);
+          wgmma_m64n128<0, 0>(d, da_hi + adv, db_hi + adv, 1u);
         }
+        wgmma_commit();
+        wgmma_wait<0>();
+        if ((threadIdx.x & 127) == 0) mbar_arrive(&bars->empty[stage]);
+        if (++stage == kStages) { stage = 0; phase ^= 1u; }
       }
+#pragma unroll
+      for (int j = 0; j < 64; ++j) acc[j] += d[j];
     }
-  } else {
-    // ------------------------------ epilogue ----------------------------------
-    const int q = warp & 3;                 // TMEM lane quarter this warp may read
-    const int half = (warp - 2) >> 2;       // which 64 of the tile's 128 columns
-    const int cbase = half * kEpiCols;
-    const int img = p.Hp * p.Wp;
-    uint8_t* scr = scratch_base + (warp - 2) * 32 * S::kScratchRow;
-    uint32_t chunk = 0;
-    for (int tile = sched_id; tile < num_tiles; tile += nsched) {
-      int ph, mn;
-      decode_tile(tile, p.nphase, nsched, ph, mn);
-      const int num_kb = p.ph_ntaps[ph] * kb_per_tap;
-      const int Hv = p.ph_Hv[ph], Wv = p.ph_Wv[ph];
-      const int n0 = (mn % n_tiles) * BN + cbase;          // first output channel of this warp
-      const int m0 = (mn / n_tiles) * BM * CG + cta_rank * BM;
-      const int prow = m0 + q * 32 + lane;
+
+    // ---- fused epilogue: rows r = m0 + 64 wg + 16 (warp % 4) + g + 8 i, columns 8 j + 2 c + e ----
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int prow = m0 + wg * 64 + (warp & 3) * 16 + g + 8 * i;
       const int b = prow / img;
       const int rem = prow - b * img;
       const int yy = rem / p.Wp;
       const int xx = rem - yy * p.Wp;
-      const bool valid = (prow < p.rows) && (yy < Hv) && (xx < Wv);
-
-      float acc[kEpiCols];
+      const int Hv = p.ph_Hv[ph], Wv = p.ph_Wv[ph];
+      const bool in_rows = prow < p.rows;
+      const bool valid = in_rows && (yy < Hv) && (xx < Wv);
+      const float* scl = (p.scale_bo && in_rows) ? p.scale_bo + static_cast<size_t>(b) * p.Cout : nullptr;
+      float* outp = (p.out != nullptr && p.out_mode == 0 && valid)
+                        ? p.out + p.ph_out_ofs[ph] + static_cast<size_t>(b) * p.out_sb +
+                              static_cast<size_t>(yy) * p.out_sy + static_cast<size_t>(xx) * p.out_sx
+                        : nullptr;
+      if (EPI == 1 || !valid) {
+        // lean epilogue, and the pad rows of the full one: only the optional scale
+        if (scl && (EPI == 1 || p.out_mode == 1)) {
 #pragma unroll
-      for (int j = 0; j < kEpiCols; ++j) acc[j] = 0.f;
-
-      for (int kb0 = 0; kb0 < num_kb; kb0 += chunk_kb, ++chunk) {
-        const int as = chunk % kNumAcc;
-        const uint32_t aphase = (chunk / kNumAcc) & 1u;
-        mbar_wait(&bars->tmem_full[as], aphase);
-        tc_fence_after();
-#pragma unroll
-        for (int c0 = 0; c0 < kEpiCols; c0 += 32) {
-          uint32_t v[32];
-          const uint32_t taddr = tmem_base + static_cast<uint32_t>(as * kAccCols + cbase + c0) +
-                                 (static_cast<uint32_t>(q * 32) << 16);
-          tmem_ld_32x32(taddr, v);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 32; ++j) acc[c0 + j] += __uint_as_float(v[j]);
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) {
-          if constexpr (CG == 2) mbar_arrive_leader(&bars->tmem_empty[as]);
-          else mbar_arrive(&bars->tmem_empty[as]);
-        }
-      }
-
-      // ---- fused epilogue -------------------------------------------------------------
-      const float* scl = p.scale_bo ? p.scale_bo + static_cast<size_t>(b) * p.Cout : nullptr;
-      if constexpr (EPI == 1) {
-        if (scl != nullptr && prow < p.rows) {
-          const float4* s4 = reinterpret_cast<const float4*>(scl + n0);
-#pragma unroll
-          for (int j4 = 0; j4 < kEpiCols / 4; ++j4) {
-            const float4 sv = __ldg(s4 + j4);
-            acc[4 * j4] *= sv.x;
-            acc[4 * j4 + 1] *= sv.y;
-            acc[4 * j4 + 2] *= sv.z;
-            acc[4 * j4 + 3] *= sv.w;
+          for (int j = 0; j < 16; ++j) {
+            const float2 sv = __ldg(reinterpret_cast<const float2*>(scl + n0 + 8 * j + 2 * c));
+            acc[4 * j + 2 * i] *= sv.x;
+            acc[4 * j + 2 * i + 1] *= sv.y;
           }
         }
-        if (p.out_mode == 0 && valid) {
-          float* outp = p.out + p.ph_out_ofs[ph] + static_cast<size_t>(b) * p.out_sb +
-                        static_cast<size_t>(yy) * p.out_sy + static_cast<size_t>(xx) * p.out_sx +
-                        static_cast<size_t>(n0) * p.out_sc;
+        if (EPI == 1 && outp) {
 #pragma unroll
-          for (int j = 0; j < kEpiCols; ++j) outp[static_cast<size_t>(j) * p.out_sc] = acc[j];
+          for (int j = 0; j < 16; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e)
+              outp[static_cast<size_t>(n0 + 8 * j + 2 * c + e) * p.out_sc] = acc[4 * j + 2 * i + e];
         }
-      } else if (valid) {
+      } else {
         float nz = 0.f;
         if (p.noise != nullptr)
           nz = __ldg(p.noise_w) * __ldg(p.noise + static_cast<size_t>(b) * p.noise_bstride +
                                         static_cast<size_t>(yy) * Wv + xx);
-        float* outp = p.out + p.ph_out_ofs[ph] + static_cast<size_t>(b) * p.out_sb +
-                      static_cast<size_t>(yy) * p.out_sy + static_cast<size_t>(xx) * p.out_sx;
         const float act_gain = p.act_gain != 0.f ? p.act_gain : 1.4142135623730951f;
-        const float* rw0 = p.rgb_w ? p.rgb_w + (static_cast<size_t>(b) * 3) * p.Cout : nullptr;
-        float r0 = 0.f, r1 = 0.f, r2 = 0.f;
 #pragma unroll
-        for (int j = 0; j < kEpiCols; ++j) {
-          const int o = n0 + j;
-          float t = acc[j];
-          if (scl) t *= __ldg(scl + o);
-          t += nz;
-          if (p.bias) t += __ldg(p.bias + o);
-          if (p.act) t = (t > 0.f ? t : 0.2f * t) * act_gain;
-          acc[j] = t;
-          if (p.out != nullptr && p.out_mode == 0) outp[static_cast<size_t>(o) * p.out_sc] = t;
-          if (rw0) {
-            r0 = fmaf(__ldg(rw0 + o), t, r0);
-            r1 = fmaf(__ldg(rw0 + p.Cout + o), t, r1);
-            r2 = fmaf(__ldg(rw0 + 2 * p.Cout + o), t, r2);
+        for (int j = 0; j < 16; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int o = n0 + 8 * j + 2 * c + e;
+            float t = acc[4 * j + 2 * i + e];
+            if (scl) t *= __ldg(scl + o);
+            t += nz;
+            if (p.bias) t += __ldg(p.bias + o);
+            if (p.act) t = (t > 0.f ? t : 0.2f * t) * act_gain;
+            acc[4 * j + 2 * i + e] = t;
+            if (outp) outp[static_cast<size_t>(o) * p.out_sc] = t;
           }
-        }
-        if (rw0) {
-          // one partial per 64-channel group: rgb_part[(n_tile*2 + half)][b][c][y*Wv+x]
-          const size_t hw = static_cast<size_t>(Hv) * Wv;
-          float* rp = p.rgb_part +
-                      ((static_cast<size_t>((mn % n_tiles) * 2 + half) * p.B + b) * 3) * hw +
-                      static_cast<size_t>(yy) * Wv + xx;
-          rp[0] = r0;
-          rp[hw] = r1;
-          rp[2 * hw] = r2;
-        }
-      } else if (p.out_mode == 1 && prow < p.rows && scl) {
-        // channels-last raw rows are written for every row (pad rows are never read back)
-#pragma unroll
-        for (int j = 0; j < kEpiCols; ++j) acc[j] *= __ldg(scl + n0 + j);
       }
-      // Row-per-lane registers -> global through a warp-private smem transpose, so that every
-      // store instruction covers whole 64-byte row segments (8 rows x 64 B) instead of
-      // 32 rows x 16 B.
-      const int rr0 = lane >> 2;        // row within a group of 8
-      const int c16 = lane & 3;         // 16-byte column slot
-      if (p.out != nullptr && p.out_mode == 1) {
+      if (EPI == 0 && p.rgb_w != nullptr) {
+        // one partial per 64-channel group: rgb_part[(n_tile*2 + half)][b][c][y*Wv+x]; the four
+        // lanes of a row hold 16 of the group's channels each
+        const float* rw0 = p.rgb_w + (static_cast<size_t>(valid ? b : 0) * 3) * p.Cout;
 #pragma unroll
-        for (int c0 = 0; c0 < kEpiCols; c0 += 16) {
+        for (int half = 0; half < 2; ++half) {
+          float r0 = 0.f, r1 = 0.f, r2 = 0.f;
+          if (valid) {
 #pragma unroll
-          for (int j4 = 0; j4 < 4; ++j4)
-            *reinterpret_cast<float4*>(scr + lane * S::kScratchRow + j4 * 16) = make_float4(
-                acc[c0 + 4 * j4], acc[c0 + 4 * j4 + 1], acc[c0 + 4 * j4 + 2], acc[c0 + 4 * j4 + 3]);
-          __syncwarp();
+            for (int j = 8 * half; j < 8 * half + 8; ++j)
 #pragma unroll
-          for (int it = 0; it < 4; ++it) {
-            const int rr = it * 8 + rr0;
-            const int grow = m0 + q * 32 + rr;
-            const float4 v = *reinterpret_cast<const float4*>(scr + rr * S::kScratchRow + c16 * 16);
-            if (grow < p.rows)
-              *reinterpret_cast<float4*>(p.out + (static_cast<size_t>(ph) * p.rows + grow) * p.Cout +
-                                         n0 + c0 + c16 * 4) = v;
-          }
-          __syncwarp();
-        }
-      }
-      if (EPI == 0 && p.next_hi != nullptr) {
-        const float* ns = p.next_scale + static_cast<size_t>(valid ? b : 0) * p.Cout + n0;
-#pragma unroll
-        for (int part = 0; part < kEpiCols / 32; ++part) {      // 32 channels = 64 B per pass
-#pragma unroll
-          for (int plane = 0; plane < 2; ++plane) {
-#pragma unroll
-            for (int j8 = 0; j8 < 4; ++j8) {
-              uint32_t w[4];
-#pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const int j = part * 32 + j8 * 8 + 2 * e;
-                const float k0 = valid ? __ldg(ns + j) * acc[j] : 0.f;
-                const float k1 = valid ? __ldg(ns + j + 1) * acc[j + 1] : 0.f;
-                const __nv_bfloat162 hh = __floats2bfloat162_rn(k0, k1);
-                if (plane == 0) {
-                  w[e] = *reinterpret_cast<const uint32_t*>(&hh);
-                } else {
-                  const float2 hf = __bfloat1622float2(hh);
-                  const __nv_bfloat162 ll = __floats2bfloat162_rn(k0 - hf.x, k1 - hf.y);
-                  w[e] = *reinterpret_cast<const uint32_t*>(&ll);
-                }
+              for (int e = 0; e < 2; ++e) {
+                const int o = n0 + 8 * j + 2 * c + e;
+                const float t = acc[4 * j + 2 * i + e];
+                r0 = fmaf(__ldg(rw0 + o), t, r0);
+                r1 = fmaf(__ldg(rw0 + p.Cout + o), t, r1);
+                r2 = fmaf(__ldg(rw0 + 2 * p.Cout + o), t, r2);
               }
-              *reinterpret_cast<uint4*>(scr + lane * S::kScratchRow + j8 * 16) =
-                  make_uint4(w[0], w[1], w[2], w[3]);
-            }
-            __syncwarp();
-            __nv_bfloat16* dstp = static_cast<__nv_bfloat16*>(plane == 0 ? p.next_hi : p.next_lo);
-#pragma unroll
-            for (int it = 0; it < 4; ++it) {
-              const int rr = it * 8 + rr0;
-              const int grow = m0 + q * 32 + rr;
-              const uint4 v = *reinterpret_cast<const uint4*>(scr + rr * S::kScratchRow + c16 * 16);
-              if (grow < p.rows)
-                *reinterpret_cast<uint4*>(dstp + static_cast<size_t>(grow) * p.Cout + n0 + part * 32 +
-                                          c16 * 8) = v;
-            }
-            __syncwarp();
           }
+#pragma unroll
+          for (int s = 1; s < 4; s <<= 1) {
+            r0 += __shfl_xor_sync(0xffffffffu, r0, s);
+            r1 += __shfl_xor_sync(0xffffffffu, r1, s);
+            r2 += __shfl_xor_sync(0xffffffffu, r2, s);
+          }
+          if (valid && c == 0) {
+            const size_t hw = static_cast<size_t>(Hv) * Wv;
+            float* rp = p.rgb_part + ((static_cast<size_t>(n_tile * 2 + half) * p.B + b) * 3) * hw +
+                        static_cast<size_t>(yy) * Wv + xx;
+            rp[0] = r0;
+            rp[hw] = r1;
+            rp[2 * hw] = r2;
+          }
+        }
+      }
+      // channels-last raw rows are written for every row (pad rows are never read back)
+      if (p.out != nullptr && p.out_mode == 1 && in_rows) {
+        float* orow = p.out + (static_cast<size_t>(ph) * p.rows + prow) * p.Cout + n0 + 2 * c;
+#pragma unroll
+        for (int j = 0; j < 16; ++j)
+          *reinterpret_cast<float2*>(orow + 8 * j) = make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+      }
+      if (EPI == 0 && p.next_hi != nullptr && in_rows) {
+        const float* ns = p.next_scale + static_cast<size_t>(valid ? b : 0) * p.Cout + n0 + 2 * c;
+        const size_t ofs = static_cast<size_t>(prow) * p.Cout + n0 + 2 * c;
+        uint32_t* nh = reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(p.next_hi) + ofs);
+        uint32_t* nl = reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(p.next_lo) + ofs);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          float k0 = 0.f, k1 = 0.f;
+          if (valid) {
+            const float2 sv = __ldg(reinterpret_cast<const float2*>(ns + 8 * j));
+            k0 = sv.x * acc[4 * j + 2 * i];
+            k1 = sv.y * acc[4 * j + 2 * i + 1];
+          }
+          const __nv_bfloat162 hh = __floats2bfloat162_rn(k0, k1);
+          const float2 hf = __bfloat1622float2(hh);
+          const __nv_bfloat162 ll = __floats2bfloat162_rn(k0 - hf.x, k1 - hf.y);
+          nh[4 * j] = *reinterpret_cast<const uint32_t*>(&hh);
+          nl[4 * j] = *reinterpret_cast<const uint32_t*>(&ll);
         }
       }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if constexpr (CG == 2) cluster_sync_all();     // the peer may still signal our barriers / TMEM
-  if (warp == 1) {
-    tc_fence_after();
-    if constexpr (CG == 2) tmem_dealloc_cg2<512>(tmem_base);
-    else tmem_dealloc<512>(tmem_base);
   }
 }
 
 }  // namespace
 
-template <int CG, int EPI>
-static int conv_tc_launch_cg(const ConvTcParams& p, const void* a_hi, const void* a_lo,
-                             const void* w_hi, const void* w_lo, int wk_total,
-                             cudaStream_t stream) {
-  constexpr int BN = 128;
+template <int EPI>
+static int conv_tc_launch_epi(const ConvTcParams& p, const void* a_hi, const void* a_lo,
+                              const void* w_hi, const void* w_lo, int wk_total,
+                              cudaStream_t stream) {
   CUtensorMap ma_hi, ma_lo, mw_hi, mw_lo;
   int rc;
   const int a_cols = p.a_cols > 0 ? p.a_cols : p.Cin;
   if ((rc = make_tmap_2d_bf16(&ma_hi, a_hi, a_cols, p.rows, (uint64_t)a_cols * 2, BK, BM))) return rc;
   if ((rc = make_tmap_2d_bf16(&ma_lo, a_lo, a_cols, p.rows, (uint64_t)a_cols * 2, BK, BM))) return rc;
-  if ((rc = make_tmap_2d_bf16(&mw_hi, w_hi, wk_total, p.Cout, (uint64_t)wk_total * 2, BK, BN / CG)))
+  if ((rc = make_tmap_2d_bf16(&mw_hi, w_hi, wk_total, p.Cout, (uint64_t)wk_total * 2, BK, BN)))
     return rc;
-  if ((rc = make_tmap_2d_bf16(&mw_lo, w_lo, wk_total, p.Cout, (uint64_t)wk_total * 2, BK, BN / CG)))
+  if ((rc = make_tmap_2d_bf16(&mw_lo, w_lo, wk_total, p.Cout, (uint64_t)wk_total * 2, BK, BN)))
     return rc;
 
-  using S = ConvSmem<BN, CG>;
   static bool attr_set = false;
   if (!attr_set) {
-    rc = check_cuda(cudaFuncSetAttribute(conv_tc_kernel<BN, CG, EPI>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, S::kTotal),
+    rc = check_cuda(cudaFuncSetAttribute(conv_tc_kernel<EPI>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, ConvSmem::kTotal),
                     "conv_tc smem attr");
     if (rc) return rc;
     attr_set = true;
   }
-  const int m_tiles = (p.rows + BM * CG - 1) / (BM * CG);
+  const int m_tiles = (p.rows + BM - 1) / BM;
   const int n_tiles = p.Cout / BN;
   const int num_tiles = m_tiles * n_tiles * p.nphase;
-  int sched = device_sm_count() / CG;
+  int sched = device_sm_count();
   if (sched > num_tiles) sched = num_tiles;
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = dim3(sched * CG);
-  cfg.blockDim = dim3(kNumThreads);
-  cfg.dynamicSmemBytes = S::kTotal;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CG;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  if constexpr (CG == 1) {
-    conv_tc_kernel<BN, 1, EPI><<<sched, kNumThreads, S::kTotal, stream>>>(ma_hi, ma_lo, mw_hi, mw_lo,
-                                                                          p);
-    return check_cuda(cudaGetLastError(), "conv_tc launch");
-  }
-  return check_cuda(cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN, CG, EPI>, ma_hi, ma_lo, mw_hi, mw_lo, p),
-                    "conv_tc launch");
+  conv_tc_kernel<EPI><<<sched, kNumThreads, ConvSmem::kTotal, stream>>>(ma_hi, ma_lo, mw_hi, mw_lo, p);
+  return check_cuda(cudaGetLastError(), "conv_tc launch");
 }
-
-// 0 = automatic (CTA pairs when the launch has at least one full wave of 256-row tiles),
-// 1 / 2 = forced (tests, RW_CONV_CG environment variable)
-static int g_conv_cg = -1;
 
 int conv_tc_launch(const ConvTcParams& p, const void* a_hi, const void* a_lo, const void* w_hi,
                    const void* w_lo, int wk_total, cudaStream_t stream) {
-  constexpr int BN = 128;
   if (p.Cin % BK != 0 || p.Cout % BN != 0 || p.nphase < 1 || p.nphase > 4 || p.rows <= 0) {
     set_last_error("conv_tc: unsupported shape Cin=%d Cout=%d nphase=%d rows=%d", p.Cin, p.Cout,
                    p.nphase, p.rows);
@@ -515,26 +345,11 @@ int conv_tc_launch(const ConvTcParams& p, const void* a_hi, const void* a_lo, co
       set_last_error("conv_tc: phase %d has %d taps", i, p.ph_ntaps[i]);
       return RW_ERR_BAD_ARG;
     }
-  if (g_conv_cg < 0) {
-    const char* e = getenv("RW_CONV_CG");
-    g_conv_cg = e ? atoi(e) : 0;
-  }
-  int cg = g_conv_cg;
-  if (cg != 1 && cg != 2) {
-    // CTA pairs (4 stages of 48 KB, 25 % fewer bytes per MMA) for launches with at least one
-    // full wave of 256-row tiles; the single-CTA kernel for the small layers
-    const long long tiles256 = ((static_cast<long long>(p.rows) + 255) / 256) * (p.Cout / BN) * p.nphase;
-    cg = (tiles256 >= device_sm_count() / 2) ? 2 : 1;
-  }
   // lean epilogue when only the optional scale and the store are asked for
   const bool lean = !p.noise && !p.bias && !p.act && !p.rgb_w && !p.rgb_part && !p.next_hi &&
-                    p.out != nullptr && (reinterpret_cast<uintptr_t>(p.scale_bo) & 15u) == 0;
-  if (cg == 2) {
-    if (lean) return conv_tc_launch_cg<2, 1>(p, a_hi, a_lo, w_hi, w_lo, wk_total, stream);
-    return conv_tc_launch_cg<2, 0>(p, a_hi, a_lo, w_hi, w_lo, wk_total, stream);
-  }
-  if (lean) return conv_tc_launch_cg<1, 1>(p, a_hi, a_lo, w_hi, w_lo, wk_total, stream);
-  return conv_tc_launch_cg<1, 0>(p, a_hi, a_lo, w_hi, w_lo, wk_total, stream);
+                    p.out != nullptr && (reinterpret_cast<uintptr_t>(p.scale_bo) & 7u) == 0;
+  if (lean) return conv_tc_launch_epi<1>(p, a_hi, a_lo, w_hi, w_lo, wk_total, stream);
+  return conv_tc_launch_epi<0>(p, a_hi, a_lo, w_hi, w_lo, wk_total, stream);
 }
 
 }  // namespace rw

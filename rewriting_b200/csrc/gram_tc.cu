@@ -1,4 +1,4 @@
-// gram_tc.cu — tcgen05 "col-GEMM": contraction over pixel rows.
+// gram_tc.cu — wgmma "col-GEMM": contraction over pixel rows.
 //
 //   out[m, n] = sum_r A[r + shift_a, m] * B[r + shift_b, n]
 //
@@ -11,9 +11,9 @@
 // Operands are the bf16 hi/lo planes [rows][C] (channels contiguous), i.e. the
 // contraction index is the *slow* one: both operands are MN-major for the
 // tensor core.  TMA boxes of 64 channels x 64 rows land as 128-byte swizzled
-// rows; the UMMA descriptor walks 8-row groups with SBO and 64-channel blocks
+// rows; the wgmma descriptor walks 8-row groups with SBO and 64-channel blocks
 // with LBO.  Three MMAs per k-step (hi*hi + lo*hi + hi*lo), fp32 accumulate in
-// TMEM.  Row ranges are split across CTAs; partial tiles go to a workspace that
+// registers.  Row ranges are split across CTAs; partial tiles go to a workspace that
 // a second kernel reduces in a fixed order (bit-reproducible, unlike atomics).
 #include "rw_common.cuh"
 #include "rw_kernels.h"
@@ -25,14 +25,14 @@ namespace {
 constexpr int TM = 128;
 constexpr int TN = 128;
 constexpr int RB = 64;            // rows (contraction) per pipeline stage
-constexpr int UMMA_K = 16;
+constexpr int MMA_K = 16;
 constexpr int kStages = 3;
-constexpr int kNumThreads = 192;
-// fp32 accumulation in the tensor core truncates (see conv_tc.cu): a TMEM accumulator holds
+constexpr int kNumThreads = 288;  // warpgroups 0, 1: wgmma + epilogue (64 rows of M each); warp 8: TMA
+constexpr int kTmaWarp = 8;
+// fp32 accumulation in the tensor core truncates (see conv_tc.cu): the wgmma accumulator holds
 // at most kChunkRB row-blocks (1024 rows = 192 accumulations); chunks are summed in fp32
-// registers (round-to-nearest) by the epilogue warps.
+// registers (round-to-nearest).
 constexpr int kChunkRB = 16;
-constexpr int kNumAcc = 4;
 constexpr int kBlockBytes = 64 * RB * 2;       // one 64-channel x RB-row box
 constexpr int kPlaneBytes = (TM / 64) * kBlockBytes;
 constexpr int kStageBytes = 4 * kPlaneBytes;   // A_hi, A_lo, B_hi, B_lo
@@ -41,9 +41,6 @@ constexpr int kSmemTotal = kStages * kStageBytes + 1024 + 256;
 struct Barriers {
   uint64_t full[kStages];
   uint64_t empty[kStages];
-  uint64_t tmem_full[kNumAcc];
-  uint64_t tmem_empty[kNumAcc];
-  uint32_t tmem_base;
 };
 
 __global__ void __launch_bounds__(kNumThreads, 1)
@@ -88,28 +85,20 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
   if (rb_end > total_rb) rb_end = total_rb;
   const int num_rb = rb_end > rb_begin ? rb_end - rb_begin : 0;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kTmaWarp && lane == 0) {
     tma_prefetch_desc(&map_a_hi);
     tma_prefetch_desc(&map_a_lo);
     tma_prefetch_desc(&map_b_hi);
     tma_prefetch_desc(&map_b_lo);
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&bars->full[s], 1);
-      mbar_init(&bars->empty[s], 1);
-    }
-    for (int s = 0; s < kNumAcc; ++s) {
-      mbar_init(&bars->tmem_full[s], 1);
-      mbar_init(&bars->tmem_empty[s], 4);
+      mbar_init(&bars->empty[s], 2);      // one arrival per consumer warpgroup
     }
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<kNumAcc * TN>(&bars->tmem_base);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = bars->tmem_base;
 
-  if (warp == 0) {
+  if (warp == kTmaWarp) {
     if (lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -132,86 +121,51 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
         if (++stage == kStages) { stage = 0; phase ^= 1u; }
       }
     }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = make_idesc_bf16(TM, TN, 1, 1);
-    // warp-uniform loop, one elected lane issues (descriptors stay in uniform registers)
-    {
-      int stage = 0;
-      uint32_t phase = 0;
-      uint32_t chunk = 0;
-      for (int i0 = 0; i0 < num_rb; i0 += kChunkRB, ++chunk) {
-        const int as = chunk % kNumAcc;
-        const uint32_t aphase = (chunk / kNumAcc) & 1u;
-        mbar_wait(&bars->tmem_empty[as], aphase ^ 1u);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + as * TN;
-        const int i_end = (i0 + kChunkRB < num_rb) ? i0 + kChunkRB : num_rb;
-        for (int i = i0; i < i_end; ++i) {
-          mbar_wait(&bars->full[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * kStageBytes);
-          const uint64_t da_hi = make_smem_desc(sa, lbo_bytes, sbo_bytes, kSwizzle128B);
-          const uint64_t da_lo =
-              make_smem_desc(sa + kPlaneBytes, lbo_bytes, sbo_bytes, kSwizzle128B);
-          const uint64_t db_hi =
-              make_smem_desc(sa + 2 * kPlaneBytes, lbo_bytes, sbo_bytes, kSwizzle128B);
-          const uint64_t db_lo =
-              make_smem_desc(sa + 3 * kPlaneBytes, lbo_bytes, sbo_bytes, kSwizzle128B);
-          if (elect_one()) {
-#pragma unroll
-            for (int kk = 0; kk < RB / UMMA_K; ++kk) {
-              // 16 rows = two 8-row swizzle groups of 1024 B
-              const uint64_t adv = static_cast<uint64_t>((kk * UMMA_K * 128) >> 4);
-              umma_bf16(tmem_d, da_lo + adv, db_hi + adv, idesc, ((i - i0) | kk) != 0);
-              umma_bf16(tmem_d, da_hi + adv, db_lo + adv, idesc, 1u);
-              umma_bf16(tmem_d, da_hi + adv, db_hi + adv, idesc, 1u);
-            }
-            umma_commit(&bars->empty[stage]);
-            if (i + 1 == i_end) umma_commit(&bars->tmem_full[as]);
-          }
-          __syncwarp();
-          if (++stage == kStages) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
-  } else {
-    const int q = warp & 3;
-    const int row = m0 + q * 32 + lane;
-    float* dst = p.partial + (static_cast<size_t>(split) * p.Cm + row) * p.ldp + col_ofs + n0;
-    float acc[TN];
-#pragma unroll
-    for (int j = 0; j < TN; ++j) acc[j] = 0.f;
-    uint32_t chunk = 0;
-    for (int i0 = 0; i0 < num_rb; i0 += kChunkRB, ++chunk) {
-      const int as = chunk % kNumAcc;
-      const uint32_t aphase = (chunk / kNumAcc) & 1u;
-      mbar_wait(&bars->tmem_full[as], aphase);
-      tc_fence_after();
-#pragma unroll
-      for (int c0 = 0; c0 < TN; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_base + static_cast<uint32_t>(as * TN + c0) +
-                          (static_cast<uint32_t>(q * 32) << 16), v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 32; ++j) acc[c0 + j] += __uint_as_float(v[j]);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bars->tmem_empty[as]);
-    }
-#pragma unroll
-    for (int j = 0; j < TN; j += 4) {
-      *reinterpret_cast<float4*>(dst + j) = make_float4(acc[j], acc[j + 1], acc[j + 2], acc[j + 3]);
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<kNumAcc * TN>(tmem_base);
+  // warpgroup wg owns the 64 output rows m0 + 64 wg .. : its A operand is the wg-th 64-channel box
+  const int wg = threadIdx.x >> 7;
+  float acc[64], d[64];
+#pragma unroll
+  for (int j = 0; j < 64; ++j) acc[j] = 0.f;
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int i0 = 0; i0 < num_rb; i0 += kChunkRB) {
+    const int i_end = (i0 + kChunkRB < num_rb) ? i0 + kChunkRB : num_rb;
+    for (int i = i0; i < i_end; ++i) {
+      mbar_wait(&bars->full[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * kStageBytes);
+      const uint64_t da_hi = make_smem_desc(sa + wg * kBlockBytes, lbo_bytes, sbo_bytes);
+      const uint64_t da_lo = make_smem_desc(sa + kPlaneBytes + wg * kBlockBytes, lbo_bytes, sbo_bytes);
+      const uint64_t db_hi = make_smem_desc(sa + 2 * kPlaneBytes, lbo_bytes, sbo_bytes);
+      const uint64_t db_lo = make_smem_desc(sa + 3 * kPlaneBytes, lbo_bytes, sbo_bytes);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < RB / MMA_K; ++kk) {
+        // 16 rows = two 8-row swizzle groups of 1024 B
+        const uint64_t adv = static_cast<uint64_t>((kk * MMA_K * 128) >> 4);
+        wgmma_m64n128<1, 1>(d, da_lo + adv, db_hi + adv, ((i - i0) | kk) != 0);
+        wgmma_m64n128<1, 1>(d, da_hi + adv, db_lo + adv, 1u);
+        wgmma_m64n128<1, 1>(d, da_hi + adv, db_hi + adv, 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      if ((threadIdx.x & 127) == 0) mbar_arrive(&bars->empty[stage]);
+      if (++stage == kStages) { stage = 0; phase ^= 1u; }
+    }
+#pragma unroll
+    for (int j = 0; j < 64; ++j) acc[j] += d[j];
   }
+  // rows m0 + 64 wg + 16 (warp % 4) + lane / 4 (+ 8), columns 8 j + 2 (lane % 4) (+ 1)
+  const int row = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  float* dst = p.partial + (static_cast<size_t>(split) * p.Cm + row) * p.ldp + col_ofs + n0 + 2 * (lane & 3);
+#pragma unroll
+  for (int i = 0; i < 2; ++i)
+#pragma unroll
+    for (int j = 0; j < 16; ++j)
+      *reinterpret_cast<float2*>(dst + static_cast<size_t>(8 * i) * p.ldp + 8 * j) =
+          make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
 }
 
 // out[m, n] (= | +=) sum_s partial[s][m][n], 32 x 32 tiles, float reads along n (coalesced).
@@ -272,8 +226,8 @@ reduce_partials_kernel(const float* __restrict__ partial, int splits, int M, int
 
 }  // namespace
 
-// test hook: descriptor geometry can be overridden (tools/umma_probe) to pin the
-// MN-major LBO/SBO convention on hardware.
+// test hook: descriptor geometry can be overridden to pin the MN-major LBO/SBO convention on
+// hardware.
 static int g_gram_lbo = kBlockBytes;
 static int g_gram_sbo = 1024;
 void gram_tc_set_desc(int lbo, int sbo) { g_gram_lbo = lbo; g_gram_sbo = sbo; }

@@ -172,7 +172,7 @@ __global__ void prep_weights_kernel(const float* __restrict__ w, int Cout, int C
     if (!transpose_io) {
       dst = (static_cast<size_t>(o) * 9 + tap) * Cin + i;
     } else if (transpose_io == 2) {     // [Cout/16][half][tap][8][Cin]: the fused up-conv's N = 144
-      // tiles; an epilogue warp reads the 72 columns of its channel half with two wide TMEM loads
+      // tiles; the 72 columns of a channel half are contiguous in the accumulator
       dst = (((static_cast<size_t>(o >> 4) * 2 + ((o >> 3) & 1)) * 9 + tap) * 8 + (o & 7)) * Cin + i;
     } else {
       const int tp = flip_taps ? 8 - tap : tap;
@@ -1166,7 +1166,7 @@ nearest_up2_kernel(const float* __restrict__ x, long long n_in, int H, int W,
   *reinterpret_cast<float2*>(d + 2 * W) = make_float2(v, v);
 }
 
-inline int grid_for(long long n, int threads, int cap = 148 * 16) {
+inline int grid_for(long long n, int threads, int cap = 132 * 16) {
   long long g = (n + threads - 1) / threads;
   if (g > cap) g = cap;
   if (g < 1) g = 1;

@@ -13,37 +13,32 @@
 //     P_uv[p, o] = sum_i k[p, i] * (scale*W)[o, i, u, v]
 // (no shifted operands at all: one A tile serves all nine taps).  The conv_transpose output is
 //     t[2y+u, 2x+v] += P_uv[(y, x)]
-// so a GEMM tile is M = 128 input pixels x N = 144 = 9 taps x 16 output channels, K = Cin:
-// tcgen05.mma M128 N144 K16 runs at 76.7 cycles (94 % of the 128*N/256 floor; N = 128 tiles
-// reach 85 %, profiles/r2_mma_rate.txt), and every accumulation chain is only Cin/16 * 3 long
-// (the 3-term bf16 split), so no chunk promotion is needed against the tensor core's truncating
-// fp32 accumulate (see conv_tc.cu).
+// so a GEMM tile is M = 128 input pixels x N = 144 = 9 taps x 16 output channels, K = Cin, issued
+// as wgmma m64n144k16 by two warpgroups (64 rows each).  Every accumulation chain is only
+// Cin/16 * 3 long (the 3-term bf16 split), so no chunk promotion is needed against the tensor
+// core's truncating fp32 accumulate (see conv_tc.cu).
 //
 // A tile is ONE image row per image: 128 / W images of width W <= 128 (a power of two).  A CTA
 // marches down the rows of its images; the 4x4 FIR needs t rows 2y-3 .. 2y+1 to emit output rows
 // 2y-2, 2y-1 after step y, all of which depend on P at rows <= y of the SAME pixel (vertical
 // direction) and of the two neighbouring pixels (horizontal direction).
 //
-// Epilogue data mapping (round 2, second version).  The tile's rows are PERMUTED inside every
-// 32-pixel quarter — tile row 8 j + g holds pixel 4 g + j — which costs nothing: the tensor map
-// lists the key planes' dimensions in the order (channel, x/4 % 8, x % 4, x/32, row) and TMA fills
-// shared memory in that order.  tcgen05.ld.16x256b then hands thread (g = lane / 4, c = lane % 4)
-// the FOUR ADJACENT pixels 4g .. 4g+3 and two output channels: three of every four horizontal
-// neighbours are in the thread's own registers, the fourth comes from lane +-4 (16 shuffles per
-// step instead of 64) or, at a quarter boundary, from a 4 KB shared-memory mailbox.  Vertical state
-// (three horizontally filtered rows + the u = 2 taps of the previous row) stays in registers;
-// nothing is recomputed except two warm-up rows per row band.  Output: bf16 hi/lo words staged
-// with stmatrix ([image][X % 8][X / 8][16 channels], 32-byte swizzle: conflict-free) and written by
-// 5-d TMA stores — as LSU stores the 32-byte pieces of 64 pixels hit 64 different lines per
-// instruction and cost a third of the step.  Measured at layer 13, batch 32 (tools/prof_upconv.py,
-// profiles/): 1 258 us (one pixel x 8 channels per thread, 16-byte stores) -> 1 074 us (partner
-// exchange, 32-byte stores) -> 830 us (this mapping) -> 794-817 us (packed FFMA2 arithmetic).
+// Epilogue data mapping.  The tile's rows are PERMUTED inside every 32-pixel quarter — tile row
+// 8 j + g holds pixel 4 g + j — which costs nothing: the tensor map lists the key planes'
+// dimensions in the order (channel, x/4 % 8, x % 4, x/32, row) and TMA fills shared memory in that
+// order.  A wgmma accumulator gives lane (g = lane / 4, c = lane % 4) rows g and g + 8 of its
+// warp's 16, so the two warps of a quarter together hold, per lane, the FOUR ADJACENT pixels
+// 4g .. 4g+3; they trade channel halves through shared memory, after which each thread owns four
+// pixels and two output channels: three of every four horizontal neighbours are in the thread's
+// own registers, the fourth comes from lane +-4 or, at a quarter boundary, from a shared-memory
+// mailbox.  Vertical state (three horizontally filtered rows + the u = 2 taps of the previous row)
+// stays in registers; nothing is recomputed except two warm-up rows per row band.  Output: bf16
+// hi/lo words staged with stmatrix ([image][X % 8][X / 8][16 channels], 32-byte swizzle:
+// conflict-free) and written by 5-d TMA stores (as LSU stores the 32-byte pieces of 64 pixels hit
+// 64 different lines per instruction).
 //
-// Warp roles (384 threads = 3 warpgroups): warps 0..7 = epilogue — lane quarter q = warp % 4
-// (hardware restriction of tcgen05.ld), channel half h = warp / 4 (8 of the tile's 16 output
-// channels); warp 8 = TMA producer, warp 9 = MMA issuer (+TMEM alloc), warps 10-11 idle.  The
-// third warpgroup gives its registers back (setmaxnreg.dec 40) so that the epilogue warps can
-// hold their ~200 live values without spilling (setmaxnreg.inc 232).
+// Warp roles (288 threads): warps 0..7 = wgmma + epilogue — lane quarter q = warp / 2, channel
+// half h = warp % 2 (8 of the tile's 16 output channels); warp 8 = TMA producer.
 #include <cstring>
 
 #include "rw_common.cuh"
@@ -58,25 +53,25 @@ constexpr int UNC = 16;                 // output channels per tile
 constexpr int UN = 9 * UNC;             // GEMM N = 144
 constexpr int UBK = 64;
 constexpr int UK = 16;
-constexpr int kUStages = 3;
-constexpr int kUThreads = 384;
-constexpr int kUTmaWarp = 8, kUMmaWarp = 9;
+constexpr int kUStages = 2;
+constexpr int kUThreads = 288;       // warps 0-7: wgmma + epilogue, warp 8: TMA
+constexpr int kUTmaWarp = 8;
 constexpr int kUABytes = UM * UBK * 2;  // one plane of A: 16 KB
 constexpr int kUBBytes = UN * UBK * 2;  // one plane of B: 18 KB
 constexpr int kUStageBytes = 2 * kUABytes + 2 * kUBBytes;    // 68 KB
-constexpr int kUAccStride = 256;        // TMEM columns between the two accumulators
 constexpr int kUMailFloats = 2 * 2 * 4 * 2 * 32;             // [buf][half][quarter][side][32]
 constexpr int kUOutSlotBytes = 64 * 32;                      // 64 output pixels x 16 channels, one plane
 constexpr int kUOutQuarterBytes = 2 * kUOutSlotBytes;        // hi + lo slot of a lane quarter
 constexpr int kUOutStageBytes = 4 * kUOutQuarterBytes;       // 16 KB
-constexpr int kUSmemTotal = kUStages * kUStageBytes + kUMailFloats * 4 + kUOutStageBytes + 1024 + 256;
+// accumulator exchange between the two warps of a lane quarter: [warp][tap][row half][lane] float2
+constexpr int kUXchgFloat2 = 9 * 2 * 32;
+constexpr int kUXchgBytes = 8 * kUXchgFloat2 * 8;
+constexpr int kUSmemTotal =
+    kUStages * kUStageBytes + kUMailFloats * 4 + kUOutStageBytes + kUXchgBytes + 1024 + 256;
 
 struct UBarriers {
   uint64_t full[kUStages];
   uint64_t empty[kUStages];
-  uint64_t tmem_full[2];
-  uint64_t tmem_empty[2];
-  uint32_t tmem_base;
 };
 
 __device__ __forceinline__ void tma_load_5d(void* smem_dst, const CUtensorMap* m, uint64_t* bar,
@@ -90,13 +85,15 @@ __device__ __forceinline__ void tma_load_5d(void* smem_dst, const CUtensorMap* m
       : "memory");
 }
 
-template <int N>
-__device__ __forceinline__ void reg_alloc() {
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(N));
+// channel-pair arithmetic, one rounding per operation (the same results as the scalar operations)
+__device__ __forceinline__ float2 f2add(float2 a, float2 b) {
+  return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y));
 }
-template <int N>
-__device__ __forceinline__ void reg_dealloc() {
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(N));
+__device__ __forceinline__ float2 f2mul(float2 a, float2 b) {
+  return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y));
+}
+__device__ __forceinline__ float2 f2fma(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
 // producer-side wait: back off between polls so the spin does not take issue slots from the
 // epilogue warps that share the scheduler
@@ -120,19 +117,6 @@ __device__ __forceinline__ void lds_v4(uint32_t a, float& x, float& y, float& z,
                : "memory");
 }
 
-// waits of the two control warps: back off between polls — they share their schedulers with
-// epilogue warps, and ncu showed ~16 % of the kernel's issued instructions in their spin loops
-__device__ __forceinline__ void mbar_wait_relaxed(uint64_t* bar, uint32_t parity, uint32_t ns) {
-  uint32_t spins = 0;
-  while (!mbar_try_wait(bar, parity)) {
-    __nanosleep(ns);
-    if (++spins > RW_SPIN_LIMIT) __trap();
-  }
-}
-
-__device__ __forceinline__ void named_bar_sync(int id, int count) {
-  asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(count) : "memory");
-}
 // named barriers: 1, 2 = mailbox of a channel half; 3 + q = the two warps of lane quarter q
 constexpr int kBarPair = 3;
 template <int N>
@@ -158,33 +142,6 @@ __device__ __forceinline__ UpItem decode_item(int item, const UpFusedParams& p) 
   it.y_first = ya - 2 < 0 ? 0 : ya - 2;
   it.y_end = yb;
   return it;
-}
-
-// tcgen05.ld.16x256b.x1: 16 TMEM lanes x 8 fp32 columns; thread t receives lane t/4, columns
-// 2(t%4), 2(t%4)+1 in r[0], r[1] and lane t/4 + 8, same columns, in r[2], r[3]
-// (tools/probe/probe_sm100.cu prints the distribution on the device); .x8 repeats that for eight
-// consecutive groups of 8 columns, 4 registers each
-__device__ __forceinline__ void tmem_ld_16x256(uint32_t taddr, float* v) {
-  uint32_t r[4];
-  asm volatile("tcgen05.ld.sync.aligned.16x256b.x1.b32 {%0, %1, %2, %3}, [%4];\n"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-               : "r"(taddr)
-               : "memory");
-#pragma unroll
-  for (int i = 0; i < 4; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld_16x256_x8(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.16x256b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, "
-      "%13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
-      "[%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]),
-        "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]),
-        "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]),
-        "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
 }
 
 // four 8x8 b16 matrices: register i of lane t is row t/4, 32-bit column t%4 of matrix i; lane t
@@ -225,7 +182,8 @@ upconv_fused_kernel(const __grid_constant__ CUtensorMap map_a_hi,
                                              ~static_cast<uintptr_t>(1023));
   float* mail = reinterpret_cast<float*>(smem + kUStages * kUStageBytes);
   uint8_t* out_stage = smem + kUStages * kUStageBytes + kUMailFloats * 4;
-  UBarriers* bars = reinterpret_cast<UBarriers*>(out_stage + kUOutStageBytes);
+  float2* xchg = reinterpret_cast<float2*>(out_stage + kUOutStageBytes);
+  UBarriers* bars = reinterpret_cast<UBarriers*>(out_stage + kUOutStageBytes + kUXchgBytes);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -241,27 +199,17 @@ upconv_fused_kernel(const __grid_constant__ CUtensorMap map_a_hi,
     tma_prefetch_desc(&map_o_lo);
     for (int s = 0; s < kUStages; ++s) {
       mbar_init(&bars->full[s], 1);
-      mbar_init(&bars->empty[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&bars->tmem_full[s], 1);
-      mbar_init(&bars->tmem_empty[s], 8);
+      mbar_init(&bars->empty[s], 2);      // one arrival per consumer warpgroup
     }
     fence_mbar_init();
   }
-  if (warp == kUMmaWarp) tmem_alloc<512>(&bars->tmem_base);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = bars->tmem_base;
 
-  if (warp >= 8) {
-    reg_dealloc<40>();
   if (warp == kUTmaWarp) {
     // ------------------------------ TMA producer ------------------------------
     // The A tile's rows are PERMUTED: inside every 32-pixel quarter, tile row 8 j + g holds pixel
-    // 4 g + j (j < 4, g < 8), so that tcgen05.ld.16x256b hands an epilogue thread four ADJACENT
-    // pixels.  The permutation is free: the tensor map lists the key planes' dimensions as
+    // 4 g + j (j < 4, g < 8), so that the wgmma accumulator rows of a warp pair hold, per thread,
+    // four ADJACENT pixels.  The permutation is free: the tensor map lists the key planes' dimensions as
     // (channel, x / 4 % 8, x % 4, x / 32, row) — TMA fills shared memory in that order — so one
     // load still brings a whole image row (W >= 32; W < 32: (channel, x / 4, image, x % 4, y), one
     // load per quarter).  [Loading the eight rows of each (quarter, j) separately — 32 one-KB
@@ -300,53 +248,19 @@ upconv_fused_kernel(const __grid_constant__ CUtensorMap map_a_hi,
         }
       }
     }
-  } else if (warp == kUMmaWarp) {
-    // ------------------------------ MMA issuer --------------------------------
-    constexpr uint32_t idesc = make_idesc_bf16(UM, UN, 0, 0);
-    int stage = 0;
-    uint32_t phase = 0;
-    uint32_t step = 0;
-    for (int item = blockIdx.x; item < p.nitems; item += gridDim.x) {
-      const UpItem it = decode_item(item, p);
-      for (int y = it.y_first; y < it.y_end; ++y, ++step) {
-        const int as = step & 1u;
-        const uint32_t aphase = (step >> 1) & 1u;
-        mbar_wait_relaxed(&bars->tmem_empty[as], aphase ^ 1u, 32);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + as * kUAccStride;
-        for (int kb = 0; kb < kb_count; ++kb) {
-          mbar_wait(&bars->full[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * kUStageBytes);
-          const uint64_t da_hi = make_smem_desc(sa, 16, 1024, kSwizzle128B);
-          const uint64_t da_lo = make_smem_desc(sa + kUABytes, 16, 1024, kSwizzle128B);
-          const uint64_t db_hi = make_smem_desc(sa + 2 * kUABytes, 16, 1024, kSwizzle128B);
-          const uint64_t db_lo = make_smem_desc(sa + 2 * kUABytes + kUBBytes, 16, 1024, kSwizzle128B);
-          if (elect_one()) {
-#pragma unroll
-            for (int kk = 0; kk < UBK / UK; ++kk) {
-              const uint64_t adv = static_cast<uint64_t>((kk * UK * 2) >> 4);
-              umma_bf16(tmem_d, da_lo + adv, db_hi + adv, idesc, (kb | kk) != 0);
-              umma_bf16(tmem_d, da_hi + adv, db_lo + adv, idesc, 1u);
-              umma_bf16(tmem_d, da_hi + adv, db_hi + adv, idesc, 1u);
-            }
-            umma_commit(&bars->empty[stage]);
-            if (kb + 1 == kb_count) umma_commit(&bars->tmem_full[as]);
-          }
-          __syncwarp();
-          if (++stage == kUStages) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
-  }
   } else {
-    // ------------------------------ epilogue ----------------------------------
-    // thread (g = lane / 4, c = lane % 4) of warp (q, h) owns the four adjacent pixels
+    // ------------------------------ MMA + epilogue ----------------------------
+    // warp w (0..7) issues, with its warpgroup, the wgmma rows 16 w .. 16 w + 15 of the tile = the
+    // pixels j = 2 (w % 2) + i (i = 0, 1) of lane quarter q = w / 2, for all 144 columns; it keeps
+    // channel half h = w % 2 and trades the other half with warp w ^ 1 through shared memory.
+    // Then thread (g = lane / 4, c = lane % 4) of warp (q, h) owns the four adjacent pixels
     // 32 q + 4 g + j of the tile and the two output channels 8 h + 2 c + e of the item's sixteen:
     // "unit" u = 2 j + e indexes its eight (pixel, channel) pairs.
-    reg_alloc<232>();
-    const int q = warp & 3;
-    const int h = warp >> 2;
+    const int wg = warp >> 2;
+    const int q = warp >> 1;
+    const int h = warp & 1;
+    int stage = 0;
+    uint32_t phase = 0;
     const int g = lane >> 2, c = lane & 3;
     const int W = p.W;
     const int T0 = q * 32 + 4 * g;             // tile index of the first of the four pixels
@@ -437,36 +351,53 @@ upconv_fused_kernel(const __grid_constant__ CUtensorMap map_a_hi,
         }
         long long tq[8];
         if constexpr (PROF) tq[0] = clock64();
-        const int as = step & 1u;
-        const uint32_t aphase = (step >> 1) & 1u;
-        mbar_wait(&bars->tmem_full[as], aphase);
-        tc_fence_after();
-        if constexpr (PROF) tq[1] = clock64();
-        // accumulator columns: [channel half][tap][8 channels] (prep_weights, transpose_io = 2)
-        const uint32_t tcol = tmem_base + static_cast<uint32_t>(as * kUAccStride + h * 72) +
-                              (static_cast<uint32_t>(q * 32) << 16);
         float2 P[9][4];                                              // [tap][pixel j] (e0, e1)
         {
-          uint32_t ra[32], rb[32];
-          float p8[8];
-          tmem_ld_16x256_x8(tcol, ra);                               // taps 0-7, pixels j = 0, 1
-          tmem_ld_16x256_x8(tcol + (16u << 16), rb);                 // taps 0-7, pixels j = 2, 3
-          tmem_ld_16x256(tcol + 64, &p8[0]);
-          tmem_ld_16x256(tcol + 64 + (16u << 16), &p8[4]);
-          tmem_ld_wait();
+          float d[72];
+          for (int kb = 0; kb < kb_count; ++kb) {
+            mbar_wait(&bars->full[stage], phase);
+            const uint32_t sa = smem_u32(smem + stage * kUStageBytes);
+            const uint64_t da_hi = make_smem_desc(sa + wg * (kUABytes / 2), 16, 1024);
+            const uint64_t da_lo = make_smem_desc(sa + kUABytes + wg * (kUABytes / 2), 16, 1024);
+            const uint64_t db_hi = make_smem_desc(sa + 2 * kUABytes, 16, 1024);
+            const uint64_t db_lo = make_smem_desc(sa + 2 * kUABytes + kUBBytes, 16, 1024);
+            wgmma_fence();
 #pragma unroll
-          for (int t = 0; t < 8; ++t) {
-            P[t][0] = make_float2(__uint_as_float(ra[4 * t]), __uint_as_float(ra[4 * t + 1]));
-            P[t][1] = make_float2(__uint_as_float(ra[4 * t + 2]), __uint_as_float(ra[4 * t + 3]));
-            P[t][2] = make_float2(__uint_as_float(rb[4 * t]), __uint_as_float(rb[4 * t + 1]));
-            P[t][3] = make_float2(__uint_as_float(rb[4 * t + 2]), __uint_as_float(rb[4 * t + 3]));
+            for (int kk = 0; kk < UBK / UK; ++kk) {
+              const uint64_t adv = static_cast<uint64_t>((kk * UK * 2) >> 4);
+              wgmma_m64n144<0, 0>(d, da_lo + adv, db_hi + adv, (kb | kk) != 0);
+              wgmma_m64n144<0, 0>(d, da_hi + adv, db_lo + adv, 1u);
+              wgmma_m64n144<0, 0>(d, da_hi + adv, db_hi + adv, 1u);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            if ((threadIdx.x & 127) == 0) mbar_arrive(&bars->empty[stage]);
+            if (++stage == kUStages) { stage = 0; phase ^= 1u; }
           }
+          if constexpr (PROF) tq[1] = clock64();
+          // accumulator columns: [channel half][tap][8 channels] (prep_weights, transpose_io = 2);
+          // every register index is a compile-time constant (a run-time one puts d in local memory)
+          float2* to = xchg + (warp ^ 1) * kUXchgFloat2 + lane;
 #pragma unroll
-          for (int j = 0; j < 4; ++j) P[8][j] = make_float2(p8[2 * j], p8[2 * j + 1]);
+          for (int t = 0; t < 9; ++t)
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+              to[(t * 2 + i) * 32] = h ? make_float2(d[4 * t + 2 * i], d[4 * t + 2 * i + 1])
+                                       : make_float2(d[4 * (9 + t) + 2 * i], d[4 * (9 + t) + 2 * i + 1]);
+          named_bar_sync(kBarPair + q, 64);
+          const float2* from = xchg + warp * kUXchgFloat2 + lane;
+#pragma unroll
+          for (int t = 0; t < 9; ++t)
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+              const float2 own = h ? make_float2(d[4 * (9 + t) + 2 * i], d[4 * (9 + t) + 2 * i + 1])
+                                   : make_float2(d[4 * t + 2 * i], d[4 * t + 2 * i + 1]);
+              const float2 other = from[(t * 2 + i) * 32];
+              P[t][i] = h ? other : own;               // pixels j = 0, 1 come from the h = 0 warp
+              P[t][2 + i] = h ? own : other;           // pixels j = 2, 3 from the h = 1 warp
+            }
+          named_bar_sync(kBarPair + q, 64);          // the slot is free for the next step
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bars->tmem_empty[as]);
         if constexpr (PROF) tq[2] = clock64();
         if (p.debug_p != nullptr && img_ok && y < p.H && y >= it.y_emit - 1) {
 #pragma unroll
@@ -482,9 +413,9 @@ upconv_fused_kernel(const __grid_constant__ CUtensorMap map_a_hi,
         float2 le[2][4], ro[2][4], od[2][4];
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-          le[0][j] = __fadd2_rn(P[0][j], c20[j]);
-          od[0][j] = __fadd2_rn(P[1][j], c21[j]);
-          ro[0][j] = __fadd2_rn(P[2][j], c22[j]);
+          le[0][j] = f2add(P[0][j], c20[j]);
+          od[0][j] = f2add(P[1][j], c21[j]);
+          ro[0][j] = f2add(P[2][j], c22[j]);
           le[1][j] = P[3][j];
           od[1][j] = P[4][j];
           ro[1][j] = P[5][j];
@@ -527,11 +458,11 @@ upconv_fused_kernel(const __grid_constant__ CUtensorMap map_a_hi,
                      kh2 = make_float2(kh[2], kh[2]), kh3 = make_float2(kh[3], kh[3]);
         float2 hf[2][2][4];                      // [t row E/O][output column 2x / 2x+1][pixel j]
         auto hfir = [&](int r, int j, float2 l_ro, float2 l_od, float2 r_le, float2 r_od) {
-          const float2 e0 = __fadd2_rn(le[r][j], l_ro);    // t col 2x
-          const float2 e1 = __fadd2_rn(r_le, ro[r][j]);    // t col 2x+2
+          const float2 e0 = f2add(le[r][j], l_ro);    // t col 2x
+          const float2 e1 = f2add(r_le, ro[r][j]);    // t col 2x+2
           const float2 o0 = od[r][j];                      // t col 2x+1
-          hf[r][0][j] = __ffma2_rn(kh3, e1, __ffma2_rn(kh2, o0, __ffma2_rn(kh1, e0, __fmul2_rn(kh0, l_od))));
-          hf[r][1][j] = __ffma2_rn(kh3, r_od, __ffma2_rn(kh2, e1, __ffma2_rn(kh1, o0, __fmul2_rn(kh0, e0))));
+          hf[r][0][j] = f2fma(kh3, e1, f2fma(kh2, o0, f2fma(kh1, e0, f2mul(kh0, l_od))));
+          hf[r][1][j] = f2fma(kh3, r_od, f2fma(kh2, e1, f2fma(kh1, o0, f2mul(kh0, e0))));
         };
 #pragma unroll
         for (int r = 0; r < 2; ++r) {
@@ -587,21 +518,21 @@ upconv_fused_kernel(const __grid_constant__ CUtensorMap map_a_hi,
                 const float nzv = nw * nz[2 * j + xi];
                 float2 v;
                 if (yi == 0)
-                  v = __ffma2_rn(kv3, hf[0][xi][j],
-                                 __ffma2_rn(kv2, w2[xi][j], __ffma2_rn(kv1, w1[xi][j], __fmul2_rn(kv0, w0[xi][j]))));
+                  v = f2fma(kv3, hf[0][xi][j],
+                                 f2fma(kv2, w2[xi][j], f2fma(kv1, w1[xi][j], f2mul(kv0, w0[xi][j]))));
                 else
-                  v = __ffma2_rn(kv3, hf[1][xi][j],
-                                 __ffma2_rn(kv2, hf[0][xi][j], __ffma2_rn(kv1, w2[xi][j], __fmul2_rn(kv0, w1[xi][j]))));
-                v = __fadd2_rn(__ffma2_rn(v, dm, make_float2(nzv, nzv)), bs);
+                  v = f2fma(kv3, hf[1][xi][j],
+                                 f2fma(kv2, hf[0][xi][j], f2fma(kv1, w2[xi][j], f2mul(kv0, w1[xi][j]))));
+                v = f2add(f2fma(v, dm, make_float2(nzv, nzv)), bs);
                 if (!NCHW || p.act) {
-                  const float2 t02 = __fmul2_rn(v, make_float2(0.2f, 0.2f));
-                  v = __fmul2_rn(make_float2(fmaxf(v.x, t02.x), fmaxf(v.y, t02.y)),
+                  const float2 t02 = f2mul(v, make_float2(0.2f, 0.2f));
+                  v = f2mul(make_float2(fmaxf(v.x, t02.x), fmaxf(v.y, t02.y)),
                                  make_float2(1.4142135623730951f, 1.4142135623730951f));
                 }
                 if constexpr (NCHW) {
                   yv[xi][j] = v;
                 } else {
-                  const float2 kk = __fmul2_rn(ns, v);
+                  const float2 kk = f2mul(ns, v);
                   const __nv_bfloat162 hh = __floats2bfloat162_rn(kk.x, kk.y);
                   const uint32_t hu = *reinterpret_cast<const uint32_t*>(&hh);
                   const __nv_bfloat162 ll = __floats2bfloat162_rn(
@@ -703,12 +634,6 @@ upconv_fused_kernel(const __grid_constant__ CUtensorMap map_a_hi,
     }
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == kUMmaWarp) {
-    tc_fence_after();
-    tmem_dealloc<512>(tmem_base);
-  }
 }
 
 }  // namespace

@@ -353,7 +353,7 @@ LRELU_GAIN = 2 ** 0.5
 class StyledConvFunction(torch.autograd.Function):
     """y = [act]([blur](conv(style*x, scale*W) * demod) + nw*noise + bias)
 
-    One fused forward (prep -> tcgen05 row-GEMM with fused epilogue); backward =
+    One fused forward (prep -> wgmma row-GEMM with fused epilogue); backward =
     dgrad row-GEMM on gradient planes + wgrad col-GEMM + small reductions.
     """
 

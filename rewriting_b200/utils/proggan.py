@@ -6,7 +6,7 @@ and `nethook.subsequence` address `layerN.conv` exactly as in the reference.
 Where the arithmetic runs (CUDA tensors; there is no CPU fallback for the forward):
   * PixelNormLayer / DoubleResolutionLayer — `rw_pixel_norm_nchw` / `rw_nearest_up2`;
   * every 3x3 conv with Cin % 64 == 0 and Cout % 128 == 0 (all 512/256/128-channel layers, in
-    particular every layer a rewriter targets) — the tcgen05 row-GEMM over bf16 hi/lo key planes
+    particular every layer a rewriter targets) — the wgmma row-GEMM over bf16 hi/lo key planes
     (`ops.plain_conv`, with autograd for the rewriter's fallback path); an intact, unhooked
     NormConvBlock runs as pixel-norm(+2x) -> planes -> ONE conv launch whose epilogue applies the
     WScale bias and the leaky-ReLU (the WScale factor is folded into the weight planes);

@@ -301,7 +301,7 @@ def _blur_pads(blur_kernel, kernel_size, factor=2):
 class DemodulatedConv2dF(nn.Module):
     """conv(k, scale*W) * demod(W, style) on an already-modulated key k = d.fmap.
     This leaf is the rewriter's linear associative memory; its `weight` is the edited
-    tensor.  Runs the tcgen05 row-GEMM with a demod-only epilogue; differentiable in
+    tensor.  Runs the wgmma row-GEMM with a demod-only epilogue; differentiable in
     k, style and weight."""
 
     def __init__(self, in_channel, out_channel, kernel_size, demodulate=True, upsample=False):

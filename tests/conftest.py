@@ -13,9 +13,9 @@ GOLD = os.path.join(ROOT, 'tests', 'golden')
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (an H100)')
     # a fresh checkout has no librw_b200.so yet (built artefacts are git-ignored): build it once
-    # (nvcc cross-compiles sm_100a without a GPU); an existing library is left alone
+    # (nvcc cross-compiles sm_90a without a GPU); an existing library is left alone
     from rewriting_b200 import build as rw_build
     if not os.path.exists(rw_build.LIB):
         rw_build.build(force=True)

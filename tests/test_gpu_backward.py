@@ -1,4 +1,4 @@
-"""GPU (B200): the StyledConv backward (csrc/bwd.cu + dgrad / wgrad tensor-core GEMMs) against
+"""GPU (H100): the StyledConv backward (csrc/bwd.cu + dgrad / wgrad tensor-core GEMMs) against
 torch autograd of the CPU oracle, plus kernel-level checks of every fused backward pass.
 
 Tolerance: gradients within 3e-4 of the gradient's max magnitude (3-term split bf16 operands,

@@ -1,4 +1,4 @@
-"""GPU (B200): BASELINE config 4 on its own fixture and horizon —
+"""GPU (H100): BASELINE config 4 on its own fixture and horizon —
 notebooks/masks/stylegan/horse/hat_on_horse_ears.json, 1000 z, layer 8, rank 1, 4 context keys,
 2001 iterations (reference: ganrewrite.py:135-169, 254-298, 333-374) — against the goldens the
 live reference produced (oracle/make_golden_config4.py) and the fp64-anchored protocol of

@@ -1,4 +1,4 @@
-"""GPU (B200): the small kernels of the generation fast path against plain torch fp32
+"""GPU (H100): the small kernels of the generation fast path against plain torch fp32
 (mapping network layers, batched demodulation / ToRGB weights, ToRGB combine, pipelined blur)."""
 import ctypes
 import math
@@ -229,8 +229,8 @@ def test_modconv_up_fused_layer_level_vs_oracle(B, H, demod, noise, act):
 
 @pytest.mark.parametrize('B,Cin,Cout,H', [(5, 64, 256, 64), (3, 128, 512, 96)])
 def test_fused_conv_cta_pair_large_shapes_vs_oracle(B, Cin, Cout, H):
-    """rw_modconv_fwd_fused on shapes with more than a wave of 256-row tiles (CTA pairs,
-    `cta_group::2`, several 128-column N tiles): fp32 output, next-layer planes and ToRGB partials against
+    """rw_modconv_fwd_fused on shapes with several waves of persistent 128-row tiles and several
+    128-column N tiles: fp32 output, next-layer planes and ToRGB partials against
     the oracle's DemodulatedConv2dF -> NoiseInjectionF -> FusedLeakyReLUF (models.py:313-329,
     535-546) and ToRGB sum (models.py:639-655)."""
     from rewriting_b200 import _cabi, ops

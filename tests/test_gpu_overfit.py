@@ -1,4 +1,4 @@
-"""GPU (B200): the all-weights baseline `apply_overfit` -> `all_weights_insert` (reference
+"""GPU (H100): the all-weights baseline `apply_overfit` -> `all_weights_insert` (reference
 rewrite/ganrewrite.py:171-181, 300-331) against what the UNMODIFIED live reference produced for the
 same request, weights, z and (seeded stand-in) VGG-16 — tests/golden/overfit3.npz, written by
 oracle/make_golden_overfit.py.  Every generator parameter is updated by Adam through this package's
@@ -42,9 +42,7 @@ def test_apply_overfit_vs_live_reference_golden(seeded_model, z40, edit_request)
     losses, grad0, upd = _run(seeded_model, z40, edit_request, niter, lr)
     names = [str(n) for n in g['names']]
     assert sorted(upd) == names                          # same parameter set, all of it trained
-    # Measured on the B200 (tools/debug_overfit.py): losses 1.4e-5 / 6.7e-5 / 3.9e-5 relative,
-    # gradient norms 8.6e-6 median, 1.8e-3 worst (a scalar noise strength: a cancelling sum over
-    # a million pixels), gradients 8e-6 .. 1.3e-4 rel-Frobenius, updates < 6e-4 element-wise.
+    # The worst gradient norm is a scalar noise strength: a cancelling sum over a million pixels.
     # (1) the losses: forward pass + pasted target + VGG features, then two Adam steps over all
     # parameters (8.1 -> 112.8 -> 28.3: the reference's lr = 0.01 is violent on this generator; the
     # reference itself moves its third loss by 9e-5 when its parameters are perturbed by 1e-6,

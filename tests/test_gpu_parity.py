@@ -1,4 +1,4 @@
-"""GPU (B200): the CUDA path against the CPU oracle and the committed golden vectors.
+"""GPU (H100): the CUDA path against the CPU oracle and the committed golden vectors.
 
 Tolerances (BASELINE.json north_star): pixels within 1e-3 fp32 on identical z/seed, edited W
 within 1e-4 (over <= 50 iterations, SURVEY.md §7), C rel-Frobenius <= 1e-5, d max-abs <= 1e-4.

@@ -1,4 +1,4 @@
-"""GPU (B200): parity cases round 1 left open (VERDICT r1, "close the parity holes") — the
+"""GPU (H100): parity cases beyond tests/test_gpu_parity.py — the
 `mconv='fast'` / `None` generator forms, an odd (upsampling) target layer, the
 SeqPreStyleGanRewriter split, `apply_erase` against the live-reference goldens on the GPU, and
 the small fast-path kernels against the ORACLE directly (not against sibling kernels / GPU torch)."""

@@ -1,4 +1,4 @@
-"""GPU (B200): `ProgressiveGanRewriter` on a ProgGAN generator (SURVEY.md §8 f-3; reference
+"""GPU (H100): `ProgressiveGanRewriter` on a ProgGAN generator (SURVEY.md §8 f-3; reference
 utils/proggan.py:63-199, rewrite/ganrewrite.py:25-96, 254-298) — the generator's 3x3 convs on the
 tensor-core row-GEMM, the key second moment on the col-GEMM, the rank-one edit of a plain
 `layerN.conv` in the fused insert kernel — against goldens from the live reference and the

@@ -220,33 +220,33 @@ def test_shard_range_partitions_exactly():
             assert max(sizes) - min(sizes) <= 1 and sum(sizes) == n
 
 
-@pytest.mark.skipif(not os.path.isdir('/root/reference/rewrite'),
-                    reason='needs a checkout of the reference (authoring container only)')
-def test_install_aliases_serves_the_reference_ui_over_this_rewriter():
+def test_install_aliases_serves_the_reference_ui_over_this_rewriter(tmp_path):
     """`from rewrite import ganrewrite, rewriteapp` in a notebook: this package's rewriter and
-    overlay renderer, the reference's device-independent GanRewriteApp / widgets."""
+    overlay renderer, the UI modules (rewriteapp, labwidget) from the given checkout of the
+    reference (here a stand-in tree holding only those two modules)."""
     import subprocess
     import sys
+    ref = tmp_path / 'reference'
+    (ref / 'rewrite').mkdir(parents=True)
+    (ref / 'utils').mkdir()
+    (ref / 'rewrite' / 'rewriteapp.py').write_text('class GanRewriteApp(object):\n    pass\n')
+    (ref / 'utils' / 'labwidget.py').write_text('class Widget(object):\n    pass\n')
+    # modules this package provides must NOT be taken from the checkout
+    (ref / 'rewrite' / 'ganrewrite.py').write_text('raise ImportError("shadowed")\n')
+    ref = str(ref)
     code = '''
-import sys, types
+import sys
 sys.path.insert(0, %r)
-if 'IPython' not in sys.modules:
-    try:
-        import IPython
-    except ImportError:
-        m = types.ModuleType('IPython'); d = types.ModuleType('IPython.display')
-        d.display = lambda *a, **k: None; m.display = d
-        sys.modules['IPython'] = m; sys.modules['IPython.display'] = d
 import rewriting_b200
-rewriting_b200.install_aliases('/root/reference')
+rewriting_b200.install_aliases(%r)
 from rewrite import ganrewrite, rewriteapp
 from utils import imgviz, labwidget, runningstats
 assert ganrewrite.__file__.startswith(%r), ganrewrite.__file__
 assert imgviz.__file__.startswith(%r) and runningstats.__file__.startswith(%r)
-assert rewriteapp.__file__.startswith('/root/reference') and labwidget.__file__.startswith('/root/reference')
+assert rewriteapp.__file__.startswith(%r) and labwidget.__file__.startswith(%r)
 assert hasattr(rewriteapp, 'GanRewriteApp') and hasattr(ganrewrite, 'SeqStyleGanRewriter')
 print('ok')
-''' % (ROOT, ROOT, ROOT, ROOT)
+''' % (ROOT, ref, ROOT, ROOT, ROOT, ref, ref)
     r = subprocess.run([sys.executable, '-W', 'ignore', '-c', code], capture_output=True, text=True,
                        timeout=300)
     assert r.returncode == 0 and r.stdout.strip().endswith('ok'), r.stderr[-2000:]

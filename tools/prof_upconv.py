@@ -1,5 +1,5 @@
 """Phase profile of the fused upsampling kernel (clock64 instrumented variant): cycles per step an
-epilogue warp spends waiting for the MMAs, draining TMEM, in combine + mailbox + barrier, in the
+epilogue warp spends waiting for the MMAs, in the accumulator exchange, in combine + mailbox + barrier, in the
 neighbour exchange + horizontal FIR, and in the vertical FIR + activation + stores.
 
     python tools/prof_upconv.py [B Cin Cout H]      (default: layer 13 at batch 32)"""
@@ -29,7 +29,7 @@ def main():
     kern = (torch.tensor([1., 3., 3., 1.])[:, None] * torch.tensor([1., 3., 3., 1.])[None, :] / 16).to(dev)
     nh = torch.empty((B * (Ho + 1) * (Ho + 1), Cout), dtype=torch.bfloat16, device=dev)
     nl = torch.empty_like(nh)
-    prof = torch.zeros(148, 8, 16, dtype=torch.int64, device=dev)
+    prof = torch.zeros(torch.cuda.get_device_properties(dev).multi_processor_count, 8, 16, dtype=torch.int64, device=dev)
     args = (ops._p(planes.hi), ops._p(planes.lo), ops._p(u_hi), ops._p(u_lo), ops._p(dm), ops._p(kern),
             ops._p(noise), noise.stride(0), ops._p(nw), ops._p(bias), ops._p(ns), ops._p(nh), ops._p(nl),
             B, Cin, Cout, H, H)
@@ -46,7 +46,7 @@ def main():
     torch.cuda.synchronize()
     p = prof.cpu().double()
     steps = p[:, :, 7].sum()
-    names = ['wait MMA', 'TMEM drain', 'combine+mailbox+barrier', 'shuffles', 'edge-lane fix-ups',
+    names = ['wait MMA', 'accumulator exchange', 'combine+mailbox+barrier', 'shuffles', 'edge-lane fix-ups',
              'horizontal FIR', 'vertical FIR+activation+stores']
     tot = p[:, :, :7].sum()
     print('steps per epilogue warp (avg) %.1f, cycles per step %.0f' % (steps / (p[:, :, 7] > 0).sum(), tot / steps))
