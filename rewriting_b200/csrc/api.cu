@@ -114,7 +114,7 @@ int make_tmap_4d_bf16(CUtensorMap* out, const void* base, const uint64_t dims[4]
 }
 
 // general form: rank <= 5, element strides (a stride s on dimension d loads every s-th element
-// of the box extent box[d]), swizzle 0 = none, 1 = 32 B, 2 = 128 B
+// of the box extent box[d]), swizzle 0 = none, 1 = 32 B, 2 = 128 B, 3 = 64 B
 int make_tmap_nd_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
                       const uint64_t* strides_bytes, const uint32_t* box, const uint32_t* estrides,
                       int swizzle) {
@@ -135,7 +135,8 @@ int make_tmap_nd_bf16(CUtensorMap* out, const void* base, int rank, const uint64
     es[i] = estrides ? estrides[i] : 1u;
     if (i + 1 < rank) gstr[i] = strides_bytes[i];
   }
-  const CUtensorMapSwizzle sw = swizzle == 2 ? CU_TENSOR_MAP_SWIZZLE_128B
+  const CUtensorMapSwizzle sw = swizzle == 2   ? CU_TENSOR_MAP_SWIZZLE_128B
+                                : swizzle == 3 ? CU_TENSOR_MAP_SWIZZLE_64B
                                 : swizzle == 1 ? CU_TENSOR_MAP_SWIZZLE_32B
                                                : CU_TENSOR_MAP_SWIZZLE_NONE;
   CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, static_cast<cuuint32_t>(rank),

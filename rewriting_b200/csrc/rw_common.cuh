@@ -90,6 +90,18 @@ __device__ __forceinline__ void named_bar_sync(int id, int count) {
 }
 
 // ---------------------------------------------------------------------------
+// per-warpgroup register reallocation (every thread of the warpgroup executes it)
+// ---------------------------------------------------------------------------
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(N));
+}
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(N));
+}
+
+// ---------------------------------------------------------------------------
 // TMA (tiled mode, 2-D), completes on an mbarrier
 // ---------------------------------------------------------------------------
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
@@ -164,17 +176,17 @@ __device__ __forceinline__ void wgmma_m64n144(float (&d)[72], uint64_t desc_a, u
 // descriptors
 // ---------------------------------------------------------------------------
 // Shared-memory matrix descriptor of wgmma (PTX ISA "Matrix Descriptor Format"), 128-byte swizzle:
-//  [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [49,52) base offset (0: 1024-byte aligned
-//  atoms) | [62,64) layout (1 = 128B swizzle).
-// K-major operand: rows of 128 B, SBO = 1024 (8-row group), LBO unused.
+//  [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [49,52) base offset (0: aligned swizzle
+//  atoms) | [62,64) layout (1 = 128B swizzle, 2 = 64B swizzle).
+// K-major operand: rows of 128 B (64 B), SBO = 1024 (512) per 8-row group, LBO unused.
 // MN-major operand: 64-element MN blocks LBO apart, 8-row K groups SBO apart.
 __host__ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes,
-                                                            uint32_t sbo_bytes) {
+                                                            uint32_t sbo_bytes, uint32_t layout = 1) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr >> 4) & 0x3FFFu);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 62;
+  d |= static_cast<uint64_t>(layout) << 62;
   return d;
 }
 

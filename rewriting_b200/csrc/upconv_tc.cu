@@ -37,8 +37,9 @@
 // conflict-free) and written by 5-d TMA stores (as LSU stores the 32-byte pieces of 64 pixels hit
 // 64 different lines per instruction).
 //
-// Warp roles (288 threads): warps 0..7 = wgmma + epilogue — lane quarter q = warp / 2, channel
-// half h = warp % 2 (8 of the tile's 16 output channels); warp 8 = TMA producer.
+// Warp roles (384 threads): warps 0..7 = wgmma + epilogue — lane quarter q = warp / 2, channel
+// half h = warp % 2 (8 of the tile's 16 output channels); warpgroup 2 = producer, which hands its
+// registers to the two consumer warpgroups (setmaxnreg) and whose warp 8 issues the TMA loads.
 #include <cstring>
 
 #include "rw_common.cuh"
@@ -51,14 +52,19 @@ namespace {
 constexpr int UM = 128;                 // input pixels per tile
 constexpr int UNC = 16;                 // output channels per tile
 constexpr int UN = 9 * UNC;             // GEMM N = 144
-constexpr int UBK = 64;
+// k-block of 32 channels = one 64-byte swizzle row: a 34 KB stage, so that five fit next to the
+// epilogue's buffers and the producer runs up to four k-blocks ahead of the MMAs
+constexpr int UBK = 32;
 constexpr int UK = 16;
-constexpr int kUStages = 2;
-constexpr int kUThreads = 288;       // warps 0-7: wgmma + epilogue, warp 8: TMA
+constexpr int kUStages = 5;
+constexpr int kUThreads = 384;       // warps 0-7: wgmma + epilogue, warpgroup 2: producer
 constexpr int kUTmaWarp = 8;
-constexpr int kUABytes = UM * UBK * 2;  // one plane of A: 16 KB
-constexpr int kUBBytes = UN * UBK * 2;  // one plane of B: 18 KB
-constexpr int kUStageBytes = 2 * kUABytes + 2 * kUBBytes;    // 68 KB
+// register split after setmaxnreg: 128 x 40 + 256 x 232 = 384 x 168, the launch allocation
+constexpr uint32_t kUProducerRegs = 40;
+constexpr uint32_t kUConsumerRegs = 232;
+constexpr int kUABytes = UM * UBK * 2;  // one plane of A: 8 KB
+constexpr int kUBBytes = UN * UBK * 2;  // one plane of B: 9 KB
+constexpr int kUStageBytes = 2 * kUABytes + 2 * kUBBytes;    // 34 KB
 constexpr int kUMailFloats = 2 * 2 * 4 * 2 * 32;             // [buf][half][quarter][side][32]
 constexpr int kUOutSlotBytes = 64 * 32;                      // 64 output pixels x 16 channels, one plane
 constexpr int kUOutQuarterBytes = 2 * kUOutSlotBytes;        // hi + lo slot of a lane quarter
@@ -67,7 +73,10 @@ constexpr int kUOutStageBytes = 4 * kUOutQuarterBytes;       // 16 KB
 constexpr int kUXchgFloat2 = 9 * 2 * 32;
 constexpr int kUXchgBytes = 8 * kUXchgFloat2 * 8;
 constexpr int kUSmemTotal =
-    kUStages * kUStageBytes + kUMailFloats * 4 + kUOutStageBytes + kUXchgBytes + 1024 + 256;
+    kUStages * kUStageBytes + kUMailFloats * 4 + kUOutStageBytes + kUXchgBytes + 512 + 256;
+// 512-byte alignment serves the 64-byte swizzle atoms of the ring and the 32-byte swizzle of the
+// output staging; the total must stay within the 227 KB a block may opt in to
+static_assert(kUSmemTotal <= 232448, "upconv_fused: shared memory over the per-block limit");
 
 struct UBarriers {
   uint64_t full[kUStages];
@@ -178,14 +187,16 @@ upconv_fused_kernel(const __grid_constant__ CUtensorMap map_a_hi,
                     const __grid_constant__ CUtensorMap map_o_hi,
                     const __grid_constant__ CUtensorMap map_o_lo, const UpFusedParams p) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 511) &
+                                             ~static_cast<uintptr_t>(511));
   float* mail = reinterpret_cast<float*>(smem + kUStages * kUStageBytes);
   uint8_t* out_stage = smem + kUStages * kUStageBytes + kUMailFloats * 4;
   float2* xchg = reinterpret_cast<float2*>(out_stage + kUOutStageBytes);
   UBarriers* bars = reinterpret_cast<UBarriers*>(out_stage + kUOutStageBytes + kUXchgBytes);
 
-  const int warp = threadIdx.x >> 5;
+  // broadcast from lane 0: the compiler then knows the role branches are warp-uniform, which it
+  // needs to give the consumer code the registers setmaxnreg grants
+  const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
   const int kb_count = p.Cin / UBK;
   const int G = UM / p.W;                 // images per tile
@@ -205,50 +216,9 @@ upconv_fused_kernel(const __grid_constant__ CUtensorMap map_a_hi,
   }
   __syncthreads();
 
-  if (warp == kUTmaWarp) {
-    // ------------------------------ TMA producer ------------------------------
-    // The A tile's rows are PERMUTED: inside every 32-pixel quarter, tile row 8 j + g holds pixel
-    // 4 g + j (j < 4, g < 8), so that the wgmma accumulator rows of a warp pair hold, per thread,
-    // four ADJACENT pixels.  The permutation is free: the tensor map lists the key planes' dimensions as
-    // (channel, x / 4 % 8, x % 4, x / 32, row) — TMA fills shared memory in that order — so one
-    // load still brings a whole image row (W >= 32; W < 32: (channel, x / 4, image, x % 4, y), one
-    // load per quarter).  [Loading the eight rows of each (quarter, j) separately — 32 one-KB
-    // boxes per plane and stage, strided or not — fed the MMAs at a third of their rate.]
-    int stage = 0;
-    uint32_t phase = 0;
-    const bool wide = p.W >= 32;
-    const int nop = wide ? G : 4;                  // loads per plane and stage
-    const int plane = lane / nop, idx = lane % nop;
-    const CUtensorMap* amap = plane ? &map_a_lo : &map_a_hi;
-    const CUtensorMap* wmap = (lane & 1) ? &map_w_lo : &map_w_hi;
-    const uint32_t a_off = plane * kUABytes + idx * (kUABytes / nop);
-    for (int item = blockIdx.x; item < p.nitems; item += gridDim.x) {
-      const UpItem it = decode_item(item, p);
-      const int b0 = it.bg * G;
-      const int wrow = it.cg * UN;
-      for (int y = it.y_first; y < it.y_end; ++y) {
-        for (int kb = 0; kb < kb_count; ++kb) {
-          if (lane == 0) {
-            mbar_wait_relaxed(&bars->empty[stage], phase ^ 1u);
-            mbar_expect_tx(&bars->full[stage], kUStageBytes);
-          }
-          __syncwarp();
-          uint8_t* st = smem + stage * kUStageBytes;
-          if (lane < 2 * nop) {
-            if (wide)
-              tma_load_5d(st + a_off, amap, &bars->full[stage], kb * UBK, 0, 0, 0,
-                          (b0 + idx) * (p.H + 1) + y);
-            else
-              tma_load_5d(st + a_off, amap, &bars->full[stage], kb * UBK, 0, b0 + idx * (32 / p.W), 0, y);
-          } else if (lane >= 30) {
-            tma_load_2d(st + 2 * kUABytes + (lane & 1) * kUBBytes, wmap, &bars->full[stage], kb * UBK,
-                        wrow);
-          }
-          if (++stage == kUStages) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
-  } else {
+  // the consumer branch comes first: with the producer first, ptxas kept the consumer code at the
+  // 168-register launch bound and spilled 480 B per thread
+  if (warp < kUTmaWarp) {
     // ------------------------------ MMA + epilogue ----------------------------
     // warp w (0..7) issues, with its warpgroup, the wgmma rows 16 w .. 16 w + 15 of the tile = the
     // pixels j = 2 (w % 2) + i (i = 0, 1) of lane quarter q = w / 2, for all 144 columns; it keeps
@@ -256,6 +226,7 @@ upconv_fused_kernel(const __grid_constant__ CUtensorMap map_a_hi,
     // Then thread (g = lane / 4, c = lane % 4) of warp (q, h) owns the four adjacent pixels
     // 32 q + 4 g + j of the tile and the two output channels 8 h + 2 c + e of the item's sixteen:
     // "unit" u = 2 j + e indexes its eight (pixel, channel) pairs.
+    setmaxnreg_inc<kUConsumerRegs>();
     const int wg = warp >> 2;
     const int q = warp >> 1;
     const int h = warp & 1;
@@ -354,13 +325,16 @@ upconv_fused_kernel(const __grid_constant__ CUtensorMap map_a_hi,
         float2 P[9][4];                                              // [tap][pixel j] (e0, e1)
         {
           float d[72];
+          // one wgmma group stays in flight: a stage is released once the group after it has
+          // been issued and the group that read it has completed
+          int held = -1;
           for (int kb = 0; kb < kb_count; ++kb) {
             mbar_wait(&bars->full[stage], phase);
             const uint32_t sa = smem_u32(smem + stage * kUStageBytes);
-            const uint64_t da_hi = make_smem_desc(sa + wg * (kUABytes / 2), 16, 1024);
-            const uint64_t da_lo = make_smem_desc(sa + kUABytes + wg * (kUABytes / 2), 16, 1024);
-            const uint64_t db_hi = make_smem_desc(sa + 2 * kUABytes, 16, 1024);
-            const uint64_t db_lo = make_smem_desc(sa + 2 * kUABytes + kUBBytes, 16, 1024);
+            const uint64_t da_hi = make_smem_desc(sa + wg * (kUABytes / 2), 16, 512, 2);
+            const uint64_t da_lo = make_smem_desc(sa + kUABytes + wg * (kUABytes / 2), 16, 512, 2);
+            const uint64_t db_hi = make_smem_desc(sa + 2 * kUABytes, 16, 512, 2);
+            const uint64_t db_lo = make_smem_desc(sa + 2 * kUABytes + kUBBytes, 16, 512, 2);
             wgmma_fence();
 #pragma unroll
             for (int kk = 0; kk < UBK / UK; ++kk) {
@@ -370,10 +344,13 @@ upconv_fused_kernel(const __grid_constant__ CUtensorMap map_a_hi,
               wgmma_m64n144<0, 0>(d, da_hi + adv, db_hi + adv, 1u);
             }
             wgmma_commit();
-            wgmma_wait<0>();
-            if ((threadIdx.x & 127) == 0) mbar_arrive(&bars->empty[stage]);
+            wgmma_wait<1>();
+            if (held >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(&bars->empty[held]);
+            held = stage;
             if (++stage == kUStages) { stage = 0; phase ^= 1u; }
           }
+          wgmma_wait<0>();
+          if ((threadIdx.x & 127) == 0) mbar_arrive(&bars->empty[held]);
           if constexpr (PROF) tq[1] = clock64();
           // accumulator columns: [channel half][tap][8 channels] (prep_weights, transpose_io = 2);
           // every register index is a compile-time constant (a run-time one puts d in local memory)
@@ -632,6 +609,52 @@ upconv_fused_kernel(const __grid_constant__ CUtensorMap map_a_hi,
         for (int i = 0; i < 16; ++i) dst[i] = prof_acc[i];
       }
     }
+  } else {
+    // ------------------------------ TMA producer ------------------------------
+    setmaxnreg_dec<kUProducerRegs>();
+    if (warp != kUTmaWarp) return;
+    // The A tile's rows are PERMUTED: inside every 32-pixel quarter, tile row 8 j + g holds pixel
+    // 4 g + j (j < 4, g < 8), so that the wgmma accumulator rows of a warp pair hold, per thread,
+    // four ADJACENT pixels.  The permutation is free: the tensor map lists the key planes' dimensions as
+    // (channel, x / 4 % 8, x % 4, x / 32, row) — TMA fills shared memory in that order — so one
+    // load still brings a whole image row (W >= 32; W < 32: (channel, x / 4, image, x % 4, y), one
+    // load per quarter).  [Loading the eight rows of each (quarter, j) separately — 32 one-KB
+    // boxes per plane and stage, strided or not — fed the MMAs at a third of their rate.]
+    int stage = 0;
+    uint32_t phase = 0;
+    const bool wide = p.W >= 32;
+    const int nop = wide ? G : 4;                  // loads per plane and stage
+    const int plane = lane / nop, idx = lane % nop;
+    const CUtensorMap* amap = plane ? &map_a_lo : &map_a_hi;
+    const CUtensorMap* wmap = (lane & 1) ? &map_w_lo : &map_w_hi;
+    const uint32_t a_off = plane * kUABytes + idx * (kUABytes / nop);
+    for (int item = blockIdx.x; item < p.nitems; item += gridDim.x) {
+      const UpItem it = decode_item(item, p);
+      const int b0 = it.bg * G;
+      const int wrow = it.cg * UN;
+      for (int y = it.y_first; y < it.y_end; ++y) {
+        for (int kb = 0; kb < kb_count; ++kb) {
+          if (lane == 0) {
+            mbar_wait_relaxed(&bars->empty[stage], phase ^ 1u);
+            mbar_expect_tx(&bars->full[stage], kUStageBytes);
+          }
+          __syncwarp();
+          uint8_t* st = smem + stage * kUStageBytes;
+          if (lane < 2 * nop) {
+            if (wide)
+              tma_load_5d(st + a_off, amap, &bars->full[stage], kb * UBK, 0, 0, 0,
+                          (b0 + idx) * (p.H + 1) + y);
+            else
+              tma_load_5d(st + a_off, amap, &bars->full[stage], kb * UBK, 0, b0 + idx * (32 / p.W), 0, y);
+          } else if (lane >= 30) {
+            tma_load_2d(st + 2 * kUABytes + (lane & 1) * kUBBytes, wmap, &bars->full[stage], kb * UBK,
+                        wrow);
+          }
+          if (++stage == kUStages) { stage = 0; phase ^= 1u; }
+        }
+      }
+    }
+    return;
   }
 
 }
@@ -685,16 +708,16 @@ int upconv_fused_launch(const UpFusedParams& pin, const void* a_hi, const void* 
                               static_cast<uint64_t>(p.B) * (H + 1)};
     const uint64_t str[4] = {4 * kpx, kpx, 32 * kpx, krow};
     const uint32_t box[5] = {UBK, 8u, 4u, static_cast<uint32_t>(W / 32), 1u};
-    if ((rc = make_tmap_nd_bf16(&ma_hi, a_hi, 5, dims, str, box, nullptr, 2))) return rc;
-    if ((rc = make_tmap_nd_bf16(&ma_lo, a_lo, 5, dims, str, box, nullptr, 2))) return rc;
+    if ((rc = make_tmap_nd_bf16(&ma_hi, a_hi, 5, dims, str, box, nullptr, 3))) return rc;
+    if ((rc = make_tmap_nd_bf16(&ma_lo, a_lo, 5, dims, str, box, nullptr, 3))) return rc;
   } else {
     // (channel, x / 4, image, x % 4, y)
     const uint64_t dims[5] = {static_cast<uint64_t>(p.Cin), static_cast<uint64_t>(W / 4),
                               static_cast<uint64_t>(p.B), 4, static_cast<uint64_t>(H + 1)};
     const uint64_t str[4] = {4 * kpx, static_cast<uint64_t>(H + 1) * krow, kpx, krow};
     const uint32_t box[5] = {UBK, static_cast<uint32_t>(W / 4), 32u / Wm, 4u, 1u};
-    if ((rc = make_tmap_nd_bf16(&ma_hi, a_hi, 5, dims, str, box, nullptr, 2))) return rc;
-    if ((rc = make_tmap_nd_bf16(&ma_lo, a_lo, 5, dims, str, box, nullptr, 2))) return rc;
+    if ((rc = make_tmap_nd_bf16(&ma_hi, a_hi, 5, dims, str, box, nullptr, 3))) return rc;
+    if ((rc = make_tmap_nd_bf16(&ma_lo, a_lo, 5, dims, str, box, nullptr, 3))) return rc;
   }
   // output planes [B][Ho+1][Wo+1][Cout] seen as (channel, X / 8, X % 8, Y, image): one store = 16
   // channels of a quarter's 64 output pixels, staged as [image][X % 8][X / 8][16 ch] so that the
@@ -715,11 +738,11 @@ int upconv_fused_launch(const UpFusedParams& pin, const void* a_hi, const void* 
     mo_hi = ma_hi;
     mo_lo = ma_lo;
   }
-  const uint64_t wrows = static_cast<uint64_t>(p.ncg) * UN;
-  if ((rc = make_tmap_2d_bf16(&mw_hi, w_hi, p.Cin, wrows, static_cast<uint64_t>(p.Cin) * 2, UBK, UN)))
-    return rc;
-  if ((rc = make_tmap_2d_bf16(&mw_lo, w_lo, p.Cin, wrows, static_cast<uint64_t>(p.Cin) * 2, UBK, UN)))
-    return rc;
+  const uint64_t wdims[2] = {static_cast<uint64_t>(p.Cin), static_cast<uint64_t>(p.ncg) * UN};
+  const uint64_t wstr[1] = {static_cast<uint64_t>(p.Cin) * 2};
+  const uint32_t wbox[2] = {UBK, UN};
+  if ((rc = make_tmap_nd_bf16(&mw_hi, w_hi, 2, wdims, wstr, wbox, nullptr, 3))) return rc;
+  if ((rc = make_tmap_nd_bf16(&mw_lo, w_lo, 2, wdims, wstr, wbox, nullptr, 3))) return rc;
   const int grid = p.nitems < sms ? p.nitems : sms;
   auto launch = [&](auto kernel, bool& attr_done) -> int {
     if (!attr_done) {
