@@ -19,8 +19,14 @@
 // each term optional, so the same kernel serves the un-fused `dconv` leaf of a
 // nethook-split layer, the conv_transpose phases of an up layer and dgrad.
 //
-// Warp roles (288 threads): warpgroups 0 and 1 each issue wgmma for 64 of the tile's 128 rows and
-// run the epilogue on their register accumulators; warp 8 is the TMA producer.  Persistent CTAs, 3-stage shared-memory ring.
+// Warp roles (384 threads): warpgroups 0 and 1 each issue wgmma for 64 of the tile's 128 rows and
+// run the epilogue on their register accumulators, raised to 232 registers by setmaxnreg;
+// warpgroup 2 is the producer, lowered to 40, whose warp 8 issues the TMA loads.  A 7-stage ring
+// of 32 KB stages (BK = 32, 64-byte swizzle); the consumers keep one wgmma group in flight and
+// release each stage one k-block behind.
+// Persistent 2-CTA clusters: the two CTAs take adjacent m-tiles with the same (phase, n), so they
+// read the same weight tile on every k-block; each loads one 64-row half of it and multicasts the
+// half to both, cutting each CTA's L2 reads per k-block from 32 KB to 24 KB.
 #include <cstdlib>
 #include <cstring>
 
@@ -33,34 +39,44 @@ namespace {
 
 constexpr int BM = 128;
 constexpr int BN = 128;
-constexpr int BK = 64;            // bf16 elements per k-block = one 128B swizzle row
+// k-block of 32 channels = one 64-byte swizzle row: a 32 KB stage, so that seven fit in shared
+// memory and the producer runs up to six k-blocks ahead of the MMAs
+constexpr int BK = 32;
 constexpr int MMA_K = 16;
-constexpr int kStages = 3;
-constexpr int kNumThreads = 288;   // two consumer warpgroups + the producer warp
+constexpr int kStages = 7;
+constexpr int kNumThreads = 384;   // warps 0-7: wgmma + epilogue, warpgroup 2: producer
 constexpr int kTmaWarp = 8;
+// register split after setmaxnreg: 128 x 40 + 256 x 232 = 384 x 168, the launch allocation
+constexpr uint32_t kProducerRegs = 40;
+constexpr uint32_t kConsumerRegs = 232;
+// CTAs per cluster: they share (multicast) the weight tile of a k-block
+constexpr int kCluster = 2;
 // The tensor core's fp32 accumulate truncates (round-toward-zero) on every MMA, a relative bias of
 // ~ -2^-25 per accumulation, i.e. 1.6e-5 after the 864 accumulations of a K=4608 tile.  So the
 // wgmma accumulator only ever holds a CHUNK of kChunkKB k-blocks (K=512: 96 accumulations); the
 // chunks are added in fp32 registers with round-to-nearest.
-// (chunk 8 -> pixel error 5.2e-4, chunk 16 -> 8.1e-4, >= 36 fails the 1e-3 bound)
-constexpr int kChunkKB = 8;
+// (K=512 -> pixel error 5.2e-4, K=1024 -> 8.1e-4, K >= 2304 fails the 1e-3 bound)
+constexpr int kChunkKB = 16;
 
 struct ConvSmem {
-  static constexpr int kABytes = BM * BK * 2;          // one plane
-  static constexpr int kBBytes = BN * BK * 2;          // one plane
+  static constexpr int kABytes = BM * BK * 2;          // one plane: 8 KB
+  static constexpr int kBBytes = BN * BK * 2;          // one plane: 8 KB
   static constexpr int kStageBytes = 2 * kABytes + 2 * kBBytes;
-  static constexpr int kTotal = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int kTotal = kStages * kStageBytes + 512 /*align slack*/ + 256 /*barriers*/;
 };
+// 512-byte alignment serves the 64-byte swizzle atoms; the total must stay within the 227 KB a
+// block may opt in to
+static_assert(ConvSmem::kTotal <= 232448, "conv_tc: shared memory over the per-block limit");
 
 struct Barriers {
   uint64_t full[kStages];
   uint64_t empty[kStages];
 };
 
-// tile -> (phase, mn).  Phases have very different tap counts (4/2/2/1 for a stride-2
+// work unit -> (phase, mn).  Phases have very different tap counts (4/2/2/1 for a stride-2
 // conv_transpose); with a static round-robin every scheduler slot would keep drawing the same
-// one or two phases, so the phase is rotated by the (m, n) group index — a bijection inside
-// every group of `nphase` consecutive tiles.
+// one or two phases, so the phase is rotated by the (m-pair, n) group index — a bijection inside
+// every group of `nphase` consecutive units.
 __device__ __forceinline__ void decode_tile(int tile, int nphase, int nsched, int& ph, int& mn) {
   mn = tile / nphase;
   ph = tile - mn * nphase;
@@ -78,19 +94,26 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
                const __grid_constant__ CUtensorMap map_w_hi,
                const __grid_constant__ CUtensorMap map_w_lo, const ConvTcParams p) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~static_cast<uintptr_t>(1023));
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 511) &
+                                             ~static_cast<uintptr_t>(511));
   using S = ConvSmem;
   Barriers* bars = reinterpret_cast<Barriers*>(smem + kStages * S::kStageBytes);
 
-  const int warp = threadIdx.x >> 5;
+  // broadcast from lane 0: the compiler then knows the role branches are warp-uniform, which it
+  // needs to give the consumer code the registers setmaxnreg grants
+  const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
-  const int nsched = gridDim.x;
+  // a cluster of kCluster CTAs works on a unit of kCluster m-tiles with the same (phase, n): CTA
+  // `rank` takes m-tile kCluster * mp + rank.  Beyond an odd last m-tile the second tile lies
+  // wholly past p.rows: TMA zero-fills its rows and the epilogue's row guards store nothing.
+  const int rank = static_cast<int>(cluster_ctarank());
+  const int nsched = static_cast<int>(num_clusters_x());
+  const int first_unit = static_cast<int>(cluster_id_x());
 
   const int m_tiles = (p.rows + BM - 1) / BM;
   const int n_tiles = p.Cout / BN;
-  const int mn_tiles = m_tiles * n_tiles;
-  const int num_tiles = mn_tiles * p.nphase;
+  const int mn_units = (m_tiles + kCluster - 1) / kCluster * n_tiles;
+  const int num_units = mn_units * p.nphase;
   const int kb_per_tap = p.Cin / BK;
 
   if (warp == kTmaWarp && lane == 0) {
@@ -100,22 +123,217 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
     tma_prefetch_desc(&map_w_lo);
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&bars->full[s], 1);
-      mbar_init(&bars->empty[s], 2);      // one arrival per consumer warpgroup
+      // one arrival per consumer warpgroup of every CTA: the stage's B tile is refilled in all
+      // of them at once
+      mbar_init(&bars->empty[s], 2 * kCluster);
     }
     fence_mbar_init();
   }
-  __syncthreads();
+  // the barriers are initialised cluster-wide before any remote arrival or multicast
+  cluster_sync();
 
-  if (warp == kTmaWarp) {
+  // the consumer branch comes first: with the producer first, ptxas keeps the consumer code at
+  // the 168-register launch bound and spills
+  if (warp < kTmaWarp) {
+    // ------------------------- MMA + epilogue (consumers) ------------------------
+    setmaxnreg_inc<kConsumerRegs>();
+    const int wg = threadIdx.x >> 7;            // 64-row half of the tile
+    const int c = lane & 3;
+    const int img = p.Hp * p.Wp;
+    // a stage is released in every CTA of the cluster (one arrival per consumer warpgroup)
+    auto release = [&](int s) {
+      if ((threadIdx.x & 127) == 0) {
+#pragma unroll
+        for (int r = 0; r < kCluster; ++r) mbar_arrive_cluster(mapa_shared(&bars->empty[s], r));
+      }
+    };
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int unit = first_unit; unit < num_units; unit += nsched) {
+      int ph, mn;
+      decode_tile(unit, p.nphase, nsched, ph, mn);
+      const int num_kb = p.ph_ntaps[ph] * kb_per_tap;
+      const int n_tile = mn % n_tiles;
+      const int n0 = n_tile * BN;
+      const int m0 = ((mn / n_tiles) * kCluster + rank) * BM;
+
+      float acc[64], d[64];
+#pragma unroll
+      for (int j = 0; j < 64; ++j) acc[j] = 0.f;
+      for (int kb0 = 0; kb0 < num_kb; kb0 += kChunkKB) {
+        const int kb_end = (kb0 + kChunkKB < num_kb) ? kb0 + kChunkKB : num_kb;
+        // one wgmma group stays in flight: a stage is released once the group after it has been
+        // issued and the group that read it has completed
+        int held = -1;
+        for (int kb = kb0; kb < kb_end; ++kb) {
+          mbar_wait(&bars->full[stage], phase);
+          const uint32_t sa = smem_u32(smem + stage * S::kStageBytes);
+          const uint64_t da_hi = make_smem_desc(sa + wg * (S::kABytes / 2), 16, 512, 2);
+          const uint64_t da_lo = make_smem_desc(sa + S::kABytes + wg * (S::kABytes / 2), 16, 512, 2);
+          const uint64_t db_hi = make_smem_desc(sa + 2 * S::kABytes, 16, 512, 2);
+          const uint64_t db_lo = make_smem_desc(sa + 2 * S::kABytes + S::kBBytes, 16, 512, 2);
+          wgmma_fence();
+#pragma unroll
+          for (int kk = 0; kk < BK / MMA_K; ++kk) {
+            const uint64_t adv = static_cast<uint64_t>((kk * MMA_K * 2) >> 4);
+            // smallest terms first, then the dominant hi*hi product
+            wgmma_m64n128<0, 0>(d, da_lo + adv, db_hi + adv, ((kb - kb0) | kk) != 0);
+            wgmma_m64n128<0, 0>(d, da_hi + adv, db_lo + adv, 1u);
+            wgmma_m64n128<0, 0>(d, da_hi + adv, db_hi + adv, 1u);
+          }
+          wgmma_commit();
+          wgmma_wait<1>();
+          if (held >= 0) release(held);
+          held = stage;
+          if (++stage == kStages) { stage = 0; phase ^= 1u; }
+        }
+        // the chunk is complete before it is added; its last stage is released here, so the
+        // producer refills the ring while the epilogue runs
+        wgmma_wait<0>();
+        release(held);
+#pragma unroll
+        for (int j = 0; j < 64; ++j) acc[j] += d[j];
+      }
+
+      // ---- fused epilogue: rows r = m0 + 64 wg + 16 (warp % 4) + g + 8 i, columns 8 j + 2 c + e ----
+      // (the thread's row offset is formed here from a fresh %tid.x: hoisted above the main loop,
+      // it is the one value ptxas spills in the full epilogue's variant)
+      uint32_t tid;
+      asm volatile("mov.u32 %0, %%tid.x;\n" : "=r"(tid));
+      const int row0 = m0 + ((tid >> 7) << 6) + (((tid >> 5) & 3) << 4) + ((tid & 31) >> 2);
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int prow = row0 + 8 * i;
+        const int b = prow / img;
+        const int rem = prow - b * img;
+        const int yy = rem / p.Wp;
+        const int xx = rem - yy * p.Wp;
+        const int Hv = p.ph_Hv[ph], Wv = p.ph_Wv[ph];
+        const bool in_rows = prow < p.rows;
+        const bool valid = in_rows && (yy < Hv) && (xx < Wv);
+        const float* scl = (p.scale_bo && in_rows) ? p.scale_bo + static_cast<size_t>(b) * p.Cout : nullptr;
+        float* outp = (p.out != nullptr && p.out_mode == 0 && valid)
+                          ? p.out + p.ph_out_ofs[ph] + static_cast<size_t>(b) * p.out_sb +
+                                static_cast<size_t>(yy) * p.out_sy + static_cast<size_t>(xx) * p.out_sx
+                          : nullptr;
+        if (EPI == 1 || !valid) {
+          // lean epilogue, and the pad rows of the full one: only the optional scale
+          if (scl && (EPI == 1 || p.out_mode == 1)) {
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+              const float2 sv = __ldg(reinterpret_cast<const float2*>(scl + n0 + 8 * j + 2 * c));
+              acc[4 * j + 2 * i] *= sv.x;
+              acc[4 * j + 2 * i + 1] *= sv.y;
+            }
+          }
+          if (EPI == 1 && outp) {
+#pragma unroll
+            for (int j = 0; j < 16; ++j)
+#pragma unroll
+              for (int e = 0; e < 2; ++e)
+                outp[static_cast<size_t>(n0 + 8 * j + 2 * c + e) * p.out_sc] = acc[4 * j + 2 * i + e];
+          }
+        } else {
+          float nz = 0.f;
+          if (p.noise != nullptr)
+            nz = __ldg(p.noise_w) * __ldg(p.noise + static_cast<size_t>(b) * p.noise_bstride +
+                                          static_cast<size_t>(yy) * Wv + xx);
+          const float act_gain = p.act_gain != 0.f ? p.act_gain : 1.4142135623730951f;
+#pragma unroll
+          for (int j = 0; j < 16; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int o = n0 + 8 * j + 2 * c + e;
+              float t = acc[4 * j + 2 * i + e];
+              if (scl) t *= __ldg(scl + o);
+              t += nz;
+              if (p.bias) t += __ldg(p.bias + o);
+              if (p.act) t = (t > 0.f ? t : 0.2f * t) * act_gain;
+              acc[4 * j + 2 * i + e] = t;
+              if (outp) outp[static_cast<size_t>(o) * p.out_sc] = t;
+            }
+        }
+        if (EPI == 0 && p.rgb_w != nullptr) {
+          // one partial per 64-channel group: rgb_part[(n_tile*2 + half)][b][c][y*Wv+x]; the four
+          // lanes of a row hold 16 of the group's channels each
+          const float* rw0 = p.rgb_w + (static_cast<size_t>(valid ? b : 0) * 3) * p.Cout;
+#pragma unroll
+          for (int half = 0; half < 2; ++half) {
+            float r0 = 0.f, r1 = 0.f, r2 = 0.f;
+            if (valid) {
+#pragma unroll
+              for (int j = 8 * half; j < 8 * half + 8; ++j)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  const int o = n0 + 8 * j + 2 * c + e;
+                  const float t = acc[4 * j + 2 * i + e];
+                  r0 = fmaf(__ldg(rw0 + o), t, r0);
+                  r1 = fmaf(__ldg(rw0 + p.Cout + o), t, r1);
+                  r2 = fmaf(__ldg(rw0 + 2 * p.Cout + o), t, r2);
+                }
+            }
+#pragma unroll
+            for (int s = 1; s < 4; s <<= 1) {
+              r0 += __shfl_xor_sync(0xffffffffu, r0, s);
+              r1 += __shfl_xor_sync(0xffffffffu, r1, s);
+              r2 += __shfl_xor_sync(0xffffffffu, r2, s);
+            }
+            if (valid && c == 0) {
+              const size_t hw = static_cast<size_t>(Hv) * Wv;
+              float* rp = p.rgb_part + ((static_cast<size_t>(n_tile * 2 + half) * p.B + b) * 3) * hw +
+                          static_cast<size_t>(yy) * Wv + xx;
+              rp[0] = r0;
+              rp[hw] = r1;
+              rp[2 * hw] = r2;
+            }
+          }
+        }
+        // channels-last raw rows are written for every row (pad rows are never read back)
+        if (p.out != nullptr && p.out_mode == 1 && in_rows) {
+          float* orow = p.out + (static_cast<size_t>(ph) * p.rows + prow) * p.Cout + n0 + 2 * c;
+#pragma unroll
+          for (int j = 0; j < 16; ++j)
+            *reinterpret_cast<float2*>(orow + 8 * j) = make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
+        }
+        if (EPI == 0 && p.next_hi != nullptr && in_rows) {
+          const float* ns = p.next_scale + static_cast<size_t>(valid ? b : 0) * p.Cout + n0 + 2 * c;
+          const size_t ofs = static_cast<size_t>(prow) * p.Cout + n0 + 2 * c;
+          uint32_t* nh = reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(p.next_hi) + ofs);
+          uint32_t* nl = reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(p.next_lo) + ofs);
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+            float k0 = 0.f, k1 = 0.f;
+            if (valid) {
+              const float2 sv = __ldg(reinterpret_cast<const float2*>(ns + 8 * j));
+              k0 = sv.x * acc[4 * j + 2 * i];
+              k1 = sv.y * acc[4 * j + 2 * i + 1];
+            }
+            const __nv_bfloat162 hh = __floats2bfloat162_rn(k0, k1);
+            const float2 hf = __bfloat1622float2(hh);
+            const __nv_bfloat162 ll = __floats2bfloat162_rn(k0 - hf.x, k1 - hf.y);
+            nh[4 * j] = *reinterpret_cast<const uint32_t*>(&hh);
+            nl[4 * j] = *reinterpret_cast<const uint32_t*>(&ll);
+          }
+        }
+      }
+    }
+  } else {
     // ------------------------------ TMA producer ------------------------------
-    if (lane == 0) {
+    // every CTA loads its own A tile and one BN / kCluster-row slice of the B tile, multicast to
+    // the same stage offset in every CTA of the cluster; a full barrier thus receives a whole
+    // stage, kStageBytes, and a stage is refilled only once all CTAs have released it
+    setmaxnreg_dec<kProducerRegs>();
+    if (warp == kTmaWarp && lane == 0) {
+      constexpr uint16_t kMask = (1u << kCluster) - 1;
+      constexpr int kBSlice = BN / kCluster;
+      const uint32_t b_off = 2 * S::kABytes + rank * (S::kBBytes / kCluster);
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += nsched) {
+      for (int unit = first_unit; unit < num_units; unit += nsched) {
         int ph, mn;
-        decode_tile(tile, p.nphase, nsched, ph, mn);
-        const int n0 = (mn % n_tiles) * BN;
-        const int m0 = (mn / n_tiles) * BM;
+        decode_tile(unit, p.nphase, nsched, ph, mn);
+        const int n0 = (mn % n_tiles) * BN + rank * kBSlice;
+        const int m0 = ((mn / n_tiles) * kCluster + rank) * BM;
         for (int t = 0; t < p.ph_ntaps[ph]; ++t) {
           const int arow = m0 + p.ph_shift[ph][t];
           const int wcol = p.ph_kofs[ph][t];
@@ -126,178 +344,20 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
             mbar_expect_tx(&bars->full[stage], S::kStageBytes);
             tma_load_2d(st, &map_a_hi, &bars->full[stage], acol + kb * BK, arow);
             tma_load_2d(st + S::kABytes, &map_a_lo, &bars->full[stage], acol + kb * BK, arow);
-            tma_load_2d(st + 2 * S::kABytes, &map_w_hi, &bars->full[stage], wcol + kb * BK, n0);
-            tma_load_2d(st + 2 * S::kABytes + S::kBBytes, &map_w_lo, &bars->full[stage],
-                        wcol + kb * BK, n0);
+            tma_load_2d_multicast(st + b_off, &map_w_hi, &bars->full[stage], wcol + kb * BK, n0,
+                                  kMask);
+            tma_load_2d_multicast(st + b_off + S::kBBytes, &map_w_lo, &bars->full[stage],
+                                  wcol + kb * BK, n0, kMask);
             if (++stage == kStages) { stage = 0; phase ^= 1u; }
           }
         }
       }
     }
-    return;
+    __syncwarp();
   }
-
-  // ------------------------- MMA + epilogue (consumers) ------------------------
-  const int wg = threadIdx.x >> 7;            // 64-row half of the tile
-  const int g = lane >> 2, c = lane & 3;
-  const int img = p.Hp * p.Wp;
-  int stage = 0;
-  uint32_t phase = 0;
-  for (int tile = blockIdx.x; tile < num_tiles; tile += nsched) {
-    int ph, mn;
-    decode_tile(tile, p.nphase, nsched, ph, mn);
-    const int num_kb = p.ph_ntaps[ph] * kb_per_tap;
-    const int n_tile = mn % n_tiles;
-    const int n0 = n_tile * BN;
-    const int m0 = (mn / n_tiles) * BM;
-
-    float acc[64], d[64];
-#pragma unroll
-    for (int j = 0; j < 64; ++j) acc[j] = 0.f;
-    for (int kb0 = 0; kb0 < num_kb; kb0 += kChunkKB) {
-      const int kb_end = (kb0 + kChunkKB < num_kb) ? kb0 + kChunkKB : num_kb;
-      for (int kb = kb0; kb < kb_end; ++kb) {
-        mbar_wait(&bars->full[stage], phase);
-        const uint32_t sa = smem_u32(smem + stage * S::kStageBytes);
-        const uint64_t da_hi = make_smem_desc(sa + wg * (S::kABytes / 2), 16, 1024);
-        const uint64_t da_lo = make_smem_desc(sa + S::kABytes + wg * (S::kABytes / 2), 16, 1024);
-        const uint64_t db_hi = make_smem_desc(sa + 2 * S::kABytes, 16, 1024);
-        const uint64_t db_lo = make_smem_desc(sa + 2 * S::kABytes + S::kBBytes, 16, 1024);
-        wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < BK / MMA_K; ++kk) {
-          const uint64_t adv = static_cast<uint64_t>((kk * MMA_K * 2) >> 4);
-          // smallest terms first, then the dominant hi*hi product
-          wgmma_m64n128<0, 0>(d, da_lo + adv, db_hi + adv, ((kb - kb0) | kk) != 0);
-          wgmma_m64n128<0, 0>(d, da_hi + adv, db_lo + adv, 1u);
-          wgmma_m64n128<0, 0>(d, da_hi + adv, db_hi + adv, 1u);
-        }
-        wgmma_commit();
-        wgmma_wait<0>();
-        if ((threadIdx.x & 127) == 0) mbar_arrive(&bars->empty[stage]);
-        if (++stage == kStages) { stage = 0; phase ^= 1u; }
-      }
-#pragma unroll
-      for (int j = 0; j < 64; ++j) acc[j] += d[j];
-    }
-
-    // ---- fused epilogue: rows r = m0 + 64 wg + 16 (warp % 4) + g + 8 i, columns 8 j + 2 c + e ----
-#pragma unroll
-    for (int i = 0; i < 2; ++i) {
-      const int prow = m0 + wg * 64 + (warp & 3) * 16 + g + 8 * i;
-      const int b = prow / img;
-      const int rem = prow - b * img;
-      const int yy = rem / p.Wp;
-      const int xx = rem - yy * p.Wp;
-      const int Hv = p.ph_Hv[ph], Wv = p.ph_Wv[ph];
-      const bool in_rows = prow < p.rows;
-      const bool valid = in_rows && (yy < Hv) && (xx < Wv);
-      const float* scl = (p.scale_bo && in_rows) ? p.scale_bo + static_cast<size_t>(b) * p.Cout : nullptr;
-      float* outp = (p.out != nullptr && p.out_mode == 0 && valid)
-                        ? p.out + p.ph_out_ofs[ph] + static_cast<size_t>(b) * p.out_sb +
-                              static_cast<size_t>(yy) * p.out_sy + static_cast<size_t>(xx) * p.out_sx
-                        : nullptr;
-      if (EPI == 1 || !valid) {
-        // lean epilogue, and the pad rows of the full one: only the optional scale
-        if (scl && (EPI == 1 || p.out_mode == 1)) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const float2 sv = __ldg(reinterpret_cast<const float2*>(scl + n0 + 8 * j + 2 * c));
-            acc[4 * j + 2 * i] *= sv.x;
-            acc[4 * j + 2 * i + 1] *= sv.y;
-          }
-        }
-        if (EPI == 1 && outp) {
-#pragma unroll
-          for (int j = 0; j < 16; ++j)
-#pragma unroll
-            for (int e = 0; e < 2; ++e)
-              outp[static_cast<size_t>(n0 + 8 * j + 2 * c + e) * p.out_sc] = acc[4 * j + 2 * i + e];
-        }
-      } else {
-        float nz = 0.f;
-        if (p.noise != nullptr)
-          nz = __ldg(p.noise_w) * __ldg(p.noise + static_cast<size_t>(b) * p.noise_bstride +
-                                        static_cast<size_t>(yy) * Wv + xx);
-        const float act_gain = p.act_gain != 0.f ? p.act_gain : 1.4142135623730951f;
-#pragma unroll
-        for (int j = 0; j < 16; ++j)
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int o = n0 + 8 * j + 2 * c + e;
-            float t = acc[4 * j + 2 * i + e];
-            if (scl) t *= __ldg(scl + o);
-            t += nz;
-            if (p.bias) t += __ldg(p.bias + o);
-            if (p.act) t = (t > 0.f ? t : 0.2f * t) * act_gain;
-            acc[4 * j + 2 * i + e] = t;
-            if (outp) outp[static_cast<size_t>(o) * p.out_sc] = t;
-          }
-      }
-      if (EPI == 0 && p.rgb_w != nullptr) {
-        // one partial per 64-channel group: rgb_part[(n_tile*2 + half)][b][c][y*Wv+x]; the four
-        // lanes of a row hold 16 of the group's channels each
-        const float* rw0 = p.rgb_w + (static_cast<size_t>(valid ? b : 0) * 3) * p.Cout;
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          float r0 = 0.f, r1 = 0.f, r2 = 0.f;
-          if (valid) {
-#pragma unroll
-            for (int j = 8 * half; j < 8 * half + 8; ++j)
-#pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                const int o = n0 + 8 * j + 2 * c + e;
-                const float t = acc[4 * j + 2 * i + e];
-                r0 = fmaf(__ldg(rw0 + o), t, r0);
-                r1 = fmaf(__ldg(rw0 + p.Cout + o), t, r1);
-                r2 = fmaf(__ldg(rw0 + 2 * p.Cout + o), t, r2);
-              }
-          }
-#pragma unroll
-          for (int s = 1; s < 4; s <<= 1) {
-            r0 += __shfl_xor_sync(0xffffffffu, r0, s);
-            r1 += __shfl_xor_sync(0xffffffffu, r1, s);
-            r2 += __shfl_xor_sync(0xffffffffu, r2, s);
-          }
-          if (valid && c == 0) {
-            const size_t hw = static_cast<size_t>(Hv) * Wv;
-            float* rp = p.rgb_part + ((static_cast<size_t>(n_tile * 2 + half) * p.B + b) * 3) * hw +
-                        static_cast<size_t>(yy) * Wv + xx;
-            rp[0] = r0;
-            rp[hw] = r1;
-            rp[2 * hw] = r2;
-          }
-        }
-      }
-      // channels-last raw rows are written for every row (pad rows are never read back)
-      if (p.out != nullptr && p.out_mode == 1 && in_rows) {
-        float* orow = p.out + (static_cast<size_t>(ph) * p.rows + prow) * p.Cout + n0 + 2 * c;
-#pragma unroll
-        for (int j = 0; j < 16; ++j)
-          *reinterpret_cast<float2*>(orow + 8 * j) = make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
-      }
-      if (EPI == 0 && p.next_hi != nullptr && in_rows) {
-        const float* ns = p.next_scale + static_cast<size_t>(valid ? b : 0) * p.Cout + n0 + 2 * c;
-        const size_t ofs = static_cast<size_t>(prow) * p.Cout + n0 + 2 * c;
-        uint32_t* nh = reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(p.next_hi) + ofs);
-        uint32_t* nl = reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(p.next_lo) + ofs);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          float k0 = 0.f, k1 = 0.f;
-          if (valid) {
-            const float2 sv = __ldg(reinterpret_cast<const float2*>(ns + 8 * j));
-            k0 = sv.x * acc[4 * j + 2 * i];
-            k1 = sv.y * acc[4 * j + 2 * i + 1];
-          }
-          const __nv_bfloat162 hh = __floats2bfloat162_rn(k0, k1);
-          const float2 hf = __bfloat1622float2(hh);
-          const __nv_bfloat162 ll = __floats2bfloat162_rn(k0 - hf.x, k1 - hf.y);
-          nh[4 * j] = *reinterpret_cast<const uint32_t*>(&hh);
-          nl[4 * j] = *reinterpret_cast<const uint32_t*>(&ll);
-        }
-      }
-    }
-  }
+  // no CTA leaves while another CTA of its cluster can still multicast into its shared memory or
+  // arrive on its barriers
+  cluster_sync();
 }
 
 }  // namespace
@@ -308,34 +368,60 @@ static int conv_tc_launch_epi(const ConvTcParams& p, const void* a_hi, const voi
                               cudaStream_t stream) {
   CUtensorMap ma_hi, ma_lo, mw_hi, mw_lo;
   int rc;
-  const int a_cols = p.a_cols > 0 ? p.a_cols : p.Cin;
-  if ((rc = make_tmap_2d_bf16(&ma_hi, a_hi, a_cols, p.rows, (uint64_t)a_cols * 2, BK, BM))) return rc;
-  if ((rc = make_tmap_2d_bf16(&ma_lo, a_lo, a_cols, p.rows, (uint64_t)a_cols * 2, BK, BM))) return rc;
-  if ((rc = make_tmap_2d_bf16(&mw_hi, w_hi, wk_total, p.Cout, (uint64_t)wk_total * 2, BK, BN)))
-    return rc;
-  if ((rc = make_tmap_2d_bf16(&mw_lo, w_lo, wk_total, p.Cout, (uint64_t)wk_total * 2, BK, BN)))
-    return rc;
+  // 64-byte swizzle: a box row is one k-block of BK = 32 channels
+  const uint64_t a_cols = p.a_cols > 0 ? p.a_cols : p.Cin;
+  const uint64_t a_dims[2] = {a_cols, static_cast<uint64_t>(p.rows)}, a_str[1] = {a_cols * 2};
+  const uint64_t w_dims[2] = {static_cast<uint64_t>(wk_total), static_cast<uint64_t>(p.Cout)};
+  const uint64_t w_str[1] = {static_cast<uint64_t>(wk_total) * 2};
+  const uint32_t a_box[2] = {BK, BM}, w_box[2] = {BK, BN / kCluster};
+  if ((rc = make_tmap_nd_bf16(&ma_hi, a_hi, 2, a_dims, a_str, a_box, nullptr, 3))) return rc;
+  if ((rc = make_tmap_nd_bf16(&ma_lo, a_lo, 2, a_dims, a_str, a_box, nullptr, 3))) return rc;
+  if ((rc = make_tmap_nd_bf16(&mw_hi, w_hi, 2, w_dims, w_str, w_box, nullptr, 3))) return rc;
+  if ((rc = make_tmap_nd_bf16(&mw_lo, w_lo, 2, w_dims, w_str, w_box, nullptr, 3))) return rc;
 
-  static bool attr_set = false;
-  if (!attr_set) {
+  cudaLaunchConfig_t cfg = {};
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = kCluster;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.blockDim = dim3(kNumThreads);
+  cfg.dynamicSmemBytes = ConvSmem::kTotal;
+  cfg.stream = stream;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  // persistent clusters: as many as can be resident at once (a GPC with an odd number of free
+  // SMs cannot host a whole cluster, so this is fewer than SMs / kCluster)
+  static int max_clusters = 0;
+  if (max_clusters == 0) {
     rc = check_cuda(cudaFuncSetAttribute(conv_tc_kernel<EPI>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, ConvSmem::kTotal),
                     "conv_tc smem attr");
     if (rc) return rc;
-    attr_set = true;
+    cfg.gridDim = dim3(kCluster * (device_sm_count() / kCluster));
+    rc = check_cuda(cudaOccupancyMaxActiveClusters(&max_clusters, conv_tc_kernel<EPI>, &cfg),
+                    "conv_tc cluster occupancy");
+    if (rc) return rc;
+    if (max_clusters < 1) {
+      set_last_error("conv_tc: no cluster of %d CTAs fits on the device", kCluster);
+      return RW_ERR_UNSUPPORTED;
+    }
   }
   const int m_tiles = (p.rows + BM - 1) / BM;
   const int n_tiles = p.Cout / BN;
-  const int num_tiles = m_tiles * n_tiles * p.nphase;
-  int sched = device_sm_count();
-  if (sched > num_tiles) sched = num_tiles;
-  conv_tc_kernel<EPI><<<sched, kNumThreads, ConvSmem::kTotal, stream>>>(ma_hi, ma_lo, mw_hi, mw_lo, p);
+  const int num_units = (m_tiles + kCluster - 1) / kCluster * n_tiles * p.nphase;
+  const int clusters = max_clusters < num_units ? max_clusters : num_units;
+  cfg.gridDim = dim3(kCluster * clusters);
+  rc = check_cuda(cudaLaunchKernelEx(&cfg, conv_tc_kernel<EPI>, ma_hi, ma_lo, mw_hi, mw_lo, p),
+                  "conv_tc launch");
+  if (rc) return rc;
   return check_cuda(cudaGetLastError(), "conv_tc launch");
 }
 
 int conv_tc_launch(const ConvTcParams& p, const void* a_hi, const void* a_lo, const void* w_hi,
                    const void* w_lo, int wk_total, cudaStream_t stream) {
-  if (p.Cin % BK != 0 || p.Cout % BN != 0 || p.nphase < 1 || p.nphase > 4 || p.rows <= 0) {
+  // the stated limit (DESIGN.md §1) stays Cin % 64, although the kernel only needs Cin % BK
+  if (p.Cin % 64 != 0 || p.Cout % BN != 0 || p.nphase < 1 || p.nphase > 4 || p.rows <= 0) {
     set_last_error("conv_tc: unsupported shape Cin=%d Cout=%d nphase=%d rows=%d", p.Cin, p.Cout,
                    p.nphase, p.rows);
     return RW_ERR_BAD_ARG;

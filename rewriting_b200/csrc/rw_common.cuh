@@ -90,6 +90,43 @@ __device__ __forceinline__ void named_bar_sync(int id, int count) {
 }
 
 // ---------------------------------------------------------------------------
+// thread-block clusters
+// ---------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;\n" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ uint32_t cluster_id_x() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%clusterid.x;\n" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ uint32_t num_clusters_x() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%nclusterid.x;\n" : "=r"(r));
+  return r;
+}
+// every thread of every CTA of the cluster; orders shared-memory writes (and mbarrier inits)
+// before it against accesses from the other CTAs after it
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;\nbarrier.cluster.wait.acquire;\n" ::: "memory");
+}
+// the shared::cluster address of the same variable in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t mapa_shared(const void* p, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;\n" : "=r"(r) : "r"(smem_u32(p)), "r"(rank));
+  return r;
+}
+// arrive on an mbarrier of any CTA of the cluster.  Default (.cta) release semantics: the
+// ".release.cluster" form compiles to a GPU-wide memory barrier before every arrive, which halves
+// the throughput of a pipeline that releases a stage per k-block; a consumer that only read the
+// stage through wgmma (completed by wgmma.wait_group) has nothing to publish
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];\n" ::"r"(cluster_addr) : "memory");
+}
+
+// ---------------------------------------------------------------------------
 // per-warpgroup register reallocation (every thread of the warpgroup executes it)
 // ---------------------------------------------------------------------------
 template <uint32_t N>
@@ -113,6 +150,18 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes"
       " [%0], [%1, {%3, %4}], [%2];\n" ::"r"(smem_u32(smem_dst)),
       "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c_inner), "r"(c_outer)
+      : "memory");
+}
+// the same box into the same shared-memory offset of every CTA in `cta_mask`; each destination
+// CTA's mbarrier at the offset of `bar` receives the bytes
+__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUtensorMap* m,
+                                                      uint64_t* bar, int32_t c_inner,
+                                                      int32_t c_outer, uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4}], [%2], %5;\n" ::"r"(smem_u32(smem_dst)),
+      "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c_inner), "r"(c_outer),
+      "h"(cta_mask)
       : "memory");
 }
 
@@ -203,6 +252,10 @@ __device__ __forceinline__ void split_bf16(float x, __nv_bfloat16& hi, __nv_bflo
 // ---------------------------------------------------------------------------
 int make_tmap_2d_bf16(CUtensorMap* out, const void* base, uint64_t inner, uint64_t outer,
                       uint64_t row_stride_bytes, uint32_t box_inner, uint32_t box_outer);
+// rank 2..5, optional element strides; swizzle 0 = none, 1 = 32 B, 2 = 128 B, 3 = 64 B
+int make_tmap_nd_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
+                      const uint64_t* strides_bytes, const uint32_t* box, const uint32_t* estrides,
+                      int swizzle);
 
 int device_sm_count();
 
