@@ -312,6 +312,17 @@ int rw_debug_upconv_profile(const void* kp_hi, const void* kp_lo, const void* wt
                             const float* bias, const float* next_scale, void* next_hi, void* next_lo,
                             int B, int Cin, int Cout, int H, int W, long long* prof_out,
                             rw_stream_t stream);
+/* rw_modconv_fwd_fused on conv_tc's clock()-instrumented variant: prof_out[grid][8 consumer
+ * warps][8] = cycles in {waiting on full barriers, issuing the main loop's MMAs (up to the wgmma
+ * wait that lets a stage go), chunk drains + promotion, epilogue}, the tile count, the cycles from
+ * the first tile to the end, and two zeros; grid <= the SM count */
+int rw_debug_conv_profile(const void* kp_hi, const void* kp_lo, const void* wt_hi,
+                          const void* wt_lo, const float* scale_bo, const float* noise,
+                          long long noise_bstride, const float* noise_w, const float* bias, int act,
+                          int B, int Cin, int Cout, int H, int W, float* out,
+                          const float* next_scale, void* next_hi, void* next_lo,
+                          const float* rgb_w, float* rgb_part, long long* prof_out,
+                          rw_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -69,6 +69,9 @@ SIGNATURES = {
                                     c_int, c_p, c_p]),
     'rw_debug_upconv_profile': (c_int, [c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_ll, c_p, c_p, c_p, c_p,
                                         c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p]),
+    'rw_debug_conv_profile': (c_int, [c_p, c_p, c_p, c_p, c_p, c_p, c_ll, c_p, c_p, c_int,
+                                      c_int, c_int, c_int, c_int, c_int, c_p, c_p, c_p, c_p,
+                                      c_p, c_p, c_p, c_p]),
     'rw_blur_up_fused': (c_int, [c_p, c_int, c_int, c_int, c_int, c_p, c_p, c_ll, c_p, c_p,
                                  c_int, c_p, c_p, c_p, c_p, c_p]),
     'rw_styles': (c_int, [c_p, c_int, c_int, c_int, c_f, c_int, c_p, c_p, c_p, c_p, c_p, c_p]),

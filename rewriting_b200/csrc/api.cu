@@ -389,12 +389,13 @@ int rw_nearest_up2(const float* x, long long planes, int H, int W, float* out, r
   return nearest_up2_launch(x, planes, H, W, out, stream);
 }
 
-int rw_modconv_fwd_fused(const void* kp_hi, const void* kp_lo, const void* wt_hi,
-                         const void* wt_lo, const float* scale_bo, const float* noise,
-                         long long noise_bstride, const float* noise_w, const float* bias, int act,
-                         int B, int Cin, int Cout, int H, int W, float* out,
-                         const float* next_scale, void* next_hi, void* next_lo,
-                         const float* rgb_w, float* rgb_part, rw_stream_t stream) {
+static int modconv_fused_impl(const void* kp_hi, const void* kp_lo, const void* wt_hi,
+                              const void* wt_lo, const float* scale_bo, const float* noise,
+                              long long noise_bstride, const float* noise_w, const float* bias,
+                              int act, int B, int Cin, int Cout, int H, int W, float* out,
+                              const float* next_scale, void* next_hi, void* next_lo,
+                              const float* rgb_w, float* rgb_part, long long* prof_out,
+                              rw_stream_t stream) {
   if (!kp_hi || !kp_lo || !wt_hi || !wt_lo || B < 1 || (noise && !noise_w) ||
       ((next_hi != nullptr) != (next_lo != nullptr)) || (next_hi && !next_scale) ||
       ((rgb_w != nullptr) != (rgb_part != nullptr)) || (!out && !next_hi && !rgb_part)) {
@@ -416,7 +417,35 @@ int rw_modconv_fwd_fused(const void* kp_hi, const void* kp_lo, const void* wt_hi
   p.next_scale = next_scale;
   p.rgb_w = rgb_w;
   p.rgb_part = rgb_part;
+  p.debug_prof = prof_out;
   return conv_tc_launch(p, kp_hi, kp_lo, wt_hi, wt_lo, 9 * Cin, stream);
+}
+
+int rw_modconv_fwd_fused(const void* kp_hi, const void* kp_lo, const void* wt_hi,
+                         const void* wt_lo, const float* scale_bo, const float* noise,
+                         long long noise_bstride, const float* noise_w, const float* bias, int act,
+                         int B, int Cin, int Cout, int H, int W, float* out,
+                         const float* next_scale, void* next_hi, void* next_lo,
+                         const float* rgb_w, float* rgb_part, rw_stream_t stream) {
+  return modconv_fused_impl(kp_hi, kp_lo, wt_hi, wt_lo, scale_bo, noise, noise_bstride, noise_w,
+                            bias, act, B, Cin, Cout, H, W, out, next_scale, next_hi, next_lo, rgb_w,
+                            rgb_part, nullptr, stream);
+}
+
+int rw_debug_conv_profile(const void* kp_hi, const void* kp_lo, const void* wt_hi,
+                          const void* wt_lo, const float* scale_bo, const float* noise,
+                          long long noise_bstride, const float* noise_w, const float* bias, int act,
+                          int B, int Cin, int Cout, int H, int W, float* out,
+                          const float* next_scale, void* next_hi, void* next_lo,
+                          const float* rgb_w, float* rgb_part, long long* prof_out,
+                          rw_stream_t stream) {
+  if (!prof_out) {
+    set_last_error("rw_debug_conv_profile: prof_out is null");
+    return RW_ERR_BAD_ARG;
+  }
+  return modconv_fused_impl(kp_hi, kp_lo, wt_hi, wt_lo, scale_bo, noise, noise_bstride, noise_w,
+                            bias, act, B, Cin, Cout, H, W, out, next_scale, next_hi, next_lo, rgb_w,
+                            rgb_part, prof_out, stream);
 }
 
 int rw_modconv_up_fused(const void* kp_hi, const void* kp_lo, const void* wt_hi, const void* wt_lo,

@@ -87,7 +87,9 @@ __device__ __forceinline__ void decode_tile(int tile, int nphase, int nsched, in
 //          layer's planes, ToRGB partials — every feature a run-time switch).
 // EPI = 1: lean epilogue — optional per-(b,o) scale and the store, nothing else.  The up-path
 //          conv_transpose phases, dgrad and the plain row-GEMM use it.
-template <int EPI>
+// PROF = true: bring-up variant that accumulates, per consumer warp, the cycles of each phase of a
+// tile (tools/prof_conv.py) into p.debug_prof; the product launches PROF = false.
+template <int EPI, bool PROF>
 __global__ void __launch_bounds__(kNumThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
                const __grid_constant__ CUtensorMap map_a_lo,
@@ -147,6 +149,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
         for (int r = 0; r < kCluster; ++r) mbar_arrive_cluster(mapa_shared(&bars->empty[s], r));
       }
     };
+    // PROF: wait full, MMA issue, chunk drain + promotion, epilogue, tiles, total
+    // (32-bit clock differences: a launch runs for far fewer than 2^32 cycles)
+    auto clk = [] { return static_cast<uint32_t>(clock()); };
+    uint32_t prof[6] = {0, 0, 0, 0, 0, 0};
+    uint32_t tp0 = 0, tp1 = 0;
+    if constexpr (PROF) prof[5] = 0u - clk();
     int stage = 0;
     uint32_t phase = 0;
     for (int unit = first_unit; unit < num_units; unit += nsched) {
@@ -166,7 +174,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
         // issued and the group that read it has completed
         int held = -1;
         for (int kb = kb0; kb < kb_end; ++kb) {
+          if constexpr (PROF) tp0 = clk();
           mbar_wait(&bars->full[stage], phase);
+          if constexpr (PROF) { tp1 = clk(); prof[0] += tp1 - tp0; }
           const uint32_t sa = smem_u32(smem + stage * S::kStageBytes);
           const uint64_t da_hi = make_smem_desc(sa + wg * (S::kABytes / 2), 16, 512, 2);
           const uint64_t da_lo = make_smem_desc(sa + S::kABytes + wg * (S::kABytes / 2), 16, 512, 2);
@@ -186,14 +196,18 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
           if (held >= 0) release(held);
           held = stage;
           if (++stage == kStages) { stage = 0; phase ^= 1u; }
+          if constexpr (PROF) prof[1] += clk() - tp1;
         }
+        if constexpr (PROF) tp0 = clk();
         // the chunk is complete before it is added; its last stage is released here, so the
         // producer refills the ring while the epilogue runs
         wgmma_wait<0>();
         release(held);
 #pragma unroll
         for (int j = 0; j < 64; ++j) acc[j] += d[j];
+        if constexpr (PROF) prof[2] += clk() - tp0;
       }
+      if constexpr (PROF) tp0 = clk();
 
       // ---- fused epilogue: rows r = m0 + 64 wg + 16 (warp % 4) + g + 8 i, columns 8 j + 2 c + e ----
       // (the thread's row offset is formed here from a fresh %tid.x: hoisted above the main loop,
@@ -239,24 +253,50 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
             nz = __ldg(p.noise_w) * __ldg(p.noise + static_cast<size_t>(b) * p.noise_bstride +
                                           static_cast<size_t>(yy) * Wv + xx);
           const float act_gain = p.act_gain != 0.f ? p.act_gain : 1.4142135623730951f;
+          // one pass over the row's 32 values per term, so that a term that is off costs no
+          // instructions: in a single loop ptxas computes the strided store's addresses for every
+          // element, although the generator's fast path stores no fp32 output.  Per-row base
+          // pointers give the loads constant offsets.  Each element sees scale, noise, bias,
+          // activation in that order.
+          if (scl) {
+            const float* sc = scl + n0 + 2 * c;
+#pragma unroll
+            for (int j = 0; j < 16; ++j)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) acc[4 * j + 2 * i + e] *= __ldg(sc + 8 * j + e);
+          }
 #pragma unroll
           for (int j = 0; j < 16; ++j)
 #pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const int o = n0 + 8 * j + 2 * c + e;
-              float t = acc[4 * j + 2 * i + e];
-              if (scl) t *= __ldg(scl + o);
-              t += nz;
-              if (p.bias) t += __ldg(p.bias + o);
-              if (p.act) t = (t > 0.f ? t : 0.2f * t) * act_gain;
-              acc[4 * j + 2 * i + e] = t;
-              if (outp) outp[static_cast<size_t>(o) * p.out_sc] = t;
+            for (int e = 0; e < 2; ++e) acc[4 * j + 2 * i + e] += nz;
+          if (p.bias) {
+            const float* bi = p.bias + n0 + 2 * c;
+#pragma unroll
+            for (int j = 0; j < 16; ++j)
+#pragma unroll
+              for (int e = 0; e < 2; ++e) acc[4 * j + 2 * i + e] += __ldg(bi + 8 * j + e);
+          }
+          if (p.act) {
+#pragma unroll
+            for (int j = 0; j < 32; ++j) {
+              float& t = acc[4 * (j >> 1) + 2 * i + (j & 1)];
+              t = (t > 0.f ? t : 0.2f * t) * act_gain;
             }
+          }
+          if (outp) {
+#pragma unroll
+            for (int j = 0; j < 16; ++j)
+#pragma unroll
+              for (int e = 0; e < 2; ++e)
+                outp[static_cast<size_t>(n0 + 8 * j + 2 * c + e) * p.out_sc] = acc[4 * j + 2 * i + e];
+          }
         }
         if (EPI == 0 && p.rgb_w != nullptr) {
           // one partial per 64-channel group: rgb_part[(n_tile*2 + half)][b][c][y*Wv+x]; the four
           // lanes of a row hold 16 of the group's channels each
-          const float* rw0 = p.rgb_w + (static_cast<size_t>(valid ? b : 0) * 3) * p.Cout;
+          const float* rw0 = p.rgb_w + (static_cast<size_t>(valid ? b : 0) * 3) * p.Cout + n0 + 2 * c;
+          const float* rw1 = rw0 + p.Cout;
+          const float* rw2 = rw1 + p.Cout;
 #pragma unroll
           for (int half = 0; half < 2; ++half) {
             float r0 = 0.f, r1 = 0.f, r2 = 0.f;
@@ -265,11 +305,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
               for (int j = 8 * half; j < 8 * half + 8; ++j)
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
-                  const int o = n0 + 8 * j + 2 * c + e;
                   const float t = acc[4 * j + 2 * i + e];
-                  r0 = fmaf(__ldg(rw0 + o), t, r0);
-                  r1 = fmaf(__ldg(rw0 + p.Cout + o), t, r1);
-                  r2 = fmaf(__ldg(rw0 + 2 * p.Cout + o), t, r2);
+                  r0 = fmaf(__ldg(rw0 + 8 * j + e), t, r0);
+                  r1 = fmaf(__ldg(rw1 + 8 * j + e), t, r1);
+                  r2 = fmaf(__ldg(rw2 + 8 * j + e), t, r2);
                 }
             }
 #pragma unroll
@@ -315,6 +354,15 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
             nl[4 * j] = *reinterpret_cast<const uint32_t*>(&ll);
           }
         }
+      }
+      if constexpr (PROF) { prof[3] += clk() - tp0; prof[4] += 1; }
+    }
+    if constexpr (PROF) {
+      prof[5] += clk();
+      if (lane == 0) {
+        long long* dst = p.debug_prof + (static_cast<size_t>(blockIdx.x) * 8 + warp) * 8;
+#pragma unroll
+        for (int i = 0; i < 8; ++i) dst[i] = i < 6 ? prof[i] : 0;
       }
     }
   } else {
@@ -362,7 +410,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
 
 }  // namespace
 
-template <int EPI>
+template <int EPI, bool PROF>
 static int conv_tc_launch_epi(const ConvTcParams& p, const void* a_hi, const void* a_lo,
                               const void* w_hi, const void* w_lo, int wk_total,
                               cudaStream_t stream) {
@@ -394,12 +442,12 @@ static int conv_tc_launch_epi(const ConvTcParams& p, const void* a_hi, const voi
   // SMs cannot host a whole cluster, so this is fewer than SMs / kCluster)
   static int max_clusters = 0;
   if (max_clusters == 0) {
-    rc = check_cuda(cudaFuncSetAttribute(conv_tc_kernel<EPI>,
+    rc = check_cuda(cudaFuncSetAttribute(conv_tc_kernel<EPI, PROF>,
                                          cudaFuncAttributeMaxDynamicSharedMemorySize, ConvSmem::kTotal),
                     "conv_tc smem attr");
     if (rc) return rc;
     cfg.gridDim = dim3(kCluster * (device_sm_count() / kCluster));
-    rc = check_cuda(cudaOccupancyMaxActiveClusters(&max_clusters, conv_tc_kernel<EPI>, &cfg),
+    rc = check_cuda(cudaOccupancyMaxActiveClusters(&max_clusters, conv_tc_kernel<EPI, PROF>, &cfg),
                     "conv_tc cluster occupancy");
     if (rc) return rc;
     if (max_clusters < 1) {
@@ -412,7 +460,7 @@ static int conv_tc_launch_epi(const ConvTcParams& p, const void* a_hi, const voi
   const int num_units = (m_tiles + kCluster - 1) / kCluster * n_tiles * p.nphase;
   const int clusters = max_clusters < num_units ? max_clusters : num_units;
   cfg.gridDim = dim3(kCluster * clusters);
-  rc = check_cuda(cudaLaunchKernelEx(&cfg, conv_tc_kernel<EPI>, ma_hi, ma_lo, mw_hi, mw_lo, p),
+  rc = check_cuda(cudaLaunchKernelEx(&cfg, conv_tc_kernel<EPI, PROF>, ma_hi, ma_lo, mw_hi, mw_lo, p),
                   "conv_tc launch");
   if (rc) return rc;
   return check_cuda(cudaGetLastError(), "conv_tc launch");
@@ -434,8 +482,9 @@ int conv_tc_launch(const ConvTcParams& p, const void* a_hi, const void* a_lo, co
   // lean epilogue when only the optional scale and the store are asked for
   const bool lean = !p.noise && !p.bias && !p.act && !p.rgb_w && !p.rgb_part && !p.next_hi &&
                     p.out != nullptr && (reinterpret_cast<uintptr_t>(p.scale_bo) & 7u) == 0;
-  if (lean) return conv_tc_launch_epi<1>(p, a_hi, a_lo, w_hi, w_lo, wk_total, stream);
-  return conv_tc_launch_epi<0>(p, a_hi, a_lo, w_hi, w_lo, wk_total, stream);
+  if (p.debug_prof) return conv_tc_launch_epi<0, true>(p, a_hi, a_lo, w_hi, w_lo, wk_total, stream);
+  if (lean) return conv_tc_launch_epi<1, false>(p, a_hi, a_lo, w_hi, w_lo, wk_total, stream);
+  return conv_tc_launch_epi<0, false>(p, a_hi, a_lo, w_hi, w_lo, wk_total, stream);
 }
 
 }  // namespace rw

@@ -50,6 +50,9 @@ struct ConvTcParams {
   //   rgb_part[nt][b][c][y*Wv+x] = sum_{o in tile} rgb_w[b][c][o] * y[b,o,y,x]
   float* rgb_part;
   const float* rgb_w;        // [B, 3, Cout] modulated 1x1 weights
+  // non-null: launch the clock()-instrumented variant, which writes per-phase cycles of every
+  // consumer warp to debug_prof[grid][8][8] (rw_debug_conv_profile)
+  long long* debug_prof;
 };
 
 int conv_tc_launch(const ConvTcParams& p, const void* a_hi, const void* a_lo, const void* w_hi,
