@@ -30,7 +30,8 @@
  *       utils/runningstats.py:1086-1097,1181-1190                          -> rw_split_rows,
  *                                                                              rw_second_moment_accum
  *   projected_conv(weight, direction)  rewrite/ganrewrite.py:806-813       -> rw_project_rank
- *   ProgressiveGanRewriter.insert hot loop rewrite/ganrewrite.py:279-294   -> rw_insert_loop
+ *   ProgressiveGanRewriter.insert hot loop rewrite/ganrewrite.py:279-294   -> rw_insert_loop,
+ *                                                                              rw_insert_loop_wide
  *
  * Layout vocabulary
  *   key planes  : the style-modulated key k = style*x as two bf16 planes (hi, lo; k ~= hi+lo)
@@ -265,6 +266,16 @@ typedef struct rw_insert_args {
   double beta2_exact;      /* 1 - beta**step from (0 -> the float fields above, widened) */
 } rw_insert_args;
 int rw_insert_loop(const rw_insert_args* args, rw_stream_t stream);
+/* The same loop for key crops beyond rw_insert_loop's limits (w > 16, B*h*w > 4096 or a shared-
+ * memory overflow): whole-map goals and wide selections, all iterations in one launch, same
+ * fp32 arithmetic.  t and g*demod go to `workspace`, at least rw_insert_wide_workspace_bytes(Cout,
+ * B, h, w) bytes (2 fp32 planes [Cout rounded up to 4][B*h*w]; 16.8 MB at 512 x 64 x 64), which the
+ * call owns until it completes on `stream`.  Needs 1 <= B <= 4, Cin % 32 == 0, 128 <= Cin <= 512,
+ * 1 <= rank <= 32; an unsupported shape or a short workspace returns RW_STATUS_BAD_ARG before
+ * anything is launched. */
+size_t rw_insert_wide_workspace_bytes(int Cout, int B, int h, int w);
+int rw_insert_loop_wide(const rw_insert_args* args, void* workspace, size_t workspace_bytes,
+                        rw_stream_t stream);
 
 /* out[rows][N] = A[rows][K] . W[N][K]^T on the tensor-core row-GEMM (3-term split bf16 planes from
  * rw_split_rows; K % 64 == 0, N % 128 == 0): the key algebra between key capture and the

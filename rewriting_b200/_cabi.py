@@ -105,6 +105,8 @@ SIGNATURES = {
     'rw_style_grad_finish': (c_int, [c_p, c_p, c_p, c_p, c_p, c_int, c_int, c_int, c_p, c_p]),
     'rw_project_rank': (c_int, [c_p, c_p, c_p, c_int, c_int, c_int, c_int, c_f, c_p, c_p]),
     'rw_insert_loop': (c_int, [ctypes.POINTER(InsertArgs), c_p]),
+    'rw_insert_wide_workspace_bytes': (c_sz, [c_int, c_int, c_int, c_int]),
+    'rw_insert_loop_wide': (c_int, [ctypes.POINTER(InsertArgs), c_p, c_sz, c_p]),
     'rw_debug_rowgemm': (c_int, [c_p, c_p, c_p, c_p, c_int, c_int, c_int, c_p, c_p]),
     'rw_debug_colgemm': (c_int, [c_p, c_p, c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_p,
                                  c_p, c_sz, c_p]),

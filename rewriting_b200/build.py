@@ -11,7 +11,8 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'librw_b200.so')
-SOURCES = ['api.cu', 'conv_tc.cu', 'upconv_tc.cu', 'gram_tc.cu', 'simt.cu', 'bwd.cu', 'rewrite.cu']
+SOURCES = ['api.cu', 'conv_tc.cu', 'upconv_tc.cu', 'gram_tc.cu', 'simt.cu', 'bwd.cu', 'rewrite.cu',
+           'insert_wide.cu']
 NVCC_FLAGS = [
     '-gencode', 'arch=compute_90a,code=sm_90a',
     '-lineinfo', '-O3', '-std=c++17',

@@ -848,13 +848,12 @@ int rw_project_rank(const float* w, const float* base, const float* d, int rank,
   return project_rank_launch_signed(w, base, d, rank, Cout, Cin, taps, sign, out, stream);
 }
 
-int rw_insert_loop(const rw_insert_args* a, rw_stream_t stream) {
+static int insert_params(const rw_insert_args* a, const char* who, InsertLoopParams& p) {
   if (!a || !a->W || !a->m || !a->v || !a->d || !a->key_cl || (!a->style && !a->plain_conv) ||
       !a->target || !a->loss_out || (a->has_noise_act && !a->bias)) {
-    set_last_error("rw_insert_loop: bad argument");
+    set_last_error("%s: bad argument", who);
     return RW_ERR_BAD_ARG;
   }
-  InsertLoopParams p;
   memset(&p, 0, sizeof(p));
   p.W = a->W; p.m = a->m; p.v = a->v; p.w_ortho = a->w_ortho; p.d = a->d; p.rank = a->rank;
   p.key = a->key_cl; p.style = a->style; p.target = a->target; p.noise = a->noise;
@@ -871,7 +870,26 @@ int rw_insert_loop(const rw_insert_args* a, rw_stream_t stream) {
   p.one_minus_beta2 = a->one_minus_beta2 != 0.f ? a->one_minus_beta2 : 1.0f - a->beta2;
   p.beta1_exact = a->beta1_exact != 0.0 ? a->beta1_exact : static_cast<double>(a->beta1);
   p.beta2_exact = a->beta2_exact != 0.0 ? a->beta2_exact : static_cast<double>(a->beta2);
+  return 0;
+}
+
+int rw_insert_loop(const rw_insert_args* a, rw_stream_t stream) {
+  InsertLoopParams p;
+  int rc = insert_params(a, "rw_insert_loop", p);
+  if (rc) return rc;
   return insert_loop_launch(p, stream);
+}
+
+size_t rw_insert_wide_workspace_bytes(int Cout, int B, int h, int w) {
+  return insert_wide_workspace_bytes(Cout, B, h, w);
+}
+
+int rw_insert_loop_wide(const rw_insert_args* a, void* workspace, size_t workspace_bytes,
+                        rw_stream_t stream) {
+  InsertLoopParams p;
+  int rc = insert_params(a, "rw_insert_loop_wide", p);
+  if (rc) return rc;
+  return insert_wide_launch(p, workspace, workspace_bytes, stream);
 }
 
 int rw_debug_rowgemm(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo,

@@ -209,5 +209,9 @@ struct InsertLoopParams {
   double beta1_exact, beta2_exact;          // betas for the bias corrections (python doubles)
 };
 int insert_loop_launch(const InsertLoopParams& p, cudaStream_t stream);
+// wide-key variant (csrc/insert_wide.cu): any crop width, t and g*demod in `workspace`
+size_t insert_wide_workspace_bytes(int Cout, int B, int h, int w);
+int insert_wide_launch(const InsertLoopParams& p, void* workspace, size_t workspace_bytes,
+                       cudaStream_t stream);
 
 }  // namespace rw

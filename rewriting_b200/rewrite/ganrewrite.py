@@ -41,6 +41,38 @@ from ..utils.stylegan2 import models as sg2
 (all_obs, all_weight, all_CinvK, all_kCinvK, e_val, e_vec, kbasis, row_dirs, q) = (None,) * 9
 
 FUSED_CHUNK = 64     # iterations per fused launch when a callback wants per-step losses
+WIDE_MAX_WORK = 512 * 32 * 32   # rw_insert_loop_wide routing limit, see fused_insert_kernel
+
+
+def fused_insert_kernel(B, Cin, Cout, h, w):
+    """The one-launch insert kernel for a key crop [B, Cin, h, w] -> [B, Cout, h, w], or None to
+    run the loop through autograd.  Small crops keep rw_insert_loop (t and g in shared memory,
+    register tile up to 16 columns).  Larger ones with 128 <= Cin <= 512 take rw_insert_loop_wide
+    (t and g in an L2-resident workspace, 16-column chunks) while wide_insert_work() is at most
+    WIDE_MAX_WORK: the largest size measured no slower per iteration than the autograd loop on an
+    H100 (DESIGN.md §6).  Beyond it the tensor-core autograd loop is faster."""
+    if B > 4 or Cin % 32 != 0:
+        return None
+    # shared memory of rw_insert_loop (csrc/rewrite.cu insert_loop_launch): 4 weight rows +
+    # 4 gradient rows + 8 crop-sized vectors + small tables, within 225 KB
+    if w <= 16 and B * h * w <= 4096 and (8 * Cin * 9 + 8 * B * h * w + 1440) * 4 <= 225 * 1024:
+        return 'rw_insert_loop'
+    if 128 <= Cin <= 512 and Cout <= 512 and wide_insert_work(B, Cin, h, w) <= WIDE_MAX_WORK:
+        return 'rw_insert_loop_wide'
+    return None
+
+
+def wide_insert_work(B, Cin, h, w):
+    """What one CTA of rw_insert_loop_wide spends per iteration, in units that make its time
+    proportional across shapes: key pixels (columns rounded up to whole 16-column chunks) times
+    max(Cin, 256).  The forward pass spreads rows over the CTA's 8 warps and costs Cin per pixel;
+    the weight gradient gives one warp to each 32 input channels, so below 256 channels it leaves
+    warps idle and takes as long as at 256.  A CTA owns 4 output channels and there is at most one
+    CTA per SM, so up to Cout = 512 the time does not depend on Cout."""
+    return max(Cin, 256) * B * h * (-(-w // 16) * 16)
+    return None
+
+
 _DCONV_RE = _re.compile(r'^layer(\d+)\.(?:sconv|conv)\.mconv\.dconv$')
 
 
@@ -503,9 +535,10 @@ class ProgressiveGanRewriter(object):
 
     # -- fused path ------------------------------------------------------------------------
     def _fused_plan(self, key, val, context):
-        """Returns (conv, noise_module, act_module, plain) if the target model is the canonical
-        [dconv (, noise, activate)] chain of a SeqStyleGAN2 layer — or the single plain
-        `layerN.conv` of a ProgGAN generator (plain = True) — on a small key, else None."""
+        """Returns (kernel, conv, noise_module, act_module, plain, key) if the target model is the
+        canonical [dconv (, noise, activate)] chain of a SeqStyleGAN2 layer — or the single plain
+        `layerN.conv` of a ProgGAN generator (plain = True) — on a key `fused_insert_kernel`
+        routes to a fused kernel, else None."""
         if context is None:
             return None
         if any('forward' in m.__dict__ for m in self.target_model.modules()):
@@ -555,18 +588,15 @@ class ProgressiveGanRewriter(object):
         if not k.is_cuda or k.dtype != torch.float32:
             return None
         B, Cin, h, w = k.shape
-        if B > 4 or w > 16 or B * h * w > 4096 or Cin % 32 != 0 or context.shape[0] > 32:
-            return None
-        # shared memory of rw_insert_loop (csrc/rewrite.cu insert_loop_launch): 4 weight rows +
-        # 4 gradient rows + 8 crop-sized vectors + small tables, within 225 KB
-        if (8 * Cin * 9 + 8 * B * h * w + 1440) * 4 > 225 * 1024:
+        kernel = fused_insert_kernel(B, Cin, cout, h, w)
+        if kernel is None or context.shape[0] > 32:
             return None
         if tuple(self.target_acts(val).shape) != (B, cout, h, w):
             return None
-        return dconv, nz, act, plain, k
+        return kernel, dconv, nz, act, plain, k
 
     def _insert_fused(self, plan, key, val, context, update_callback, niter, piter, lr):
-        dconv, nz, act, plain, k = plan
+        kernel, dconv, nz, act, plain, k = plan
         weight = self.target_weights()
         assert weight is dconv.weight
         B, Cin, h, w = k.shape
@@ -612,12 +642,18 @@ class ProgressiveGanRewriter(object):
             args.plain_conv = 1 if plain else 0
             args.niter_total, args.piter = niter, piter
             args.project_gradient = 1 if self.low_rank_gradient else 0
+            launch = (ctypes.byref(args),)
+            if kernel == 'rw_insert_loop_wide':
+                # per-pixel t and g*demod of every channel: [Cout][B*h*w] x 2 fp32 scratch
+                nbytes = _cabi.load().rw_insert_wide_workspace_bytes(Cout, B, h, w)
+                workspace = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+                launch += (workspace.data_ptr(), nbytes)
             it0 = 0
             stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
             while it0 < niter:
                 n = min(chunk, niter - it0)
                 args.it0, args.nsteps = it0, n
-                _cabi.call('rw_insert_loop', ctypes.byref(args), stream)
+                _cabi.call(kernel, *launch, stream)
                 _bump_version(weight)
                 if update_callback is not None:
                     losses = loss_buf[:n].sum(dim=1) / numel
