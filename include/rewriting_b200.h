@@ -32,6 +32,8 @@
  *   projected_conv(weight, direction)  rewrite/ganrewrite.py:806-813       -> rw_project_rank
  *   ProgressiveGanRewriter.insert hot loop rewrite/ganrewrite.py:279-294   -> rw_insert_loop,
  *                                                                              rw_insert_loop_wide
+ *   ProgressiveGanRewriter.linear_insert   rewrite/ganrewrite.py:201-252   -> rw_linear_insert_loop,
+ *                                                                              rw_linear_insert_loop_wide
  *
  * Layout vocabulary
  *   key planes  : the style-modulated key k = style*x as two bf16 planes (hi, lo; k ~= hi+lo)
@@ -276,6 +278,29 @@ int rw_insert_loop(const rw_insert_args* args, rw_stream_t stream);
 size_t rw_insert_wide_workspace_bytes(int Cout, int B, int h, int w);
 int rw_insert_loop_wide(const rw_insert_args* args, void* workspace, size_t workspace_bytes,
                         rw_stream_t stream);
+
+/* linear_insert (reference rewrite/ganrewrite.py:201-252): the same loop with Adam on Λ in
+ * W = W0 + Λ d instead of on W.  Per iteration: forward, L1 gradient and dW exactly as above, then
+ * dΛ[o,r,t] = Σ_i dW[o,i,t] d[r,i], one Adam step on Λ, and W = W0 + Λ d with the product and the
+ * sum rounded separately (a rank-1 rebuild equals the reference's `W0 + einsum(...)` bit for bit).
+ * There is no projection: base->w_ortho must be NULL and base->project_gradient and
+ * base->plain_conv 0; base->m, base->v and base->piter are unused.  base->W is not read; at the end
+ * of the call it holds W0 + Λ d, and lam / lam_m / lam_v hold the state to continue from
+ * (it0 = the next iteration).  W0 must not alias base->W.  Shape limits are those of
+ * rw_insert_loop / rw_insert_loop_wide (rw_insert_loop needs 13.5 KB more shared memory for the
+ * Λ state).  A wrong struct_size, a NULL W0 / lam / moment buffer or a set w_ortho,
+ * project_gradient or plain_conv returns RW_STATUS_BAD_ARG before anything is launched. */
+typedef struct rw_linear_insert_args {
+  size_t struct_size;            /* sizeof(rw_linear_insert_args), checked */
+  const rw_insert_args* base;    /* shapes, key_cl, style, target, noise/bias, Adam constants,
+                                    it0/nsteps/niter_total, loss_out; base->W receives W0 + Λd */
+  const float* W0;               /* [Cout,Cin,3,3] original weight, read only */
+  float* lam;                    /* [Cout,rank,3,3] Λ (zero before it0 = 0), updated in place */
+  float* lam_m; float* lam_v;    /* Adam state of Λ, same shape */
+} rw_linear_insert_args;
+int rw_linear_insert_loop(const rw_linear_insert_args* args, rw_stream_t stream);
+int rw_linear_insert_loop_wide(const rw_linear_insert_args* args, void* workspace,
+                               size_t workspace_bytes, rw_stream_t stream);
 
 /* out[rows][N] = A[rows][K] . W[N][K]^T on the tensor-core row-GEMM (3-term split bf16 planes from
  * rw_split_rows; K % 64 == 0, N % 128 == 0): the key algebra between key capture and the

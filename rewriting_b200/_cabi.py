@@ -37,6 +37,14 @@ class InsertArgs(ctypes.Structure):
     ]
 
 
+class LinearInsertArgs(ctypes.Structure):
+    """Mirror of `rw_linear_insert_args` (struct_size must be set to ctypes.sizeof of it)."""
+    _fields_ = [
+        ('struct_size', c_sz), ('base', ctypes.POINTER(InsertArgs)),
+        ('W0', c_p), ('lam', c_p), ('lam_m', c_p), ('lam_v', c_p),
+    ]
+
+
 # name -> (restype, argtypes); every symbol include/rewriting_b200.h declares
 SIGNATURES = {
     'rw_version': (c_int, []),
@@ -107,6 +115,8 @@ SIGNATURES = {
     'rw_insert_loop': (c_int, [ctypes.POINTER(InsertArgs), c_p]),
     'rw_insert_wide_workspace_bytes': (c_sz, [c_int, c_int, c_int, c_int]),
     'rw_insert_loop_wide': (c_int, [ctypes.POINTER(InsertArgs), c_p, c_sz, c_p]),
+    'rw_linear_insert_loop': (c_int, [ctypes.POINTER(LinearInsertArgs), c_p]),
+    'rw_linear_insert_loop_wide': (c_int, [ctypes.POINTER(LinearInsertArgs), c_p, c_sz, c_p]),
     'rw_debug_rowgemm': (c_int, [c_p, c_p, c_p, c_p, c_int, c_int, c_int, c_p, c_p]),
     'rw_debug_colgemm': (c_int, [c_p, c_p, c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_p,
                                  c_p, c_sz, c_p]),

@@ -848,8 +848,10 @@ int rw_project_rank(const float* w, const float* base, const float* d, int rank,
   return project_rank_launch_signed(w, base, d, rank, Cout, Cin, taps, sign, out, stream);
 }
 
-static int insert_params(const rw_insert_args* a, const char* who, InsertLoopParams& p) {
-  if (!a || !a->W || !a->m || !a->v || !a->d || !a->key_cl || (!a->style && !a->plain_conv) ||
+static int insert_params(const rw_insert_args* a, const char* who, InsertLoopParams& p,
+                         bool need_moments = true) {
+  if (!a || !a->W || (need_moments && (!a->m || !a->v)) || !a->d || !a->key_cl ||
+      (!a->style && !a->plain_conv) ||
       !a->target || !a->loss_out || (a->has_noise_act && !a->bias)) {
     set_last_error("%s: bad argument", who);
     return RW_ERR_BAD_ARG;
@@ -890,6 +892,46 @@ int rw_insert_loop_wide(const rw_insert_args* a, void* workspace, size_t workspa
   int rc = insert_params(a, "rw_insert_loop_wide", p);
   if (rc) return rc;
   return insert_wide_launch(p, workspace, workspace_bytes, stream);
+}
+
+// Λ mode: the base arguments without W's Adam moments, plus W0, Λ and Λ's moments.  The reference's
+// linear_insert ignores low_rank_insert / low_rank_gradient and has no plain-conv (4-D weight) form.
+static int linear_insert_params(const rw_linear_insert_args* a, const char* who,
+                                InsertLoopParams& p) {
+  if (!a || a->struct_size != sizeof(rw_linear_insert_args)) {
+    set_last_error("%s: struct_size %zu != %zu", who, a ? a->struct_size : static_cast<size_t>(0),
+                   sizeof(rw_linear_insert_args));
+    return RW_ERR_BAD_ARG;
+  }
+  if (!a->base || !a->W0 || !a->lam || !a->lam_m || !a->lam_v) {
+    set_last_error("%s: NULL base, W0, lam or moment buffer", who);
+    return RW_ERR_BAD_ARG;
+  }
+  const rw_insert_args* b = a->base;
+  if (b->w_ortho != nullptr || b->project_gradient != 0 || b->plain_conv != 0) {
+    set_last_error("%s: w_ortho, project_gradient and plain_conv must be unset for linear_insert", who);
+    return RW_ERR_BAD_ARG;
+  }
+  int rc = insert_params(b, who, p, false);
+  if (rc) return rc;
+  p.m = p.v = nullptr;
+  p.W0 = a->W0; p.lam = a->lam; p.lam_m = a->lam_m; p.lam_v = a->lam_v;
+  return 0;
+}
+
+int rw_linear_insert_loop(const rw_linear_insert_args* a, rw_stream_t stream) {
+  InsertLoopParams p;
+  int rc = linear_insert_params(a, "rw_linear_insert_loop", p);
+  if (rc) return rc;
+  return linear_insert_loop_launch(p, stream);
+}
+
+int rw_linear_insert_loop_wide(const rw_linear_insert_args* a, void* workspace,
+                               size_t workspace_bytes, rw_stream_t stream) {
+  InsertLoopParams p;
+  int rc = linear_insert_params(a, "rw_linear_insert_loop_wide", p);
+  if (rc) return rc;
+  return linear_insert_wide_launch(p, workspace, workspace_bytes, stream);
 }
 
 int rw_debug_rowgemm(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo,

@@ -17,8 +17,11 @@
 //     times.
 // The demodulation, loss, demod-term, projection and Adam phases are insert_loop_kernel's code;
 // they are repeated here rather than shared so that the small-crop kernel stays exactly as it is.
+// kLinear selects the Λ mode (linear_insert), whose update phases both kernels share from
+// csrc/insert_linear.cuh.
 #include "rw_common.cuh"
 #include "rw_kernels.h"
+#include "insert_linear.cuh"
 
 namespace rw {
 
@@ -31,7 +34,10 @@ constexpr int OC = 4;
 constexpr int MW = 16;          // column chunk = register tile width
 constexpr int kMinCin = 128;    // the sizes the tests hold to the oracle
 constexpr int kMaxCin = 512;    // 2 * OC weight rows of Cin*9 floats in shared memory
+constexpr int kMiscFloats = 64 + kWarps * OC * 5;       // demod, coef, loss and G tables
+constexpr int kLamFloats = 3 * OC * kMaxRank * 9;       // Λ mode: Λ, exp_avg, exp_avg_sq
 
+template <bool kLinear>
 __global__ void __launch_bounds__(kThreads, 1)
 insert_wide_kernel(const InsertLoopParams p, const float* __restrict__ kpT, float* tG, float* gdG) {
   extern __shared__ float sm[];
@@ -48,6 +54,9 @@ insert_wide_kernel(const InsertLoopParams p, const float* __restrict__ kpT, floa
   float* coefS = misc + 16;            // [OC][4]
   float* lossS = misc + 32;            // [kWarps][OC]
   float* GS = misc + 64;               // [kWarps][OC][4]
+  float* lamS = misc + kMiscFloats;    // Λ mode: [OC][kMaxRank*9] Λ, then exp_avg, exp_avg_sq
+  float* lamMS = lamS + OC * kMaxRank * 9;
+  float* lamVS = lamMS + OC * kMaxRank * 9;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const bool plain = p.plain_conv != 0;  // nn.Conv2d target: no demodulation, no weight scale
@@ -59,9 +68,15 @@ insert_wide_kernel(const InsertLoopParams p, const float* __restrict__ kpT, floa
     const int noc = (p.Cout - o0 < OC) ? p.Cout - o0 : OC;
     float* tS = tG + static_cast<size_t>(o0) * P;     // this CTA's rows of the scratch
     float* gdS = gdG + static_cast<size_t>(o0) * P;
-    for (int i = threadIdx.x; i < OC * nW; i += kThreads) {
-      const int oc = i / nW;
-      Ws[i] = (oc < noc) ? p.W[static_cast<size_t>(o0) * nW + i] : 0.f;
+    if constexpr (kLinear) {
+      linear_mode::load_state<OC, kMaxRank * 9, kThreads>(p, o0, noc, lamS, lamMS, lamVS);
+      __syncthreads();
+      linear_mode::rebuild_weights<OC, kMaxRank * 9, kThreads>(p, o0, noc, lamS, Ws);
+    } else {
+      for (int i = threadIdx.x; i < OC * nW; i += kThreads) {
+        const int oc = i / nW;
+        Ws[i] = (oc < noc) ? p.W[static_cast<size_t>(o0) * nW + i] : 0.f;
+      }
     }
     __syncthreads();
 
@@ -277,6 +292,15 @@ insert_wide_kernel(const InsertLoopParams p, const float* __restrict__ kpT, floa
         }
       }
       __syncthreads();
+      if constexpr (kLinear) {
+        // ---- Λ mode: dΛ = dW d^T, Adam on Λ, W = W0 + Λ d   (ganrewrite.py:219-240)
+        linear_mode::adam_step<OC, kMaxRank * 9, kWarps>(p, noc, dWS, lamS, lamMS, lamVS,
+                                                         step_size, bc2_sqrt, one_m_b1, one_m_b2);
+        __syncthreads();
+        linear_mode::rebuild_weights<OC, kMaxRank * 9, kThreads>(p, o0, noc, lamS, Ws);
+        __syncthreads();
+        continue;
+      }
       // ---- optional gradient projection onto span(d)   (ganrewrite.py:285-286)
       if (p.project_gradient) {
         for (int ort = warp; ort < OC * p.rank * 9; ort += kWarps) {
@@ -339,25 +363,20 @@ insert_wide_kernel(const InsertLoopParams p, const float* __restrict__ kpT, floa
     }
     for (int i = threadIdx.x; i < noc * nW; i += kThreads)
       p.W[static_cast<size_t>(o0) * nW + i] = Ws[i];
+    if constexpr (kLinear)
+      linear_mode::store_state<OC, kMaxRank * 9, kThreads>(p, o0, noc, lamS, lamMS, lamVS);
     __syncthreads();
   }
 }
 
-size_t wide_smem_bytes(int Cin) {
-  return (static_cast<size_t>(2 * OC) * Cin * 9 + OC * kMaxRank * 9 + 64 + kWarps * OC * 5) *
-         sizeof(float);
+size_t wide_smem_bytes(int Cin, bool linear) {
+  return (static_cast<size_t>(2 * OC) * Cin * 9 + OC * kMaxRank * 9 + kMiscFloats +
+          (linear ? kLamFloats : 0)) * sizeof(float);
 }
 
-}  // namespace
-
-size_t insert_wide_workspace_bytes(int Cout, int B, int h, int w) {
-  if (Cout < 1 || B < 1 || h < 1 || w < 1) return 0;
-  const size_t cout4 = (static_cast<size_t>(Cout) + OC - 1) / OC * OC;
-  return 2 * cout4 * static_cast<size_t>(B) * h * w * sizeof(float);
-}
-
-int insert_wide_launch(const InsertLoopParams& p, void* workspace, size_t workspace_bytes,
-                       cudaStream_t stream) {
+template <bool kLinear>
+int wide_launch_mode(const InsertLoopParams& p, void* workspace, size_t workspace_bytes,
+                     cudaStream_t stream) {
   if (p.B < 1 || p.B > 4 || p.h < 1 || p.w < 1 || p.Cout < 1 || p.Cin < kMinCin || p.Cin % 32 != 0 ||
       p.Cin > kMaxCin || p.rank < 1 || p.rank > kMaxRank ||
       static_cast<long long>(p.Cout + OC) * p.B * p.h * p.w > (1LL << 31) - 1) {
@@ -371,10 +390,10 @@ int insert_wide_launch(const InsertLoopParams& p, void* workspace, size_t worksp
     set_last_error("insert_loop_wide: workspace %zu B < %zu B needed", workspace_bytes, need);
     return RW_ERR_BAD_ARG;
   }
-  const size_t smem = wide_smem_bytes(p.Cin);
+  const size_t smem = wide_smem_bytes(p.Cin, kLinear);
   static size_t attr = 0;
   if (smem > attr) {
-    int rc = check_cuda(cudaFuncSetAttribute(insert_wide_kernel,
+    int rc = check_cuda(cudaFuncSetAttribute(insert_wide_kernel<kLinear>,
                                              cudaFuncAttributeMaxDynamicSharedMemorySize,
                                              static_cast<int>(smem)),
                         "insert_loop_wide smem attr");
@@ -387,8 +406,26 @@ int insert_wide_launch(const InsertLoopParams& p, void* workspace, size_t worksp
   int grid = (p.Cout + OC - 1) / OC;
   const int sms = device_sm_count();
   if (grid > sms) grid = sms;
-  insert_wide_kernel<<<grid, kThreads, smem, stream>>>(p, p.key, tG, gdG);
+  insert_wide_kernel<kLinear><<<grid, kThreads, smem, stream>>>(p, p.key, tG, gdG);
   return check_cuda(cudaGetLastError(), "insert_loop_wide launch");
+}
+
+}  // namespace
+
+size_t insert_wide_workspace_bytes(int Cout, int B, int h, int w) {
+  if (Cout < 1 || B < 1 || h < 1 || w < 1) return 0;
+  const size_t cout4 = (static_cast<size_t>(Cout) + OC - 1) / OC * OC;
+  return 2 * cout4 * static_cast<size_t>(B) * h * w * sizeof(float);
+}
+
+int insert_wide_launch(const InsertLoopParams& p, void* workspace, size_t workspace_bytes,
+                       cudaStream_t stream) {
+  return wide_launch_mode<false>(p, workspace, workspace_bytes, stream);
+}
+
+int linear_insert_wide_launch(const InsertLoopParams& p, void* workspace, size_t workspace_bytes,
+                              cudaStream_t stream) {
+  return wide_launch_mode<true>(p, workspace, workspace_bytes, stream);
 }
 
 }  // namespace rw

@@ -17,6 +17,7 @@
 // that lanes <-> input channels gives coalesced 128-byte loads.
 #include "rw_common.cuh"
 #include "rw_kernels.h"
+#include "insert_linear.cuh"
 
 namespace rw {
 
@@ -69,10 +70,15 @@ project_rank_kernel(const float* __restrict__ w, const float* __restrict__ base,
 // so it is streamed from L2 — the dominant cost.  Blocking four output channels per CTA makes
 // every loaded key value feed four accumulators (4x less L2 traffic than one channel per CTA:
 // measured 180 us -> see profiles), and the register tile is templated on the crop width.
+//
+// kLinear selects the Λ mode (linear_insert, csrc/insert_linear.cuh): the same forward, loss and
+// weight gradient, then Adam on Λ and W = W0 + Λ d instead of Adam on W and the projections.
 // ---------------------------------------------------------------------------
 constexpr int OC = 4;
+constexpr int kMiscFloats = 64 + kWarps * OC * 5 + 64;   // demod, coef, loss and G tables
+constexpr int kLamFloats = 3 * OC * kMaxRank * 9;       // Λ mode: Λ, exp_avg, exp_avg_sq
 
-template <int MW>   // register tile width >= crop width w
+template <int MW, bool kLinear>   // register tile width >= crop width w
 __global__ void __launch_bounds__(kThreads, 1)
 insert_loop_kernel(const InsertLoopParams p, const float* __restrict__ kpT) {
   extern __shared__ float sm[];
@@ -90,6 +96,9 @@ insert_loop_kernel(const InsertLoopParams p, const float* __restrict__ kpT) {
   float* coefS = misc + 16;            // [OC][4]
   float* lossS = misc + 32;            // [kWarps][OC]
   float* GS = misc + 64;               // [kWarps][OC][4]
+  float* lamS = misc + kMiscFloats;    // Λ mode: [OC][kMaxRank*9] Λ, then exp_avg, exp_avg_sq
+  float* lamMS = lamS + OC * kMaxRank * 9;
+  float* lamVS = lamMS + OC * kMaxRank * 9;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const bool plain = p.plain_conv != 0;  // nn.Conv2d target: no demodulation, no weight scale
@@ -99,9 +108,15 @@ insert_loop_kernel(const InsertLoopParams p, const float* __restrict__ kpT) {
 
   for (int o0 = blockIdx.x * OC; o0 < p.Cout; o0 += gridDim.x * OC) {
     const int noc = (p.Cout - o0 < OC) ? p.Cout - o0 : OC;
-    for (int i = threadIdx.x; i < OC * nW; i += kThreads) {
-      const int oc = i / nW;
-      Ws[i] = (oc < noc) ? p.W[static_cast<size_t>(o0) * nW + i] : 0.f;
+    if constexpr (kLinear) {
+      linear_mode::load_state<OC, kMaxRank * 9, kThreads>(p, o0, noc, lamS, lamMS, lamVS);
+      __syncthreads();
+      linear_mode::rebuild_weights<OC, kMaxRank * 9, kThreads>(p, o0, noc, lamS, Ws);
+    } else {
+      for (int i = threadIdx.x; i < OC * nW; i += kThreads) {
+        const int oc = i / nW;
+        Ws[i] = (oc < noc) ? p.W[static_cast<size_t>(o0) * nW + i] : 0.f;
+      }
     }
     __syncthreads();
 
@@ -303,6 +318,15 @@ insert_loop_kernel(const InsertLoopParams p, const float* __restrict__ kpT) {
         }
       }
       __syncthreads();
+      if constexpr (kLinear) {
+        // ---- Λ mode: dΛ = dW d^T, Adam on Λ, W = W0 + Λ d   (ganrewrite.py:219-240)
+        linear_mode::adam_step<OC, kMaxRank * 9, kWarps>(p, noc, dWS, lamS, lamMS, lamVS,
+                                                         step_size, bc2_sqrt, one_m_b1, one_m_b2);
+        __syncthreads();
+        linear_mode::rebuild_weights<OC, kMaxRank * 9, kThreads>(p, o0, noc, lamS, Ws);
+        __syncthreads();
+        continue;
+      }
       // ---- optional gradient projection onto span(d)   (ganrewrite.py:285-286)
       if (p.project_gradient) {
         for (int ort = warp; ort < OC * p.rank * 9; ort += kWarps) {
@@ -365,15 +389,17 @@ insert_loop_kernel(const InsertLoopParams p, const float* __restrict__ kpT) {
     }
     for (int i = threadIdx.x; i < noc * nW; i += kThreads)
       p.W[static_cast<size_t>(o0) * nW + i] = Ws[i];
+    if constexpr (kLinear)
+      linear_mode::store_state<OC, kMaxRank * 9, kThreads>(p, o0, noc, lamS, lamMS, lamVS);
     __syncthreads();
   }
 }
 
-template <int MW>
+template <int MW, bool kLinear>
 static int launch_insert(const InsertLoopParams& p, size_t smem, cudaStream_t stream) {
   static size_t attr = 0;
   if (smem > attr) {
-    int rc = check_cuda(cudaFuncSetAttribute(insert_loop_kernel<MW>,
+    int rc = check_cuda(cudaFuncSetAttribute(insert_loop_kernel<MW, kLinear>,
                                              cudaFuncAttributeMaxDynamicSharedMemorySize,
                                              static_cast<int>(smem)),
                         "insert_loop smem attr");
@@ -383,7 +409,7 @@ static int launch_insert(const InsertLoopParams& p, size_t smem, cudaStream_t st
   int grid = (p.Cout + OC - 1) / OC;
   const int sms = device_sm_count();
   if (grid > sms) grid = sms;
-  insert_loop_kernel<MW><<<grid, kThreads, smem, stream>>>(p, p.key);
+  insert_loop_kernel<MW, kLinear><<<grid, kThreads, smem, stream>>>(p, p.key);
   return check_cuda(cudaGetLastError(), "insert_loop launch");
 }
 
@@ -418,7 +444,8 @@ int project_rank_launch_signed(const float* w, const float* base, const float* d
   return check_cuda(cudaGetLastError(), "project_rank launch");
 }
 
-int insert_loop_launch(const InsertLoopParams& p, cudaStream_t stream) {
+template <bool kLinear>
+static int insert_loop_launch_mode(const InsertLoopParams& p, cudaStream_t stream) {
   if (p.w > kMaxW || p.B > 4 || p.B < 1 || p.Cin % 32 != 0 || p.rank > kMaxRank || p.rank < 1 ||
       static_cast<long long>(p.B) * p.h * p.w > 4096) {
     set_last_error("insert_loop: unsupported crop B=%d h=%d w=%d Cin=%d rank=%d", p.B, p.h, p.w,
@@ -428,14 +455,23 @@ int insert_loop_launch(const InsertLoopParams& p, cudaStream_t stream) {
   const int P = p.B * p.h * p.w;
   const int nW = p.Cin * 9;
   const size_t smem = (static_cast<size_t>(2 * OC) * nW + static_cast<size_t>(2 * OC) * P +
-                       OC * kMaxRank * 9 + 64 + kWarps * OC * 5 + 64) * sizeof(float);
+                       OC * kMaxRank * 9 + kMiscFloats + (kLinear ? kLamFloats : 0)) *
+                      sizeof(float);
   if (smem > 225 * 1024) {
     set_last_error("insert_loop: shared memory %zu B too large", smem);
     return RW_ERR_UNSUPPORTED;
   }
-  if (p.w <= 8) return launch_insert<8>(p, smem, stream);
-  if (p.w <= 12) return launch_insert<12>(p, smem, stream);
-  return launch_insert<16>(p, smem, stream);
+  if (p.w <= 8) return launch_insert<8, kLinear>(p, smem, stream);
+  if (p.w <= 12) return launch_insert<12, kLinear>(p, smem, stream);
+  return launch_insert<16, kLinear>(p, smem, stream);
+}
+
+int insert_loop_launch(const InsertLoopParams& p, cudaStream_t stream) {
+  return insert_loop_launch_mode<false>(p, stream);
+}
+
+int linear_insert_loop_launch(const InsertLoopParams& p, cudaStream_t stream) {
+  return insert_loop_launch_mode<true>(p, stream);
 }
 
 }  // namespace rw

@@ -207,11 +207,21 @@ struct InsertLoopParams {
   int plain_conv;       // 1: no demodulation, weight scale 1 (ProgGAN `layerN.conv`)
   float one_minus_beta1, one_minus_beta2;   // 1-beta as torch forms it (double, rounded once)
   double beta1_exact, beta2_exact;          // betas for the bias corrections (python doubles)
+  // Λ mode only (linear_insert: W = W0 + Λ d, Adam on Λ; csrc/insert_linear.cuh).  m, v, w_ortho,
+  // piter and project_gradient are then unused.
+  const float* W0;      // [Cout, Cin, 3, 3] original weight, read only (must not alias W)
+  float* lam;           // [Cout, rank, 3, 3] Λ, updated in place
+  float* lam_m;         // Adam exp_avg of Λ
+  float* lam_v;         // Adam exp_avg_sq of Λ
 };
 int insert_loop_launch(const InsertLoopParams& p, cudaStream_t stream);
 // wide-key variant (csrc/insert_wide.cu): any crop width, t and g*demod in `workspace`
 size_t insert_wide_workspace_bytes(int Cout, int B, int h, int w);
 int insert_wide_launch(const InsertLoopParams& p, void* workspace, size_t workspace_bytes,
                        cudaStream_t stream);
+// the same two loops in Λ mode
+int linear_insert_loop_launch(const InsertLoopParams& p, cudaStream_t stream);
+int linear_insert_wide_launch(const InsertLoopParams& p, void* workspace, size_t workspace_bytes,
+                              cudaStream_t stream);
 
 }  // namespace rw

@@ -44,21 +44,28 @@ FUSED_CHUNK = 64     # iterations per fused launch when a callback wants per-ste
 WIDE_MAX_WORK = 512 * 32 * 32   # rw_insert_loop_wide routing limit, see fused_insert_kernel
 
 
-def fused_insert_kernel(B, Cin, Cout, h, w):
+def fused_insert_kernel(B, Cin, Cout, h, w, linear=False):
     """The one-launch insert kernel for a key crop [B, Cin, h, w] -> [B, Cout, h, w], or None to
     run the loop through autograd.  Small crops keep rw_insert_loop (t and g in shared memory,
     register tile up to 16 columns).  Larger ones with 128 <= Cin <= 512 take rw_insert_loop_wide
     (t and g in an L2-resident workspace, 16-column chunks) while wide_insert_work() is at most
     WIDE_MAX_WORK: the largest size measured no slower per iteration than the autograd loop on an
-    H100 (DESIGN.md §6).  Beyond it the tensor-core autograd loop is faster."""
+    H100 (DESIGN.md §6).  Beyond it the tensor-core autograd loop is faster.
+
+    linear=True routes linear_insert to the Λ-mode twins (rw_linear_insert_loop,
+    rw_linear_insert_loop_wide).  The only difference is the Λ state in shared memory, 3 x 4 x 32 x 9
+    floats next to rw_insert_loop's crop: at Cin 512 its largest crops (1980 < B*h*w <= 2412) no
+    longer fit, and being far past WIDE_MAX_WORK they stay on autograd."""
     if B > 4 or Cin % 32 != 0:
         return None
+    prefix = 'rw_linear_' if linear else 'rw_'
     # shared memory of rw_insert_loop (csrc/rewrite.cu insert_loop_launch): 4 weight rows +
-    # 4 gradient rows + 8 crop-sized vectors + small tables, within 225 KB
-    if w <= 16 and B * h * w <= 4096 and (8 * Cin * 9 + 8 * B * h * w + 1440) * 4 <= 225 * 1024:
-        return 'rw_insert_loop'
+    # 4 gradient rows + 8 crop-sized vectors + small tables (+ the Λ state), within 225 KB
+    small = 8 * Cin * 9 + 8 * B * h * w + 1440 + (3 * 4 * 32 * 9 if linear else 0)
+    if w <= 16 and B * h * w <= 4096 and small * 4 <= 225 * 1024:
+        return prefix + 'insert_loop'
     if 128 <= Cin <= 512 and Cout <= 512 and wide_insert_work(B, Cin, h, w) <= WIDE_MAX_WORK:
-        return 'rw_insert_loop_wide'
+        return prefix + 'insert_loop_wide'
     return None
 
 
@@ -455,12 +462,27 @@ class ProgressiveGanRewriter(object):
 
     def linear_insert(self, key, val, context=None, update_callback=None, niter=2001, lr=0.05,
                       return_timing=False):
-        """Optimises Lambda in W = W0 + Lambda d directly [ganrewrite.py:201-252]."""
+        """Optimises Lambda in W = W0 + Lambda d directly [ganrewrite.py:201-252].  The targets
+        `_fused_plan` recognises run in one kernel per launch (`_insert_fused` in Λ mode); every
+        other one runs the reference's loop through autograd."""
         if return_timing:
             torch.cuda.synchronize()
             t0 = time.time()
         nethook.set_requires_grad(False, self.model)
         key, val = [self.detach(d) for d in [key, val]]
+        plan = self._fused_plan(key, val, context, linear=True) if self.fused_insert else None
+        if plan is not None:
+            with nvtx.range('rw:linear_insert'):
+                self._insert_fused(plan, key, val, context, update_callback, niter, 1, lr,
+                                   linear=True)
+        else:
+            self._linear_insert_autograd(key, val, context, update_callback, niter, lr)
+        if return_timing:
+            torch.cuda.synchronize()
+            return (time.time() - t0) * 1000
+
+    def _linear_insert_autograd(self, key, val, context, update_callback, niter, lr):
+        """The reference's hooked-weight loop: W = W0 + einsum(Lambda, d) rebuilt every forward."""
         w0 = self.target_weights()
         owner = [m for m in self.target_model.modules()
                  if getattr(m, 'weight', None) is w0][0]
@@ -488,9 +510,6 @@ class ProgressiveGanRewriter(object):
             del owner.weight
             owner.register_parameter('weight', w0)
             del owner.__dict__['forward']
-        if return_timing:
-            torch.cuda.synchronize()
-            return (time.time() - t0) * 1000
 
     def insert(self, key, val, context=None, update_callback=None, niter=2001, piter=10,
                lr=0.05, return_timing=False):
@@ -534,11 +553,12 @@ class ProgressiveGanRewriter(object):
                         weight[...] = projected_conv(weight, context, base=ortho_weight)
 
     # -- fused path ------------------------------------------------------------------------
-    def _fused_plan(self, key, val, context):
+    def _fused_plan(self, key, val, context, linear=False):
         """Returns (kernel, conv, noise_module, act_module, plain, key) if the target model is the
         canonical [dconv (, noise, activate)] chain of a SeqStyleGAN2 layer — or the single plain
         `layerN.conv` of a ProgGAN generator (plain = True) — on a key `fused_insert_kernel`
-        routes to a fused kernel, else None."""
+        routes to a fused kernel, else None.  linear=True plans linear_insert, whose kernels
+        take no plain conv: the reference's Lambda is 5-D and fails on a ProgGAN weight."""
         if context is None:
             return None
         if any('forward' in m.__dict__ for m in self.target_model.modules()):
@@ -577,6 +597,8 @@ class ProgressiveGanRewriter(object):
             # ProgressiveGanRewriter on a ProgGAN: target = `layerN.conv`, a bias-free 3x3 conv
             if len(leaves) != 1 or not isinstance(leaves[0], torch.nn.Conv2d):
                 return None
+            if linear:
+                return None
             dconv, nz, act, plain = leaves[0], None, None, True
             if (dconv.kernel_size != (3, 3) or dconv.padding != (1, 1) or dconv.stride != (1, 1) or
                     dconv.bias is not None or dconv.groups != 1 or dconv.dilation != (1, 1)):
@@ -588,14 +610,18 @@ class ProgressiveGanRewriter(object):
         if not k.is_cuda or k.dtype != torch.float32:
             return None
         B, Cin, h, w = k.shape
-        kernel = fused_insert_kernel(B, Cin, cout, h, w)
+        kernel = fused_insert_kernel(B, Cin, cout, h, w, linear=linear)
         if kernel is None or context.shape[0] > 32:
             return None
         if tuple(self.target_acts(val).shape) != (B, cout, h, w):
             return None
         return kernel, dconv, nz, act, plain, k
 
-    def _insert_fused(self, plan, key, val, context, update_callback, niter, piter, lr):
+    def _insert_fused(self, plan, key, val, context, update_callback, niter, piter, lr,
+                      linear=False):
+        """Runs the planned kernel in launches of all `niter` iterations, or of FUSED_CHUNK when a
+        callback wants the loss of every step.  linear=True: Adam on Lambda in W = W0 + Lambda d
+        (rw_linear_insert_loop*), Lambda and its moments carried from launch to launch."""
         kernel, dconv, nz, act, plain, k = plan
         weight = self.target_weights()
         assert weight is dconv.weight
@@ -605,9 +631,9 @@ class ProgressiveGanRewriter(object):
         with torch.no_grad():
             d = context.detach().to(dev, torch.float32).contiguous()
             ortho = (projected_conv(weight, d, base=weight, sign=-1.0).contiguous()
-                     if self.low_rank_insert else None)
-            m = torch.zeros_like(weight)
-            v = torch.zeros_like(weight)
+                     if self.low_rank_insert and not linear else None)
+            m = torch.zeros_like(weight) if not linear else None
+            v = torch.zeros_like(weight) if not linear else None
             key_cl = torch.nn.functional.pad(k, (1, 1, 1, 1)).permute(0, 2, 3, 1).contiguous()
             style = None if plain else key.style.detach().to(torch.float32).contiguous()
             target = self.target_acts(val).detach().to(torch.float32).contiguous()
@@ -620,7 +646,9 @@ class ProgressiveGanRewriter(object):
             if not wdata.is_contiguous():
                 raise _cabi.RwError('insert: target weight must be contiguous')
             args = _cabi.InsertArgs()
-            args.W, args.m, args.v = wdata.data_ptr(), m.data_ptr(), v.data_ptr()
+            args.W = wdata.data_ptr()
+            if not linear:
+                args.m, args.v = m.data_ptr(), v.data_ptr()
             args.w_ortho = ortho.data_ptr() if ortho is not None else None
             args.d = d.data_ptr()
             args.key_cl, args.target = key_cl.data_ptr(), target.data_ptr()
@@ -641,9 +669,20 @@ class ProgressiveGanRewriter(object):
             args.has_noise_act = 1 if nz is not None else 0
             args.plain_conv = 1 if plain else 0
             args.niter_total, args.piter = niter, piter
-            args.project_gradient = 1 if self.low_rank_gradient else 0
+            args.project_gradient = 1 if self.low_rank_gradient and not linear else 0
             launch = (ctypes.byref(args),)
-            if kernel == 'rw_insert_loop_wide':
+            if linear:
+                # W0 (L2-resident copy), Lambda and its Adam moments, [Cout, rank, 3, 3] each
+                w0 = wdata.clone()
+                lam = torch.zeros(Cout, d.shape[0], 3, 3, device=dev)
+                lam_m, lam_v = torch.zeros_like(lam), torch.zeros_like(lam)
+                largs = _cabi.LinearInsertArgs()
+                largs.struct_size = ctypes.sizeof(_cabi.LinearInsertArgs)
+                largs.base = ctypes.pointer(args)
+                largs.W0, largs.lam = w0.data_ptr(), lam.data_ptr()
+                largs.lam_m, largs.lam_v = lam_m.data_ptr(), lam_v.data_ptr()
+                launch = (ctypes.byref(largs),)
+            if kernel.endswith('insert_loop_wide'):
                 # per-pixel t and g*demod of every channel: [Cout][B*h*w] x 2 fp32 scratch
                 nbytes = _cabi.load().rw_insert_wide_workspace_bytes(Cout, B, h, w)
                 workspace = torch.empty(nbytes, dtype=torch.uint8, device=dev)
