@@ -32,8 +32,10 @@
  *   projected_conv(weight, direction)  rewrite/ganrewrite.py:806-813       -> rw_project_rank
  *   ProgressiveGanRewriter.insert hot loop rewrite/ganrewrite.py:279-294   -> rw_insert_loop,
  *                                                                              rw_insert_loop_wide
+ *                                           (upsampling target)           -> rw_insert_loop_up
  *   ProgressiveGanRewriter.linear_insert   rewrite/ganrewrite.py:201-252   -> rw_linear_insert_loop,
  *                                                                              rw_linear_insert_loop_wide
+ *                                           (upsampling target)           -> rw_linear_insert_loop_up
  *
  * Layout vocabulary
  *   key planes  : the style-modulated key k = style*x as two bf16 planes (hi, lo; k ~= hi+lo)
@@ -301,6 +303,25 @@ typedef struct rw_linear_insert_args {
 int rw_linear_insert_loop(const rw_linear_insert_args* args, rw_stream_t stream);
 int rw_linear_insert_loop_wide(const rw_linear_insert_args* args, void* workspace,
                                size_t workspace_bytes, rw_stream_t stream);
+
+/* The two loops above for the upsampling target of an odd StyleGAN2 layer: dconv (conv_transpose,
+ * stride 2, no padding) -> blur (upfirdn2d with `blur`, pad (1,1)) -> noise -> activate.  h and w
+ * are the key crop's size (key_cl as above); target is [B,Cout,2h,2w] and noise [B,4*h*w] or NULL.
+ * `blur` is the layer's 4x4 blur kernel exactly as stored (mconv.blur.kernel, row-major), applied
+ * flipped as upfirdn2d applies it; it is a host array, copied into the launch.  The conv_transpose
+ * plane T, the output gradient g and gT = demod * blur^T(g) go to `workspace`, at least
+ * rw_insert_up_workspace_bytes(Cout, B, h, w) bytes (fp32 planes [Cout rounded up to 4][B][...]:
+ * two of (2h+1)x(2w+1) and one of 2h x 2w), which the call owns until it completes on `stream`.
+ * Everything after dW (projections, low_rank_gradient, Adam, the Λ mode) is as in
+ * rw_insert_loop_wide / rw_linear_insert_loop_wide.  Needs 1 <= B <= 4, Cin % 32 == 0,
+ * 128 <= Cin <= 512, 1 <= rank <= 32 and plain_conv 0 (ProgGAN has no upsampling target); any other
+ * shape, a NULL blur or a NULL or short workspace returns RW_STATUS_BAD_ARG before anything is
+ * launched, with the reason in rw_last_error(). */
+size_t rw_insert_up_workspace_bytes(int Cout, int B, int h, int w);
+int rw_insert_loop_up(const rw_insert_args* args, const float blur[16], void* workspace,
+                      size_t workspace_bytes, rw_stream_t stream);
+int rw_linear_insert_loop_up(const rw_linear_insert_args* args, const float blur[16],
+                             void* workspace, size_t workspace_bytes, rw_stream_t stream);
 
 /* out[rows][N] = A[rows][K] . W[N][K]^T on the tensor-core row-GEMM (3-term split bf16 planes from
  * rw_split_rows; K % 64 == 0, N % 128 == 0): the key algebra between key capture and the

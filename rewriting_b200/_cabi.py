@@ -117,6 +117,9 @@ SIGNATURES = {
     'rw_insert_loop_wide': (c_int, [ctypes.POINTER(InsertArgs), c_p, c_sz, c_p]),
     'rw_linear_insert_loop': (c_int, [ctypes.POINTER(LinearInsertArgs), c_p]),
     'rw_linear_insert_loop_wide': (c_int, [ctypes.POINTER(LinearInsertArgs), c_p, c_sz, c_p]),
+    'rw_insert_up_workspace_bytes': (c_sz, [c_int, c_int, c_int, c_int]),
+    'rw_insert_loop_up': (c_int, [ctypes.POINTER(InsertArgs), c_p, c_p, c_sz, c_p]),
+    'rw_linear_insert_loop_up': (c_int, [ctypes.POINTER(LinearInsertArgs), c_p, c_p, c_sz, c_p]),
     'rw_debug_rowgemm': (c_int, [c_p, c_p, c_p, c_p, c_int, c_int, c_int, c_p, c_p]),
     'rw_debug_colgemm': (c_int, [c_p, c_p, c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_p,
                                  c_p, c_sz, c_p]),

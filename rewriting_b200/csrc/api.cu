@@ -934,6 +934,26 @@ int rw_linear_insert_loop_wide(const rw_linear_insert_args* a, void* workspace,
   return linear_insert_wide_launch(p, workspace, workspace_bytes, stream);
 }
 
+size_t rw_insert_up_workspace_bytes(int Cout, int B, int h, int w) {
+  return insert_up_workspace_bytes(Cout, B, h, w);
+}
+
+int rw_insert_loop_up(const rw_insert_args* a, const float blur[16], void* workspace,
+                      size_t workspace_bytes, rw_stream_t stream) {
+  InsertLoopParams p;
+  int rc = insert_params(a, "rw_insert_loop_up", p);
+  if (rc) return rc;
+  return insert_up_launch(p, blur, workspace, workspace_bytes, stream);
+}
+
+int rw_linear_insert_loop_up(const rw_linear_insert_args* a, const float blur[16], void* workspace,
+                             size_t workspace_bytes, rw_stream_t stream) {
+  InsertLoopParams p;
+  int rc = linear_insert_params(a, "rw_linear_insert_loop_up", p);
+  if (rc) return rc;
+  return linear_insert_up_launch(p, blur, workspace, workspace_bytes, stream);
+}
+
 int rw_debug_rowgemm(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo,
                      int rows, int K, int N, float* out, rw_stream_t stream) {
   ConvTcParams p;

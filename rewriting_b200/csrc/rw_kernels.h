@@ -223,5 +223,12 @@ int insert_wide_launch(const InsertLoopParams& p, void* workspace, size_t worksp
 int linear_insert_loop_launch(const InsertLoopParams& p, cudaStream_t stream);
 int linear_insert_wide_launch(const InsertLoopParams& p, void* workspace, size_t workspace_bytes,
                               cudaStream_t stream);
+// upsampling target of the odd StyleGAN2 layers (insert_wide.cu up mode): key crop h x w, value
+// crop 2h x 2w; blur = the layer's 4x4 blur kernel (host array, copied into the launch)
+size_t insert_up_workspace_bytes(int Cout, int B, int h, int w);
+int insert_up_launch(const InsertLoopParams& p, const float* blur, void* workspace,
+                     size_t workspace_bytes, cudaStream_t stream);
+int linear_insert_up_launch(const InsertLoopParams& p, const float* blur, void* workspace,
+                            size_t workspace_bytes, cudaStream_t stream);
 
 }  // namespace rw

@@ -42,6 +42,7 @@ from ..utils.stylegan2 import models as sg2
 
 FUSED_CHUNK = 64     # iterations per fused launch when a callback wants per-step losses
 WIDE_MAX_WORK = 512 * 32 * 32   # rw_insert_loop_wide routing limit, see fused_insert_kernel
+UP_MAX_WORK = 512 * 33 * 33     # rw_insert_loop_up routing limit, see fused_insert_up_kernel
 
 
 def fused_insert_kernel(B, Cin, Cout, h, w, linear=False):
@@ -78,6 +79,27 @@ def wide_insert_work(B, Cin, h, w):
     CTA per SM, so up to Cout = 512 the time does not depend on Cout."""
     return max(Cin, 256) * B * h * (-(-w // 16) * 16)
     return None
+
+
+def fused_insert_up_kernel(B, Cin, Cout, h, w, linear=False):
+    """The one-launch insert kernel for the upsampling target of an odd StyleGAN2 layer (dconv
+    conv_transpose -> blur -> noise -> activate) on a key crop [B, Cin, h, w] -> [B, Cout, 2h, 2w],
+    or None to run the loop through autograd.  Keys go to rw_insert_loop_up while
+    up_insert_work() is at most UP_MAX_WORK: the largest size measured no slower per iteration
+    than the autograd loop on an H100 (DESIGN.md §6; the whole 32 x 32 layer-9 map).  Beyond it
+    the next size measured, 815 360, was slower.  linear=True names the Λ-mode twin."""
+    if B > 4 or Cin % 32 != 0 or not 128 <= Cin <= 512 or Cout > 512:
+        return None
+    if up_insert_work(B, Cin, h, w) > UP_MAX_WORK:
+        return None
+    return 'rw_linear_insert_loop_up' if linear else 'rw_insert_loop_up'
+
+
+def up_insert_work(B, Cin, h, w):
+    """What one CTA of rw_insert_loop_up spends per iteration, in the units of wide_insert_work:
+    points of the (h+1) x (w+1) polyphase grid the conv_transpose gathers over, times
+    max(Cin, 256) (the weight gradient gives a warp to each 32 input channels)."""
+    return max(Cin, 256) * B * (h + 1) * (w + 1)
 
 
 _DCONV_RE = _re.compile(r'^layer(\d+)\.(?:sconv|conv)\.mconv\.dconv$')
@@ -470,7 +492,10 @@ class ProgressiveGanRewriter(object):
             t0 = time.time()
         nethook.set_requires_grad(False, self.model)
         key, val = [self.detach(d) for d in [key, val]]
-        plan = self._fused_plan(key, val, context, linear=True) if self.fused_insert else None
+        plan = None
+        if self.fused_insert:
+            plan = (self._fused_plan(key, val, context, linear=True) or
+                    self._fused_up_plan(key, val, context, linear=True))
         if plan is not None:
             with nvtx.range('rw:linear_insert'):
                 self._insert_fused(plan, key, val, context, update_callback, niter, 1, lr,
@@ -521,7 +546,9 @@ class ProgressiveGanRewriter(object):
             torch.cuda.synchronize()
             t0 = time.time()
         key, val = [self.detach(d) for d in [key, val]]
-        plan = self._fused_plan(key, val, context) if self.fused_insert else None
+        plan = None
+        if self.fused_insert:
+            plan = self._fused_plan(key, val, context) or self._fused_up_plan(key, val, context)
         with nvtx.range('rw:insert'):
             if plan is not None:
                 self._insert_fused(plan, key, val, context, update_callback, niter, piter, lr)
@@ -617,17 +644,64 @@ class ProgressiveGanRewriter(object):
             return None
         return kernel, dconv, nz, act, plain, k
 
+    def _fused_up_plan(self, key, val, context, linear=False):
+        """Returns (kernel, conv, noise_module, act_module, False, key, blur_taps) if the target
+        model is the upsampling chain [dconv (upsample), blur, noise, activate] of an odd
+        SeqStyleGAN2 layer — or SeqPre's [adain, ...] form, whose key is style (.) fmap — on a key
+        `fused_insert_up_kernel` routes to rw_insert_loop_up, else None.  SeqTiny's odd target
+        (dconv alone) yields the unblurred (2h+1)x(2w+1) map and stays on autograd."""
+        if context is None or context.shape[0] > 32:
+            return None
+        if any('forward' in m.__dict__ for m in self.target_model.modules()):
+            return None
+        if not isinstance(key, dict) or 'fmap' not in key or 'style' not in key:
+            return None
+        leaves = [m for m in self.target_model.modules() if len(list(m.children())) == 0]
+        premod = len(leaves) == 5 and isinstance(leaves[0], sg2.ApplyStyle)
+        if premod:
+            leaves = leaves[1:]
+        if len(leaves) != 4:
+            return None
+        dconv, blur, nz, act = leaves
+        if not (isinstance(dconv, sg2.DemodulatedConv2dF) and isinstance(blur, sg2.BlurF) and
+                isinstance(nz, sg2.NoiseInjectionF) and isinstance(act, sg2.FusedLeakyReLUF)):
+            return None
+        if not dconv.upsample or not dconv.demodulate or dconv.kernel_size != 3:
+            return None
+        if tuple(blur.kernel.shape) != (4, 4) or tuple(blur.pad) != (1, 1):
+            return None
+        if abs(act.negative_slope - 0.2) > 0 or abs(act.scale - 2 ** 0.5) > 1e-12:
+            return None
+        if key.get('noise', None) is not None:
+            return None
+        k = key.fmap
+        if premod:
+            k = key.style.detach()[:, :, None, None] * k
+        if not k.is_cuda or k.dtype != torch.float32:
+            return None
+        B, Cin, h, w = k.shape
+        cout = dconv.out_channel
+        kernel = fused_insert_up_kernel(B, Cin, cout, h, w, linear=linear)
+        if kernel is None:
+            return None
+        if tuple(self.target_acts(val).shape) != (B, cout, 2 * h, 2 * w):
+            return None
+        taps = [float(t) for t in blur.kernel.detach().to(torch.float32).reshape(16).cpu()]
+        return kernel, dconv, nz, act, False, k, taps
+
     def _insert_fused(self, plan, key, val, context, update_callback, niter, piter, lr,
                       linear=False):
         """Runs the planned kernel in launches of all `niter` iterations, or of FUSED_CHUNK when a
         callback wants the loss of every step.  linear=True: Adam on Lambda in W = W0 + Lambda d
-        (rw_linear_insert_loop*), Lambda and its moments carried from launch to launch."""
-        kernel, dconv, nz, act, plain, k = plan
+        (rw_linear_insert_loop*), Lambda and its moments carried from launch to launch.  An
+        `_fused_up_plan` plan carries the blur taps and runs on a [B, Cout, 2h, 2w] value crop."""
+        kernel, dconv, nz, act, plain, k, *up = plan
         weight = self.target_weights()
         assert weight is dconv.weight
         B, Cin, h, w = k.shape
         Cout = weight.shape[-4]
         dev = k.device
+        vpix = 4 * h * w if up else h * w      # value-crop pixels per channel
         with torch.no_grad():
             d = context.detach().to(dev, torch.float32).contiguous()
             ortho = (projected_conv(weight, d, base=weight, sign=-1.0).contiguous()
@@ -637,9 +711,9 @@ class ProgressiveGanRewriter(object):
             key_cl = torch.nn.functional.pad(k, (1, 1, 1, 1)).permute(0, 2, 3, 1).contiguous()
             style = None if plain else key.style.detach().to(torch.float32).contiguous()
             target = self.target_acts(val).detach().to(torch.float32).contiguous()
-            noise = ops.noise_table(B, h * w, dev) if nz is not None else None
+            noise = ops.noise_table(B, vpix, dev) if nz is not None else None
             bias = act.bias.detach().contiguous() if act is not None else None
-            numel = float(B * Cout * h * w)
+            numel = float(B * Cout * vpix)
             chunk = niter if update_callback is None else min(niter, FUSED_CHUNK)
             loss_buf = torch.zeros(max(chunk, 1), Cout, device=dev)
             wdata = weight.data
@@ -687,6 +761,12 @@ class ProgressiveGanRewriter(object):
                 nbytes = _cabi.load().rw_insert_wide_workspace_bytes(Cout, B, h, w)
                 workspace = torch.empty(nbytes, dtype=torch.uint8, device=dev)
                 launch += (workspace.data_ptr(), nbytes)
+            elif up:
+                # T, gT ((2h+1)x(2w+1)) and g (2h x 2w) of every channel, fp32
+                blur = (ctypes.c_float * 16)(*up[0])
+                nbytes = _cabi.load().rw_insert_up_workspace_bytes(Cout, B, h, w)
+                workspace = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+                launch += (ctypes.addressof(blur), workspace.data_ptr(), nbytes)
             it0 = 0
             stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
             while it0 < niter:
