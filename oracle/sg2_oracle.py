@@ -63,6 +63,35 @@ def make_kernel(k):
     return k / k.sum()
 
 
+def blur_pads(ntaps, factor=2, kernel_size=3):
+    """models.py:277-279: the upsampling blur's pad from its length ((1, 1) for 4 taps, (1, 0)
+    for 3, (2, 1) for 5)."""
+    p = (ntaps - factor) - (kernel_size - 1)
+    return (p + 1) // 2 + factor - 1, p // 2 + 1
+
+
+def blur_case(name):
+    """4x4 test FIRs, x 4 as Blur(upsample_factor=2) scales them.  The model's [1,3,3,1]^2 ('sym')
+    is unchanged by flips and transposition, so a kernel reading its taps in the wrong
+    orientation passes with it; these do not:
+      'np'  make_kernel([1,2,4,1]): not palindromic, exactly rank one (the sum is 8)
+      't'   outer([1,2,4,1], [3,1,2,2]) / 64: also changes under transposition, exactly rank one
+      'z'   make_kernel([1,3,4,0]): rank one with a zero last tap
+      'ns'  'sym' + 0.03 N(0, 1): neither symmetric nor separable."""
+    if name == 'sym':
+        return make_kernel([1, 3, 3, 1]) * 4
+    if name == 'np':
+        return make_kernel([1, 2, 4, 1]) * 4
+    if name == 't':
+        return torch.outer(torch.tensor([1., 2., 4., 1.]), torch.tensor([3., 1., 2., 2.])) / 64 * 4
+    if name == 'z':
+        return make_kernel([1, 3, 4, 0]) * 4
+    if name == 'ns':
+        g = torch.Generator().manual_seed(77)
+        return make_kernel([1, 3, 3, 1]) * 4 + 0.03 * torch.randn(4, 4, generator=g)
+    raise ValueError(name)
+
+
 def noise_table(batch, hw, dtype=torch.float32):
     """models.py:542-545: RandomState(0).randn(batch, H*W) on every call."""
     return torch.from_numpy(np.random.RandomState(0).randn(batch, hw).astype('float32')).to(dtype)
@@ -113,9 +142,9 @@ def styled_conv(x, w_lat, p, upsample, blur_kernel=(1, 3, 3, 1)):
     style = modulate(w_lat, p['mod_w'], p['mod_b'])
     k = style[:, :, None, None] * x                                   # ApplyStyle :616-620
     t = demod_conv(k, style, p['weight'], upsample)
-    if upsample:                                                      # BlurF pad (1,1) :275-281
+    if upsample:                                                      # BlurF :275-281
         kern = (make_kernel(list(blur_kernel)) * 4).to(t.dtype)
-        t = upfirdn2d(t, kern, pad=(1, 1))
+        t = upfirdn2d(t, kern, pad=blur_pads(len(blur_kernel)))
     b, _, h, w = t.shape
     n = noise_table(b, h * w, t.dtype).view(b, 1, h, w)               # NoiseInjectionF :535-546
     pre = t + p['noise_w'] * n
@@ -147,10 +176,12 @@ def _rgb_params(sd, name):
                 weight=sd[pre + '.conv.weight'], bias=sd[pre + '.bias'])
 
 
-def generator_forward(sd, z, size=256, upto_key_layer=None, record=None):
+def generator_forward(sd, z, size=256, upto_key_layer=None, record=None,
+                      blur_kernel=(1, 3, 3, 1)):
     """SeqStyleGAN2.forward for mconv='seq', truncation=1 (models.py:92-141).
     `upto_key_layer=N` stops after layerN's adain and returns its key (the context model of
-    ganrewrite.py:48-50).  `record` (dict) receives per-layer activations."""
+    ganrewrite.py:48-50).  `record` (dict) receives per-layer activations.  `blur_kernel` is the
+    odd layers' blur; the RGB skip's UpsampleO keeps [1, 3, 3, 1] whatever it is (models.py:117)."""
     log_size = int(math.log(size, 2))
     w = mapping(sd, z)
     batch = z.shape[0]
@@ -162,7 +193,7 @@ def generator_forward(sd, z, size=256, upto_key_layer=None, record=None):
         if upto_key_layer == n:
             style = modulate(w, p['mod_w'], p['mod_b'])
             return None, style[:, :, None, None] * x
-        r = styled_conv(x, w, p, upsample)
+        r = styled_conv(x, w, p, upsample, blur_kernel)
         if record is not None:
             record['layer%d' % n] = r
         return r['y'], None

@@ -56,7 +56,7 @@ def _layer_list(model):
         want = ['modulation', 'adain', 'dconv'] + (['blur'] if mc.upsample else [])
         if list(mc._modules.keys()) != want or list(sconv._modules.keys()) != ['mconv', 'noise', 'activate']:
             return None
-        if mc.dconv.kernel_size != 3 or not mc.dconv.demodulate:
+        if mc.dconv.kernel_size != 3 or not mc.dconv.demodulate or not sg2.fused_blur_ok(mc):
             return None
         rgb = None
         rgb_lat = None

@@ -183,17 +183,21 @@ def up_fused_eligible(Cin, Cout, H, W, blur_kernel):
 
 def blur_is_separable(kernel):
     """True if the 4x4 FIR is rank one (the model's [1,3,3,1] x [1,3,3,1] always is), which the
-    fused upsampling kernel requires.  One device->host read per kernel tensor version (done in
-    the warm-up pass, never inside a graph capture)."""
+    fused upsampling kernel requires.  The kernel splits the flipped FIR by its corner k[3,3]
+    (csrc/upconv_tc.cu), so that tap must be nonzero too.  One device->host read per kernel tensor
+    object and version (done in the warm-up pass, never inside a graph capture).  An entry holds a
+    weak reference to its tensor: a new kernel allocated at a freed one's address is a miss."""
+    import weakref
     key = (kernel.data_ptr(), kernel._version, tuple(kernel.shape))
-    r = _SEPARABLE.get(key)
-    if r is None:
-        k = kernel.detach().double().cpu()
-        r = bool(tuple(k.shape) == (4, 4) and k[0, 0] != 0 and
-                 torch.equal(k * k[0, 0], torch.outer(k[:, 0], k[0, :])))
-        if len(_SEPARABLE) > 64:
-            _SEPARABLE.clear()
-        _SEPARABLE[key] = r
+    ent = _SEPARABLE.get(key)
+    if ent is not None and ent[0]() is kernel:
+        return ent[1]
+    k = kernel.detach().double().cpu()
+    r = bool(tuple(k.shape) == (4, 4) and k[0, 0] != 0 and k[3, 3] != 0 and
+             torch.equal(k * k[0, 0], torch.outer(k[:, 0], k[0, :])))
+    if len(_SEPARABLE) > 64:
+        _SEPARABLE.clear()
+    _SEPARABLE[key] = (weakref.ref(kernel), r)
     return r
 
 
@@ -563,6 +567,10 @@ def conv_transpose_leaf(k, style, weight, demodulate=True):
 
 def styled_conv(x, style, weight, noise_weight=None, bias=None, upsample=False, blur_kernel=None,
                 demodulate=True, with_noise=True, with_act=True, pre_modulated=False):
+    if upsample and (blur_kernel is None or tuple(blur_kernel.shape) != (4, 4)):
+        # every upsampling kernel (fused, blur_up_act, blur_adj_phase) reads 16 taps with pad (1, 1)
+        raise _cabi.RwError('styled_conv(upsample=True) takes a 4x4 blur kernel (pad (1, 1)); got %s'
+                            % (None if blur_kernel is None else tuple(blur_kernel.shape),))
     return StyledConvFunction.apply(x, style, weight, noise_weight, bias, upsample, blur_kernel,
                                     demodulate, with_noise, with_act, pre_modulated,
                                     _WeightHolder(weight))

@@ -298,6 +298,15 @@ def _blur_pads(blur_kernel, kernel_size, factor=2):
     return (p + 1) // 2 + factor - 1, p // 2 + 1
 
 
+def fused_blur_ok(mconv):
+    """False if an upsampling mconv's blur is anything but a 4x4 FIR with pad (1, 1), the only
+    blur the fused upsampling kernels implement; such layers run leaf by leaf (BlurF is the
+    generic upfirdn2d)."""
+    if not mconv.upsample:
+        return True
+    return tuple(mconv.blur.kernel.shape) == (4, 4) and tuple(mconv.blur.pad) == (1, 1)
+
+
 class DemodulatedConv2dF(nn.Module):
     """conv(k, scale*W) * demod(W, style) on an already-modulated key k = d.fmap.
     This leaf is the rewriter's linear associative memory; its `weight` is the edited
@@ -441,7 +450,7 @@ class StyledConvSeq(nn.Sequential):
                 return False
         else:
             return False
-        return not _is_hooked(self)
+        return fused_blur_ok(mc) and not _is_hooked(self)
 
     def forward(self, d):
         if not self._fusable(d):

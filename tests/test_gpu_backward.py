@@ -149,7 +149,7 @@ def test_wgrad_and_style_grad_finish_vs_torch(B, Cout, Cin, demod):
 # ------------------------------------------------------------------------------------------
 # layer level: every gradient of the fused StyledConv vs autograd of the oracle
 # ------------------------------------------------------------------------------------------
-def _oracle_layer(x, style, weight, nw, bias, up, demodulate, with_noise, with_act):
+def _oracle_layer(x, style, weight, nw, bias, up, demodulate, with_noise, with_act, kern=None):
     """CPU fp32 restatement of one StyledConv with optional pieces (oracle building blocks)."""
     B = x.shape[0]
     k = style[:, :, None, None] * x
@@ -163,7 +163,7 @@ def _oracle_layer(x, style, weight, nw, bias, up, demodulate, with_noise, with_a
         else:
             t = torch.nn.functional.conv2d(k, w, padding=1)
     if up:
-        t = orc.upfirdn2d(t, _kern(), pad=(1, 1))
+        t = orc.upfirdn2d(t, _kern() if kern is None else kern, pad=(1, 1))
     if with_noise:
         H, W = t.shape[2:]
         t = t + nw * orc.noise_table(B, H * W).view(B, 1, H, W)
@@ -172,7 +172,13 @@ def _oracle_layer(x, style, weight, nw, bias, up, demodulate, with_noise, with_a
     return t
 
 
-@pytest.mark.parametrize('B,Cin,Cout,H,W,up,demod,noise,act', [
+def _sym_then(cases, extra):
+    """parameter sets: `cases` with the model's blur ('sym', ids unchanged), then `extra`."""
+    return ([pytest.param(*c, 'sym', id='-'.join(map(str, c))) for c in cases] +
+            [pytest.param(*c, id='-'.join(map(str, c))) for c in extra])
+
+
+@pytest.mark.parametrize('B,Cin,Cout,H,W,up,demod,noise,act,blur', _sym_then([
     (2, 128, 128, 6, 7, False, True, True, True),
     (2, 256, 128, 5, 6, True, True, True, True),       # Cin != Cout, upsampling (layer-13 shape)
     (2, 128, 256, 8, 8, False, True, True, True),      # vectorised planes
@@ -181,8 +187,14 @@ def _oracle_layer(x, style, weight, nw, bias, up, demodulate, with_noise, with_a
     (2, 128, 128, 6, 5, False, True, False, False),    # conv + demod only (target ends at dconv)
     (2, 128, 128, 3, 5, True, True, False, False),     # up, conv + blur only
     (3, 128, 128, 16, 16, False, True, True, True),
-])
-def test_styled_conv_backward_variants_vs_oracle_autograd(B, Cin, Cout, H, W, up, demod, noise, act):
+], [
+    # upsampling with an FIR that changes under flips and transposition: the forward's taps and
+    # the adjoint taps of rw_blur_adj_phase_keys in the backward
+    (2, 256, 128, 5, 6, True, True, True, True, 't'),    # round-1 pair (H != W)
+    (2, 128, 128, 8, 8, True, True, True, True, 't'),    # fused forward (square, power of two)
+]))
+def test_styled_conv_backward_variants_vs_oracle_autograd(B, Cin, Cout, H, W, up, demod, noise, act,
+                                                          blur):
     from rewriting_b200 import ops
     torch.manual_seed(11)
     x = torch.randn(B, Cin, H, W, requires_grad=True)
@@ -192,14 +204,17 @@ def test_styled_conv_backward_variants_vs_oracle_autograd(B, Cin, Cout, H, W, up
     bias = torch.randn(Cout, requires_grad=True)
     Ho, Wo = (2 * H, 2 * W) if up else (H, W)
     gy = torch.randn(B, Cout, Ho, Wo)
-    ref = _oracle_layer(x, style, weight, nw, bias, up, demod, noise, act)
+    kern = orc.blur_case(blur)
+    ref = _oracle_layer(x, style, weight, nw, bias, up, demod, noise, act, kern)
     ref.backward(gy)
     xc = x.detach().cuda().requires_grad_(True)
     sc = style.detach().cuda().requires_grad_(True)
     wc = torch.nn.Parameter(weight.detach().cuda())
     nc = torch.nn.Parameter(nw.detach().cuda())
     bc = torch.nn.Parameter(bias.detach().cuda())
-    y = ops.styled_conv(xc, sc, wc, nc, bc, upsample=up, blur_kernel=_kern().cuda() if up else None,
+    if up:
+        assert ops.up_fused_eligible(Cin, Cout, H, W, kern) == (H == W)
+    y = ops.styled_conv(xc, sc, wc, nc, bc, upsample=up, blur_kernel=kern.cuda() if up else None,
                         demodulate=demod, with_noise=noise, with_act=act)
     assert (y.detach().cpu() - ref.detach()).abs().max().item() < 2e-4 * max(1.0, ref.abs().max().item())
     y.backward(gy.cuda())

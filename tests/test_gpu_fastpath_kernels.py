@@ -144,10 +144,19 @@ def test_blur_up_fused_vs_layer_kernels(B, C, H, W, separable):
         assert v[:, Ho].abs().max() == 0 and v[:, :, Wo].abs().max() == 0   # pad row / column
 
 
-@pytest.mark.parametrize('B,Cin,Cout,H', [(2, 64, 16, 4), (3, 128, 32, 8), (5, 64, 48, 16),
-                                          (2, 128, 32, 32), (3, 64, 16, 64), (2, 64, 32, 128),
-                                          (33, 64, 16, 4)])
-def test_modconv_up_fused_vs_oracle(B, Cin, Cout, H):
+def _sym_then(cases, extra):
+    """parameter sets: `cases` with the model's blur ('sym', ids unchanged), then `extra`."""
+    return ([pytest.param(*c, 'sym', id='-'.join(map(str, c))) for c in cases] +
+            [pytest.param(*c, id='-'.join(map(str, c))) for c in extra])
+
+
+@pytest.mark.parametrize('B,Cin,Cout,H,blur', _sym_then(
+    [(2, 64, 16, 4), (3, 128, 32, 8), (5, 64, 48, 16), (2, 128, 32, 32), (3, 64, 16, 64),
+     (2, 64, 32, 128), (33, 64, 16, 4)],
+    # asymmetric rank-one FIRs: the kv / kh split and the horizontal neighbours, within a lane
+    # quarter (W < 32) and through the cross-quarter mailbox (W > 32)
+    [(3, 128, 32, 8, 'np'), (3, 64, 16, 64, 'np'), (3, 128, 32, 8, 't'), (3, 64, 16, 64, 't')]))
+def test_modconv_up_fused_vs_oracle(B, Cin, Cout, H, blur):
     """ONE kernel for conv_transpose + blur + demod + noise + bias + leaky-ReLU + next style ->
     bf16 planes (csrc/upconv_tc.cu) against the oracle's DemodulatedConv2dF(upsample) -> BlurF ->
     NoiseInjectionF -> FusedLeakyReLUF chain (models.py:313-329, 275-281, 535-546) on the CPU."""
@@ -161,7 +170,8 @@ def test_modconv_up_fused_vs_oracle(B, Cin, Cout, H):
     nw = torch.tensor([0.37])
     bias = torch.randn(Cout)
     nscale = torch.randn(B, Cout) * 0.5 + 1
-    kern = orc.make_kernel([1, 3, 3, 1]) * 4
+    kern = orc.blur_case(blur)
+    assert ops.blur_is_separable(kern)
     # oracle (CPU fp32)
     k = style[:, :, None, None] * x
     t = orc.demod_conv(k, style, weight, True)
@@ -192,9 +202,12 @@ def test_modconv_up_fused_vs_oracle(B, Cin, Cout, H):
     assert err < 2e-4 * max(1.0, want.abs().max().item()), err
 
 
-@pytest.mark.parametrize('B,H,demod,noise,act', [(3, 8, True, True, True), (2, 32, False, False, False),
-                                                 (2, 64, True, False, True), (5, 16, False, True, False)])
-def test_modconv_up_fused_layer_level_vs_oracle(B, H, demod, noise, act):
+@pytest.mark.parametrize('B,H,demod,noise,act,blur', _sym_then(
+    [(3, 8, True, True, True), (2, 32, False, False, False), (2, 64, True, False, True),
+     (5, 16, False, True, False)],
+    [(3, 8, True, True, True, 'np'), (2, 64, True, True, True, 'np'),
+     (3, 8, True, True, True, 't'), (2, 64, True, True, True, 't')]))
+def test_modconv_up_fused_layer_level_vs_oracle(B, H, demod, noise, act, blur):
     """The same kernel in its layer-level mode (rw_modconv_up_fused_y: y as fp32 NCHW, optional
     demodulation / noise / bias + activation) — what the autograd op of an upsampling StyledConv
     launches — against the oracle chain, through ops.styled_conv."""
@@ -206,7 +219,7 @@ def test_modconv_up_fused_layer_level_vs_oracle(B, H, demod, noise, act):
     style = torch.randn(B, Cin) * 0.5 + 1
     weight = torch.randn(1, Cout, Cin, 3, 3)
     nw, bias = torch.tensor([0.37]), torch.randn(Cout)
-    kern = orc.make_kernel([1, 3, 3, 1]) * 4
+    kern = orc.blur_case(blur)
     k = style[:, :, None, None] * x
     if demod:
         t = orc.demod_conv(k, style, weight, True)

@@ -85,9 +85,11 @@ def _direction(rank, cin=512, seed=5):
 
 
 def _target_fn(sd, layer, k, style, dtype=torch.float32):
-    """The odd layer's target model on key crop k (k already modulated), as the oracle states it."""
+    """The odd layer's target model on key crop k (k already modulated), as the oracle states it,
+    with the layer's own blur kernel."""
     p = orc._layer_params(sd, 'layer%d' % layer)
-    kern = (orc.make_kernel([1, 3, 3, 1]) * 4).to(dtype)
+    kern = sd['layer%d.sconv.mconv.blur.kernel' % layer].cpu().to(dtype)
+    assert tuple(kern.shape) == (4, 4)
     B, _, h, w = k.shape
     n = orc.noise_table(B, 4 * h * w, dtype).view(B, 1, 2 * h, 2 * w)
     nw, bias = p['noise_w'].cpu().to(dtype), p['bias'].cpu().to(dtype)
@@ -271,6 +273,30 @@ def test_tight_crops_at_every_odd_layer_vs_oracle(cuda_model, zds, layer, ys, xs
     W0, W_orc = _oracle(gw, layer, gin, gout, d, NITER, 0.05)
     assert (W.cpu() - W_orc).abs().max().item() < 1e-4, layer
     assert (W_orc - W0).abs().max().item() > 1e-3, layer
+
+
+@pytest.mark.parametrize('blur', ['t', 'ns'])
+def test_tight_crop_layer9_other_blur_kernels_vs_oracle(cuda_model, zds, blur):
+    """The kernel applies the layer's blur flipped and its adjoint with no symmetry or
+    separability assumed: with the layer-9 blur buffer replaced by an FIR that changes under
+    flips and transposition ('t'), and by one that is not separable either ('ns')."""
+    kbuf = cuda_model.layer9.sconv.mconv.blur.kernel
+    saved = kbuf.clone()
+    try:
+        with torch.no_grad():
+            kbuf.copy_(orc.blur_case(blur))
+        gw = _rewriter(cuda_model, zds, 9)
+        gin, gout = _crop_goal(gw, [0], slice(8, 14), slice(10, 15))
+        d = _direction(1)
+        plan = gw._fused_up_plan(gin, gout, d.cuda())
+        assert plan[0] == UP and torch.equal(torch.tensor(plan[-1]), orc.blur_case(blur).reshape(16))
+        W = _run(gw, gin, gout, d.cuda(), NITER, 0.05)
+        W0, W_orc = _oracle(gw, 9, gin, gout, d, NITER, 0.05)
+    finally:
+        with torch.no_grad():
+            kbuf.copy_(saved)
+    assert (W.cpu() - W_orc).abs().max().item() < 1e-4
+    assert (W_orc - W0).abs().max().item() > 1e-3
 
 
 @pytest.mark.parametrize('lrg', [False, True])

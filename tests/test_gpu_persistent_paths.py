@@ -404,11 +404,15 @@ def test_insert_wide_batch_of_four_vs_oracle():
 
 
 # ================================================================== pipelined blur
-@pytest.mark.parametrize('separable', [True, False])
-def test_blur_up_pipelined_every_cta_two_tiles_ragged_vs_fp64(separable):
+@pytest.mark.parametrize('separable,blur', [pytest.param(True, 'sym', id='True'),
+                                            pytest.param(False, 'sym', id='False'),
+                                            pytest.param(True, 't', id='True-t')])
+def test_blur_up_pipelined_every_cta_two_tiles_ragged_vs_fp64(separable, blur):
     """rw_blur_up_fused with planes only takes the persistent, double-buffered kernel.  At B = 8,
     C = 128 and a 32x32 input there are 720 tiles of 8x16 outputs x 64 channels: every CTA runs at
-    least two (so it prefetches into its second buffer) and the last round is ragged."""
+    least two (so it prefetches into its second buffer) and the last round is ragged.  'sym' and
+    't' take the separable branch; 't' changes under flips and transposition, so it also catches
+    taps read in the wrong orientation there."""
     from rewriting_b200 import _cabi, ops
     B, C, H, W = 8, 128, 32, 32
     Ho, Wo = 2 * H, 2 * W
@@ -418,8 +422,10 @@ def test_blur_up_pipelined_every_cta_two_tiles_ragged_vs_fp64(separable):
     dev = 'cuda'
     g = torch.Generator().manual_seed(31 + separable)
     t = torch.randn(B, C, 2 * H + 1, 2 * W + 1, generator=g)
-    kern = orc.make_kernel([1, 3, 3, 1]) * 4
-    if not separable:
+    kern = orc.blur_case(blur)
+    if separable:
+        assert ops.blur_is_separable(kern)
+    else:
         kern = kern + 0.03 * torch.randn(4, 4, generator=g)     # asymmetric: also catches a wrong flip
         assert torch.linalg.matrix_rank(kern.double()) > 1
     nw, bias = torch.tensor([0.37]), torch.randn(C, generator=g)
