@@ -186,7 +186,8 @@ int rw_upfirdn2d(const float* in, const float* kernel, int major, int in_h, int 
 
 /* ---- key second moment / weight gradient (wgmma col-GEMM) ---- */
 size_t rw_gram_workspace_bytes(int Cm, int Cn, long long rows, int ntaps);
-/* mom2[C,C] += sum_r a_r a_r^T over `rows` rows of the hi/lo planes [rows][C] */
+/* mom2[C,C] += sum_r a_r a_r^T over `rows` rows of the hi/lo planes [rows][C]; C % 64 == 0 (the
+ * col-GEMM takes channel counts in multiples of 64, tiles of 128 where the count allows) */
 int rw_second_moment_accum(const void* hi, const void* lo, long long rows, int C, float* mom2,
                            void* workspace, size_t workspace_bytes, rw_stream_t stream);
 /* dW[o][tap][i] = sum_p G[p,o] * K[p + shift(tap), i]  for a 3x3 conv over the padded-flat grid
@@ -324,7 +325,7 @@ int rw_linear_insert_loop_up(const rw_linear_insert_args* args, const float blur
                              void* workspace, size_t workspace_bytes, rw_stream_t stream);
 
 /* out[rows][N] = A[rows][K] . W[N][K]^T on the tensor-core row-GEMM (3-term split bf16 planes from
- * rw_split_rows; K % 64 == 0, N % 128 == 0): the key algebra between key capture and the
+ * rw_split_rows; K % 64 == 0, N % 64 == 0): the key algebra between key capture and the
  * direction d — ZCA . k and ZCA . v of ganrewrite.py:107-110, 339-374 — without a cuBLAS call */
 int rw_rowgemm(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo, int rows, int K,
                int N, float* out, rw_stream_t stream);

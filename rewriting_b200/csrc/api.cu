@@ -641,9 +641,9 @@ int rw_upfirdn2d(const float* in, const float* kernel, int major, int in_h, int 
 }
 
 size_t rw_gram_workspace_bytes(int Cm, int Cn, long long rows, int ntaps) {
-  if (Cm < 128 || Cn < 128 || ntaps < 1) return 0;
-  const int mt = Cm / 128, nt = Cn / 128;
-  const int tiles_full = mt * nt;
+  if (Cm < 64 || Cn < 64 || Cm % 64 != 0 || Cn % 64 != 0 || ntaps < 1) return 0;
+  const int mt = Cm / gram_tile_width(Cm);
+  const int tiles_full = gram_tiles(Cm, Cn);
   // the symmetric path uses fewer tiles -> more splits; size for the larger of the two
   const int tiles_sym = (Cm == Cn) ? mt * (mt + 1) / 2 : tiles_full;
   const int s1 = gram_splits(tiles_full, rows, ntaps);
@@ -655,7 +655,7 @@ size_t rw_gram_workspace_bytes(int Cm, int Cn, long long rows, int ntaps) {
 int rw_second_moment_accum(const void* hi, const void* lo, long long rows, int C, float* mom2,
                            void* workspace, size_t workspace_bytes, rw_stream_t stream) {
   if (rows == 0) return RW_OK;
-  if (!hi || !lo || !mom2 || !workspace || rows < 0 || rows > 0x7fffffffLL || C % 128 != 0) {
+  if (!hi || !lo || !mom2 || !workspace || rows < 0 || rows > 0x7fffffffLL || C < 64 || C % 64 != 0) {
     set_last_error("rw_second_moment_accum: bad argument (rows=%lld C=%d)", rows, C);
     return RW_ERR_BAD_ARG;
   }
@@ -666,7 +666,7 @@ int rw_second_moment_accum(const void* hi, const void* lo, long long rows, int C
   p.Cm = p.Cn = C;
   p.ntaps = 1;
   p.upper_only = 1;
-  const int mt = C / 128;
+  const int mt = C / gram_tile_width(C);
   p.splits = gram_splits(mt * (mt + 1) / 2, rows, 1);
   p.ldp = C;
   p.partial = static_cast<float*>(workspace);
@@ -702,7 +702,7 @@ int rw_conv_wgrad(const void* g_hi, const void* g_lo, const void* kp_hi, const v
       p.tap_col_ofs[u * 3 + v] = (u * 3 + v) * Cin;
     }
   p.upper_only = 0;
-  p.splits = gram_splits((Cout / 128) * (Cin / 128), rows, 9);
+  p.splits = gram_splits(gram_tiles(Cout, Cin), rows, 9);
   p.ldp = 9LL * Cin;
   p.partial = static_cast<float*>(workspace);
   const size_t need = static_cast<size_t>(p.splits) * Cout * 9 * Cin * sizeof(float);
@@ -774,7 +774,7 @@ int rw_conv_up_wgrad(const void* gph_hi, const void* gph_lo, const void* kp_hi, 
       p.tap_acol[t] = ((u & 1) * 2 + (v & 1)) * Cout;
       p.tap_col_ofs[t] = t * Cin;
     }
-  p.splits = gram_splits((Cout / 128) * (Cin / 128), rows, 9);
+  p.splits = gram_splits(gram_tiles(Cout, Cin), rows, 9);
   p.ldp = 9LL * Cin;
   p.partial = static_cast<float*>(workspace);
   const size_t need = static_cast<size_t>(p.splits) * Cout * 9 * Cin * sizeof(float);
@@ -966,7 +966,7 @@ int rw_debug_rowgemm(const void* a_hi, const void* a_lo, const void* w_hi, const
 
 int rw_rowgemm(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo, int rows, int K,
                int N, float* out, rw_stream_t stream) {
-  if (!a_hi || !a_lo || !w_hi || !w_lo || !out || rows < 1 || K % 64 != 0 || N % 128 != 0) {
+  if (!a_hi || !a_lo || !w_hi || !w_lo || !out || rows < 1 || K % 64 != 0 || N % 64 != 0) {
     set_last_error("rw_rowgemm: bad argument (rows=%d K=%d N=%d)", rows, K, N);
     return RW_ERR_BAD_ARG;
   }
@@ -979,7 +979,7 @@ int rw_debug_colgemm(const void* a_hi, const void* a_lo, const void* b_hi, const
   GramTcParams p;
   memset(&p, 0, sizeof(p));
   p.rows = rows; p.rows_a = p.rows_b = rows; p.Cm = Cm; p.Cn = Cn; p.ntaps = 1;
-  p.splits = gram_splits((Cm / 128) * (Cn / 128), rows, 1);
+  p.splits = gram_splits(gram_tiles(Cm, Cn), rows, 1);
   p.ldp = Cn;
   p.partial = static_cast<float*>(workspace);
   const size_t need = static_cast<size_t>(p.splits) * Cm * Cn * sizeof(float);

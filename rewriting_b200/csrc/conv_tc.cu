@@ -38,7 +38,7 @@ namespace rw {
 namespace {
 
 constexpr int BM = 128;
-constexpr int BN = 128;
+// the tile's output channels, BN, is a template parameter: 128, or 64 where Cout % 128 != 0
 // k-block of 32 channels = one 64-byte swizzle row: a 32 KB stage, so that seven fit in shared
 // memory and the producer runs up to six k-blocks ahead of the MMAs
 constexpr int BK = 32;
@@ -58,15 +58,16 @@ constexpr int kCluster = 2;
 // (K=512 -> pixel error 5.2e-4, K=1024 -> 8.1e-4, K >= 2304 fails the 1e-3 bound)
 constexpr int kChunkKB = 16;
 
+template <int BN>
 struct ConvSmem {
   static constexpr int kABytes = BM * BK * 2;          // one plane: 8 KB
-  static constexpr int kBBytes = BN * BK * 2;          // one plane: 8 KB
+  static constexpr int kBBytes = BN * BK * 2;          // one plane: 8 KB (BN = 64: 4 KB)
   static constexpr int kStageBytes = 2 * kABytes + 2 * kBBytes;
   static constexpr int kTotal = kStages * kStageBytes + 512 /*align slack*/ + 256 /*barriers*/;
 };
 // 512-byte alignment serves the 64-byte swizzle atoms; the total must stay within the 227 KB a
 // block may opt in to
-static_assert(ConvSmem::kTotal <= 232448, "conv_tc: shared memory over the per-block limit");
+static_assert(ConvSmem<128>::kTotal <= 232448, "conv_tc: shared memory over the per-block limit");
 
 struct Barriers {
   uint64_t full[kStages];
@@ -89,7 +90,10 @@ __device__ __forceinline__ void decode_tile(int tile, int nphase, int nsched, in
 //          conv_transpose phases, dgrad and the plain row-GEMM use it.
 // PROF = true: bring-up variant that accumulates, per consumer warp, the cycles of each phase of a
 // tile (tools/prof_conv.py) into p.debug_prof; the product launches PROF = false.
-template <int EPI, bool PROF>
+// BN = 64 (Cout % 128 != 0, the 64-channel layers of the 512² generator): wgmma.m64n64k16 on a
+// 64-row weight tile, still multicast as two 32-row halves across the CTA pair; the epilogue is
+// the same code over 32 accumulators per thread instead of 64.
+template <int BN, int EPI, bool PROF>
 __global__ void __launch_bounds__(kNumThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
                const __grid_constant__ CUtensorMap map_a_lo,
@@ -98,7 +102,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 511) &
                                              ~static_cast<uintptr_t>(511));
-  using S = ConvSmem;
+  using S = ConvSmem<BN>;
+  constexpr int NR = BN / 2;    // accumulator registers per thread
+  constexpr int NJ = BN / 8;    // 8-column groups per thread row
   Barriers* bars = reinterpret_cast<Barriers*>(smem + kStages * S::kStageBytes);
 
   // broadcast from lane 0: the compiler then knows the role branches are warp-uniform, which it
@@ -165,9 +171,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
       const int n0 = n_tile * BN;
       const int m0 = ((mn / n_tiles) * kCluster + rank) * BM;
 
-      float acc[64], d[64];
+      float acc[NR], d[NR];
 #pragma unroll
-      for (int j = 0; j < 64; ++j) acc[j] = 0.f;
+      for (int j = 0; j < NR; ++j) acc[j] = 0.f;
       for (int kb0 = 0; kb0 < num_kb; kb0 += kChunkKB) {
         const int kb_end = (kb0 + kChunkKB < num_kb) ? kb0 + kChunkKB : num_kb;
         // one wgmma group stays in flight: a stage is released once the group after it has been
@@ -187,9 +193,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
           for (int kk = 0; kk < BK / MMA_K; ++kk) {
             const uint64_t adv = static_cast<uint64_t>((kk * MMA_K * 2) >> 4);
             // smallest terms first, then the dominant hi*hi product
-            wgmma_m64n128<0, 0>(d, da_lo + adv, db_hi + adv, ((kb - kb0) | kk) != 0);
-            wgmma_m64n128<0, 0>(d, da_hi + adv, db_lo + adv, 1u);
-            wgmma_m64n128<0, 0>(d, da_hi + adv, db_hi + adv, 1u);
+            wgmma_m64nN<0, 0>(d, da_lo + adv, db_hi + adv, ((kb - kb0) | kk) != 0);
+            wgmma_m64nN<0, 0>(d, da_hi + adv, db_lo + adv, 1u);
+            wgmma_m64nN<0, 0>(d, da_hi + adv, db_hi + adv, 1u);
           }
           wgmma_commit();
           wgmma_wait<1>();
@@ -204,7 +210,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
         wgmma_wait<0>();
         release(held);
 #pragma unroll
-        for (int j = 0; j < 64; ++j) acc[j] += d[j];
+        for (int j = 0; j < NR; ++j) acc[j] += d[j];
         if constexpr (PROF) prof[2] += clk() - tp0;
       }
       if constexpr (PROF) tp0 = clk();
@@ -234,7 +240,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
           // lean epilogue, and the pad rows of the full one: only the optional scale
           if (scl && (EPI == 1 || p.out_mode == 1)) {
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
+            for (int j = 0; j < NJ; ++j) {
               const float2 sv = __ldg(reinterpret_cast<const float2*>(scl + n0 + 8 * j + 2 * c));
               acc[4 * j + 2 * i] *= sv.x;
               acc[4 * j + 2 * i + 1] *= sv.y;
@@ -242,7 +248,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
           }
           if (EPI == 1 && outp) {
 #pragma unroll
-            for (int j = 0; j < 16; ++j)
+            for (int j = 0; j < NJ; ++j)
 #pragma unroll
               for (int e = 0; e < 2; ++e)
                 outp[static_cast<size_t>(n0 + 8 * j + 2 * c + e) * p.out_sc] = acc[4 * j + 2 * i + e];
@@ -261,44 +267,44 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
           if (scl) {
             const float* sc = scl + n0 + 2 * c;
 #pragma unroll
-            for (int j = 0; j < 16; ++j)
+            for (int j = 0; j < NJ; ++j)
 #pragma unroll
               for (int e = 0; e < 2; ++e) acc[4 * j + 2 * i + e] *= __ldg(sc + 8 * j + e);
           }
 #pragma unroll
-          for (int j = 0; j < 16; ++j)
+          for (int j = 0; j < NJ; ++j)
 #pragma unroll
             for (int e = 0; e < 2; ++e) acc[4 * j + 2 * i + e] += nz;
           if (p.bias) {
             const float* bi = p.bias + n0 + 2 * c;
 #pragma unroll
-            for (int j = 0; j < 16; ++j)
+            for (int j = 0; j < NJ; ++j)
 #pragma unroll
               for (int e = 0; e < 2; ++e) acc[4 * j + 2 * i + e] += __ldg(bi + 8 * j + e);
           }
           if (p.act) {
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
+            for (int j = 0; j < 2 * NJ; ++j) {
               float& t = acc[4 * (j >> 1) + 2 * i + (j & 1)];
               t = (t > 0.f ? t : 0.2f * t) * act_gain;
             }
           }
           if (outp) {
 #pragma unroll
-            for (int j = 0; j < 16; ++j)
+            for (int j = 0; j < NJ; ++j)
 #pragma unroll
               for (int e = 0; e < 2; ++e)
                 outp[static_cast<size_t>(n0 + 8 * j + 2 * c + e) * p.out_sc] = acc[4 * j + 2 * i + e];
           }
         }
         if (EPI == 0 && p.rgb_w != nullptr) {
-          // one partial per 64-channel group: rgb_part[(n_tile*2 + half)][b][c][y*Wv+x]; the four
-          // lanes of a row hold 16 of the group's channels each
+          // one partial per 64-channel group: rgb_part[(n_tile*BN/64 + half)][b][c][y*Wv+x]; the
+          // four lanes of a row hold 16 of the group's channels each
           const float* rw0 = p.rgb_w + (static_cast<size_t>(valid ? b : 0) * 3) * p.Cout + n0 + 2 * c;
           const float* rw1 = rw0 + p.Cout;
           const float* rw2 = rw1 + p.Cout;
 #pragma unroll
-          for (int half = 0; half < 2; ++half) {
+          for (int half = 0; half < BN / 64; ++half) {
             float r0 = 0.f, r1 = 0.f, r2 = 0.f;
             if (valid) {
 #pragma unroll
@@ -319,7 +325,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
             }
             if (valid && c == 0) {
               const size_t hw = static_cast<size_t>(Hv) * Wv;
-              float* rp = p.rgb_part + ((static_cast<size_t>(n_tile * 2 + half) * p.B + b) * 3) * hw +
+              float* rp = p.rgb_part + ((static_cast<size_t>(n_tile * (BN / 64) + half) * p.B + b) * 3) * hw +
                           static_cast<size_t>(yy) * Wv + xx;
               rp[0] = r0;
               rp[hw] = r1;
@@ -331,7 +337,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
         if (p.out != nullptr && p.out_mode == 1 && in_rows) {
           float* orow = p.out + (static_cast<size_t>(ph) * p.rows + prow) * p.Cout + n0 + 2 * c;
 #pragma unroll
-          for (int j = 0; j < 16; ++j)
+          for (int j = 0; j < NJ; ++j)
             *reinterpret_cast<float2*>(orow + 8 * j) = make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
         }
         if (EPI == 0 && p.next_hi != nullptr && in_rows) {
@@ -340,7 +346,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
           uint32_t* nh = reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(p.next_hi) + ofs);
           uint32_t* nl = reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(p.next_lo) + ofs);
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
+          for (int j = 0; j < NJ; ++j) {
             float k0 = 0.f, k1 = 0.f;
             if (valid) {
               const float2 sv = __ldg(reinterpret_cast<const float2*>(ns + 8 * j));
@@ -410,7 +416,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
 
 }  // namespace
 
-template <int EPI, bool PROF>
+template <int BN, int EPI, bool PROF>
 static int conv_tc_launch_epi(const ConvTcParams& p, const void* a_hi, const void* a_lo,
                               const void* w_hi, const void* w_lo, int wk_total,
                               cudaStream_t stream) {
@@ -434,7 +440,7 @@ static int conv_tc_launch_epi(const ConvTcParams& p, const void* a_hi, const voi
   attr[0].val.clusterDim.y = 1;
   attr[0].val.clusterDim.z = 1;
   cfg.blockDim = dim3(kNumThreads);
-  cfg.dynamicSmemBytes = ConvSmem::kTotal;
+  cfg.dynamicSmemBytes = ConvSmem<BN>::kTotal;
   cfg.stream = stream;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
@@ -442,12 +448,12 @@ static int conv_tc_launch_epi(const ConvTcParams& p, const void* a_hi, const voi
   // SMs cannot host a whole cluster, so this is fewer than SMs / kCluster)
   static int max_clusters = 0;
   if (max_clusters == 0) {
-    rc = check_cuda(cudaFuncSetAttribute(conv_tc_kernel<EPI, PROF>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, ConvSmem::kTotal),
+    rc = check_cuda(cudaFuncSetAttribute(conv_tc_kernel<BN, EPI, PROF>,
+                                         cudaFuncAttributeMaxDynamicSharedMemorySize, ConvSmem<BN>::kTotal),
                     "conv_tc smem attr");
     if (rc) return rc;
     cfg.gridDim = dim3(kCluster * (device_sm_count() / kCluster));
-    rc = check_cuda(cudaOccupancyMaxActiveClusters(&max_clusters, conv_tc_kernel<EPI, PROF>, &cfg),
+    rc = check_cuda(cudaOccupancyMaxActiveClusters(&max_clusters, conv_tc_kernel<BN, EPI, PROF>, &cfg),
                     "conv_tc cluster occupancy");
     if (rc) return rc;
     if (max_clusters < 1) {
@@ -460,16 +466,27 @@ static int conv_tc_launch_epi(const ConvTcParams& p, const void* a_hi, const voi
   const int num_units = (m_tiles + kCluster - 1) / kCluster * n_tiles * p.nphase;
   const int clusters = max_clusters < num_units ? max_clusters : num_units;
   cfg.gridDim = dim3(kCluster * clusters);
-  rc = check_cuda(cudaLaunchKernelEx(&cfg, conv_tc_kernel<EPI, PROF>, ma_hi, ma_lo, mw_hi, mw_lo, p),
+  rc = check_cuda(cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN, EPI, PROF>, ma_hi, ma_lo, mw_hi, mw_lo, p),
                   "conv_tc launch");
   if (rc) return rc;
   return check_cuda(cudaGetLastError(), "conv_tc launch");
 }
 
+template <int BN>
+static int conv_tc_launch_bn(const ConvTcParams& p, const void* a_hi, const void* a_lo,
+                             const void* w_hi, const void* w_lo, int wk_total, cudaStream_t stream) {
+  // lean epilogue when only the optional scale and the store are asked for
+  const bool lean = !p.noise && !p.bias && !p.act && !p.rgb_w && !p.rgb_part && !p.next_hi &&
+                    p.out != nullptr && (reinterpret_cast<uintptr_t>(p.scale_bo) & 7u) == 0;
+  if (p.debug_prof) return conv_tc_launch_epi<BN, 0, true>(p, a_hi, a_lo, w_hi, w_lo, wk_total, stream);
+  if (lean) return conv_tc_launch_epi<BN, 1, false>(p, a_hi, a_lo, w_hi, w_lo, wk_total, stream);
+  return conv_tc_launch_epi<BN, 0, false>(p, a_hi, a_lo, w_hi, w_lo, wk_total, stream);
+}
+
 int conv_tc_launch(const ConvTcParams& p, const void* a_hi, const void* a_lo, const void* w_hi,
                    const void* w_lo, int wk_total, cudaStream_t stream) {
   // the stated limit (DESIGN.md §1) stays Cin % 64, although the kernel only needs Cin % BK
-  if (p.Cin % 64 != 0 || p.Cout % BN != 0 || p.nphase < 1 || p.nphase > 4 || p.rows <= 0) {
+  if (p.Cin % 64 != 0 || p.Cout % 64 != 0 || p.nphase < 1 || p.nphase > 4 || p.rows <= 0) {
     set_last_error("conv_tc: unsupported shape Cin=%d Cout=%d nphase=%d rows=%d", p.Cin, p.Cout,
                    p.nphase, p.rows);
     return RW_ERR_BAD_ARG;
@@ -479,12 +496,9 @@ int conv_tc_launch(const ConvTcParams& p, const void* a_hi, const void* a_lo, co
       set_last_error("conv_tc: phase %d has %d taps", i, p.ph_ntaps[i]);
       return RW_ERR_BAD_ARG;
     }
-  // lean epilogue when only the optional scale and the store are asked for
-  const bool lean = !p.noise && !p.bias && !p.act && !p.rgb_w && !p.rgb_part && !p.next_hi &&
-                    p.out != nullptr && (reinterpret_cast<uintptr_t>(p.scale_bo) & 7u) == 0;
-  if (p.debug_prof) return conv_tc_launch_epi<0, true>(p, a_hi, a_lo, w_hi, w_lo, wk_total, stream);
-  if (lean) return conv_tc_launch_epi<1, false>(p, a_hi, a_lo, w_hi, w_lo, wk_total, stream);
-  return conv_tc_launch_epi<0, false>(p, a_hi, a_lo, w_hi, w_lo, wk_total, stream);
+  // 128-channel tiles wherever Cout allows them; 64 only for the 64-channel layers
+  if (p.Cout % 128 == 0) return conv_tc_launch_bn<128>(p, a_hi, a_lo, w_hi, w_lo, wk_total, stream);
+  return conv_tc_launch_bn<64>(p, a_hi, a_lo, w_hi, w_lo, wk_total, stream);
 }
 
 }  // namespace rw

@@ -22,33 +22,44 @@ namespace rw {
 
 namespace {
 
-constexpr int TM = 128;
-constexpr int TN = 128;
+// The output tile is TM x TN, each 128 or 64 (gram_tile_width: 64 only where the channel count is
+// not a multiple of 128, as at the 64-channel layers of the 512² generator).
 constexpr int RB = 64;            // rows (contraction) per pipeline stage
 constexpr int MMA_K = 16;
 constexpr int kStages = 3;
-constexpr int kNumThreads = 288;  // warpgroups 0, 1: wgmma + epilogue (64 rows of M each); warp 8: TMA
-constexpr int kTmaWarp = 8;
 // fp32 accumulation in the tensor core truncates (see conv_tc.cu): the wgmma accumulator holds
 // at most kChunkRB row-blocks (1024 rows = 192 accumulations); chunks are summed in fp32
 // registers (round-to-nearest).
 constexpr int kChunkRB = 16;
 constexpr int kBlockBytes = 64 * RB * 2;       // one 64-channel x RB-row box
-constexpr int kPlaneBytes = (TM / 64) * kBlockBytes;
-constexpr int kStageBytes = 4 * kPlaneBytes;   // A_hi, A_lo, B_hi, B_lo
-constexpr int kSmemTotal = kStages * kStageBytes + 1024 + 256;
+template <int TM, int TN>
+struct GramCfg {
+  // one consumer warpgroup per 64 rows of M (wgmma + epilogue), then one TMA warp
+  static constexpr int kConsumers = TM / 64;
+  static constexpr int kNumThreads = kConsumers * 128 + 32;
+  static constexpr int kTmaWarp = kConsumers * 4;
+  static constexpr int kAPlaneBytes = (TM / 64) * kBlockBytes;
+  static constexpr int kBPlaneBytes = (TN / 64) * kBlockBytes;
+  static constexpr int kStageBytes = 2 * kAPlaneBytes + 2 * kBPlaneBytes;  // A_hi, A_lo, B_hi, B_lo
+  static constexpr int kSmemTotal = kStages * kStageBytes + 1024 + 256;
+};
 
 struct Barriers {
   uint64_t full[kStages];
   uint64_t empty[kStages];
 };
 
-__global__ void __launch_bounds__(kNumThreads, 1)
+template <int TM, int TN>
+__global__ void __launch_bounds__(GramCfg<TM, TN>::kNumThreads, 1)
 gram_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
                const __grid_constant__ CUtensorMap map_a_lo,
                const __grid_constant__ CUtensorMap map_b_hi,
                const __grid_constant__ CUtensorMap map_b_lo, const GramTcParams p,
                const int lbo_bytes, const int sbo_bytes) {
+  using G = GramCfg<TM, TN>;
+  constexpr int kTmaWarp = G::kTmaWarp, kStageBytes = G::kStageBytes;
+  constexpr int kAPlane = G::kAPlaneBytes, kBPlane = G::kBPlaneBytes;
+  constexpr int NR = TN / 2;    // accumulator registers per thread
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~static_cast<uintptr_t>(1023));
@@ -92,7 +103,7 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
     tma_prefetch_desc(&map_b_lo);
     for (int s = 0; s < kStages; ++s) {
       mbar_init(&bars->full[s], 1);
-      mbar_init(&bars->empty[s], 2);      // one arrival per consumer warpgroup
+      mbar_init(&bars->empty[s], G::kConsumers);   // one arrival per consumer warpgroup
     }
     fence_mbar_init();
   }
@@ -109,14 +120,18 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
         const int ra = rb * RB + shift_a;
         const int rbb = rb * RB + shift_b;
 #pragma unroll
-        for (int j = 0; j < TM / 64; ++j) {
-          tma_load_2d(st + j * kBlockBytes, &map_a_hi, &bars->full[stage], acol + m0 + j * 64, ra);
-          tma_load_2d(st + kPlaneBytes + j * kBlockBytes, &map_a_lo, &bars->full[stage],
-                      acol + m0 + j * 64, ra);
-          tma_load_2d(st + 2 * kPlaneBytes + j * kBlockBytes, &map_b_hi, &bars->full[stage],
-                      n0 + j * 64, rbb);
-          tma_load_2d(st + 3 * kPlaneBytes + j * kBlockBytes, &map_b_lo, &bars->full[stage],
-                      n0 + j * 64, rbb);
+        for (int j = 0; j < (TM > TN ? TM : TN) / 64; ++j) {
+          if (j < TM / 64) {
+            tma_load_2d(st + j * kBlockBytes, &map_a_hi, &bars->full[stage], acol + m0 + j * 64, ra);
+            tma_load_2d(st + kAPlane + j * kBlockBytes, &map_a_lo, &bars->full[stage],
+                        acol + m0 + j * 64, ra);
+          }
+          if (j < TN / 64) {
+            tma_load_2d(st + 2 * kAPlane + j * kBlockBytes, &map_b_hi, &bars->full[stage],
+                        n0 + j * 64, rbb);
+            tma_load_2d(st + 2 * kAPlane + kBPlane + j * kBlockBytes, &map_b_lo, &bars->full[stage],
+                        n0 + j * 64, rbb);
+          }
         }
         if (++stage == kStages) { stage = 0; phase ^= 1u; }
       }
@@ -126,9 +141,9 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
 
   // warpgroup wg owns the 64 output rows m0 + 64 wg .. : its A operand is the wg-th 64-channel box
   const int wg = threadIdx.x >> 7;
-  float acc[64], d[64];
+  float acc[NR], d[NR];
 #pragma unroll
-  for (int j = 0; j < 64; ++j) acc[j] = 0.f;
+  for (int j = 0; j < NR; ++j) acc[j] = 0.f;
   int stage = 0;
   uint32_t phase = 0;
   for (int i0 = 0; i0 < num_rb; i0 += kChunkRB) {
@@ -137,17 +152,17 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
       mbar_wait(&bars->full[stage], phase);
       const uint32_t sa = smem_u32(smem + stage * kStageBytes);
       const uint64_t da_hi = make_smem_desc(sa + wg * kBlockBytes, lbo_bytes, sbo_bytes);
-      const uint64_t da_lo = make_smem_desc(sa + kPlaneBytes + wg * kBlockBytes, lbo_bytes, sbo_bytes);
-      const uint64_t db_hi = make_smem_desc(sa + 2 * kPlaneBytes, lbo_bytes, sbo_bytes);
-      const uint64_t db_lo = make_smem_desc(sa + 3 * kPlaneBytes, lbo_bytes, sbo_bytes);
+      const uint64_t da_lo = make_smem_desc(sa + kAPlane + wg * kBlockBytes, lbo_bytes, sbo_bytes);
+      const uint64_t db_hi = make_smem_desc(sa + 2 * kAPlane, lbo_bytes, sbo_bytes);
+      const uint64_t db_lo = make_smem_desc(sa + 2 * kAPlane + kBPlane, lbo_bytes, sbo_bytes);
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < RB / MMA_K; ++kk) {
         // 16 rows = two 8-row swizzle groups of 1024 B
         const uint64_t adv = static_cast<uint64_t>((kk * MMA_K * 128) >> 4);
-        wgmma_m64n128<1, 1>(d, da_lo + adv, db_hi + adv, ((i - i0) | kk) != 0);
-        wgmma_m64n128<1, 1>(d, da_hi + adv, db_lo + adv, 1u);
-        wgmma_m64n128<1, 1>(d, da_hi + adv, db_hi + adv, 1u);
+        wgmma_m64nN<1, 1>(d, da_lo + adv, db_hi + adv, ((i - i0) | kk) != 0);
+        wgmma_m64nN<1, 1>(d, da_hi + adv, db_lo + adv, 1u);
+        wgmma_m64nN<1, 1>(d, da_hi + adv, db_hi + adv, 1u);
       }
       wgmma_commit();
       wgmma_wait<0>();
@@ -155,7 +170,7 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
       if (++stage == kStages) { stage = 0; phase ^= 1u; }
     }
 #pragma unroll
-    for (int j = 0; j < 64; ++j) acc[j] += d[j];
+    for (int j = 0; j < NR; ++j) acc[j] += d[j];
   }
   // rows m0 + 64 wg + 16 (warp % 4) + lane / 4 (+ 8), columns 8 j + 2 (lane % 4) (+ 1)
   const int row = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
@@ -163,7 +178,7 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
 #pragma unroll
   for (int i = 0; i < 2; ++i)
 #pragma unroll
-    for (int j = 0; j < 16; ++j)
+    for (int j = 0; j < TN / 8; ++j)
       *reinterpret_cast<float2*>(dst + static_cast<size_t>(8 * i) * p.ldp + 8 * j) =
           make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
 }
@@ -232,9 +247,32 @@ static int g_gram_lbo = kBlockBytes;
 static int g_gram_sbo = 1024;
 void gram_tc_set_desc(int lbo, int sbo) { g_gram_lbo = lbo; g_gram_sbo = sbo; }
 
+template <int TM, int TN>
+static int gram_tc_launch_tile(const GramTcParams& p, const CUtensorMap& ma_hi,
+                               const CUtensorMap& ma_lo, const CUtensorMap& mb_hi,
+                               const CUtensorMap& mb_lo, cudaStream_t stream) {
+  using G = GramCfg<TM, TN>;
+  static bool attr_set = false;
+  if (!attr_set) {
+    int rc = check_cuda(cudaFuncSetAttribute(gram_tc_kernel<TM, TN>,
+                                             cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             G::kSmemTotal),
+                        "gram_tc smem attr");
+    if (rc) return rc;
+    attr_set = true;
+  }
+  const int mt = p.Cm / TM, nt = p.Cn / TN;
+  const int tiles = p.upper_only ? mt * (mt + 1) / 2 : mt * nt;
+  dim3 grid(tiles, p.splits, p.ntaps);
+  gram_tc_kernel<TM, TN><<<grid, G::kNumThreads, G::kSmemTotal, stream>>>(
+      ma_hi, ma_lo, mb_hi, mb_lo, p, g_gram_lbo, g_gram_sbo);
+  return check_cuda(cudaGetLastError(), "gram_tc launch");
+}
+
 int gram_tc_launch(const GramTcParams& p, const void* a_hi, const void* a_lo, const void* b_hi,
                    const void* b_lo, cudaStream_t stream) {
-  if (p.Cm % TM != 0 || p.Cn % TN != 0 || p.rows <= 0 || p.splits < 1 || p.ntaps < 1 || p.ntaps > 9) {
+  if (p.Cm % 64 != 0 || p.Cn % 64 != 0 || p.Cm < 64 || p.Cn < 64 || p.rows <= 0 || p.splits < 1 ||
+      p.ntaps < 1 || p.ntaps > 9) {
     set_last_error("gram_tc: unsupported shape Cm=%d Cn=%d rows=%d splits=%d", p.Cm, p.Cn, p.rows,
                    p.splits);
     return RW_ERR_BAD_ARG;
@@ -258,21 +296,11 @@ int gram_tc_launch(const GramTcParams& p, const void* a_hi, const void* a_lo, co
   if ((rc = make_tmap_2d_bf16(&ma_lo, a_lo, a_cols, a_extent, (uint64_t)a_cols * 2, 64, RB))) return rc;
   if ((rc = make_tmap_2d_bf16(&mb_hi, b_hi, p.Cn, b_extent, (uint64_t)p.Cn * 2, 64, RB))) return rc;
   if ((rc = make_tmap_2d_bf16(&mb_lo, b_lo, p.Cn, b_extent, (uint64_t)p.Cn * 2, 64, RB))) return rc;
-
-  static bool attr_set = false;
-  if (!attr_set) {
-    rc = check_cuda(cudaFuncSetAttribute(gram_tc_kernel,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemTotal),
-                    "gram_tc smem attr");
-    if (rc) return rc;
-    attr_set = true;
-  }
-  const int mt = p.Cm / TM, nt = p.Cn / TN;
-  const int tiles = p.upper_only ? mt * (mt + 1) / 2 : mt * nt;
-  dim3 grid(tiles, p.splits, p.ntaps);
-  gram_tc_kernel<<<grid, kNumThreads, kSmemTotal, stream>>>(ma_hi, ma_lo, mb_hi, mb_lo, p,
-                                                            g_gram_lbo, g_gram_sbo);
-  return check_cuda(cudaGetLastError(), "gram_tc launch");
+  const bool m128 = gram_tile_width(p.Cm) == 128, n128 = gram_tile_width(p.Cn) == 128;
+  if (m128 && n128) return gram_tc_launch_tile<128, 128>(p, ma_hi, ma_lo, mb_hi, mb_lo, stream);
+  if (m128) return gram_tc_launch_tile<128, 64>(p, ma_hi, ma_lo, mb_hi, mb_lo, stream);
+  if (n128) return gram_tc_launch_tile<64, 128>(p, ma_hi, ma_lo, mb_hi, mb_lo, stream);
+  return gram_tc_launch_tile<64, 64>(p, ma_hi, ma_lo, mb_hi, mb_lo, stream);
 }
 
 int reduce_partials_launch(const float* partial, int splits, int M, int N, long long ldp,

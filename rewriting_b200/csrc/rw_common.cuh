@@ -201,6 +201,29 @@ __device__ __forceinline__ void wgmma_m64n128(float (&d)[64], uint64_t desc_a, u
       : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(TA), "n"(TB));
 }
 template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n64(float (&d)[32], uint64_t desc_a, uint64_t desc_b,
+                                              uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1, %35, %36;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(TA), "n"(TB));
+}
+// M = 64, N = 128 or 64 by the accumulator array's length (BN / 2 registers per thread)
+template <int TA, int TB, int NR>
+__device__ __forceinline__ void wgmma_m64nN(float (&d)[NR], uint64_t desc_a, uint64_t desc_b,
+                                             uint32_t accumulate) {
+  static_assert(NR == 64 || NR == 32, "wgmma_m64nN: N = 128 or 64");
+  if constexpr (NR == 64) wgmma_m64n128<TA, TB>(d, desc_a, desc_b, accumulate);
+  else wgmma_m64n64<TA, TB>(d, desc_a, desc_b, accumulate);
+}
+template <int TA, int TB>
 __device__ __forceinline__ void wgmma_m64n144(float (&d)[72], uint64_t desc_a, uint64_t desc_b,
                                                uint32_t accumulate) {
   asm volatile(

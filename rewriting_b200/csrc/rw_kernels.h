@@ -109,6 +109,11 @@ struct GramTcParams {
 
 int gram_tc_launch(const GramTcParams& p, const void* a_hi, const void* a_lo, const void* b_hi,
                    const void* b_lo, cudaStream_t stream);
+// the col-GEMM's tile extent along a channel dimension of C (C % 64 == 0): 128 where it divides C
+inline int gram_tile_width(int C) { return C % 128 == 0 ? 128 : 64; }
+inline int gram_tiles(int Cm, int Cn) {
+  return (Cm / gram_tile_width(Cm)) * (Cn / gram_tile_width(Cn));
+}
 
 // out[m*ldo+n] (= or +=) sum_s partial[s][m][n]; optional symmetric mirror of the
 // upper triangle into the lower one.

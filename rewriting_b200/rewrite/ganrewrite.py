@@ -294,7 +294,7 @@ class ProgressiveGanRewriter(object):
         cached), so no cuBLAS call sits between key capture and the direction d."""
         zca = self.zca_matrix
         if k.dim() == 2 and k.is_cuda and zca.is_cuda and k.dtype == torch.float32 and \
-                zca.shape[0] % 128 == 0 and zca.shape[1] % 64 == 0 and k.shape[0] > 0:
+                zca.shape[0] % 64 == 0 and zca.shape[1] % 64 == 0 and k.shape[0] > 0:
             ent = self.__dict__.get('_zca_planes')
             tag = (zca.data_ptr(), zca._version)
             if ent is None or ent[0] != tag:

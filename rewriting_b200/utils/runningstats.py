@@ -53,9 +53,9 @@ class RunningSecondMoment(object):
         if not a.is_cuda:
             raise RuntimeError('RunningSecondMoment.add needs CUDA data (no CPU fallback); got '
                                + str(a.device))
-        if a.shape[1] % 128 != 0:
+        if a.shape[1] % 64 != 0:
             raise RuntimeError('RunningSecondMoment.add: channel count %d is not a multiple of '
-                               '128 (tensor-core tile)' % a.shape[1])
+                               '64 (tensor-core tile)' % a.shape[1])
         ops.second_moment_accum(self.mom2, a.detach())
 
     def add_planes(self, hi, lo, count):
