@@ -80,6 +80,12 @@ int rw_demod(const float* style, const float* wsq, int B, int Cout, int Cin, flo
              float* demod, rw_stream_t stream);
 
 /* ---- fused modulated 3x3 convolution (wgmma) ---- */
+/* Alignment, for every entry point on the tensor-core row-GEMM (rw_modconv_fwd, _up_fwd,
+ * _fwd_fused, _up_fwd_cl, _up_dgrad, rw_rowgemm, rw_conv3x3_bias_act): fp32 pointers are 4-byte
+ * aligned; next_scale, and the channels-last t_cl and its scale_bo (rw_modconv_up_fwd_cl), are
+ * 8-byte aligned; next_hi / next_lo are 4-byte aligned.  Otherwise the call returns
+ * RW_STATUS_BAD_ARG before anything is launched, with the reason in rw_last_error().  A scale_bo
+ * that is only 4-byte aligned is accepted elsewhere, on the slower full epilogue. */
 /* out[b,o,y,x] = act( conv3x3(k, scale*W)[b,o,y,x] * scale_bo[b,o] + noise_w[0]*noise[b,y*W+x] + bias[o] )
  * scale_bo / noise / bias may be NULL; noise_w is a DEVICE scalar (the nn.Parameter's storage,
  * so no host sync per layer); act: 0 none, 1 leaky_relu(0.2)*sqrt(2). */

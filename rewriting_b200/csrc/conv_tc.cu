@@ -496,6 +496,30 @@ int conv_tc_launch(const ConvTcParams& p, const void* a_hi, const void* a_lo, co
       set_last_error("conv_tc: phase %d has %d taps", i, p.ph_ntaps[i]);
       return RW_ERR_BAD_ARG;
     }
+  // the epilogue's accesses, at offsets that keep each base pointer's alignment (Cout % 64 == 0,
+  // even column): float2 loads of next_scale, and of scale_bo on the pad rows of a channels-last
+  // store; float2 stores of channels-last out; bf16 pairs stored as uint32 into next_hi / next_lo
+  const struct {
+    const void* ptr;
+    unsigned align;
+    const char* name;
+  } need[] = {
+      {p.scale_bo, p.out_mode == 1 ? 8u : 4u, "scale_bo"},
+      {p.out, p.out_mode == 1 ? 8u : 4u, "out"},
+      {p.noise, 4u, "noise"},
+      {p.noise_w, 4u, "noise_w"},
+      {p.bias, 4u, "bias"},
+      {p.next_scale, 8u, "next_scale"},
+      {p.next_hi, 4u, "next_hi"},
+      {p.next_lo, 4u, "next_lo"},
+      {p.rgb_w, 4u, "rgb_w"},
+      {p.rgb_part, 4u, "rgb_part"},
+  };
+  for (const auto& n : need)
+    if (n.ptr != nullptr && (reinterpret_cast<uintptr_t>(n.ptr) & (n.align - 1)) != 0) {
+      set_last_error("conv_tc: %s (%p) is not %u-byte aligned", n.name, n.ptr, n.align);
+      return RW_ERR_BAD_ARG;
+    }
   // 128-channel tiles wherever Cout allows them; 64 only for the 64-channel layers
   if (p.Cout % 128 == 0) return conv_tc_launch_bn<128>(p, a_hi, a_lo, w_hi, w_lo, wk_total, stream);
   return conv_tc_launch_bn<64>(p, a_hi, a_lo, w_hi, w_lo, wk_total, stream);
