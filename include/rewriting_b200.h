@@ -347,6 +347,15 @@ int rw_rowgemm(const void* a_hi, const void* a_lo, const void* w_hi, const void*
 int rw_pixel_norm_nchw(const float* x, int B, int C, int H, int W, int up2, float* out,
                        rw_stream_t stream);
 int rw_nearest_up2(const float* x, long long planes, int H, int W, float* out, rw_stream_t stream);
+/* Backwards of the two leaves (gradients of a training loss through PixelNormLayer and
+ * DoubleResolutionLayer).  rw_pixel_norm_nchw_bwd: gx [B,C,H,W] from the forward's input x
+ * [B,C,H,W] and gy ([B,C,2H,2W] when up2 = 1, 8-byte aligned); rw_nearest_up2_bwd: gx
+ * [planes,H,W] = 2 x 2 sums of gy [planes,2H,2W] (8-byte aligned).  Null pointers and sizes < 1
+ * return RW_STATUS_BAD_ARG before any launch; neither call allocates or synchronises. */
+int rw_pixel_norm_nchw_bwd(const float* x, const float* gy, int B, int C, int H, int W, int up2,
+                           float* gx, rw_stream_t stream);
+int rw_nearest_up2_bwd(const float* gy, long long planes, int H, int W, float* gx,
+                       rw_stream_t stream);
 int rw_conv3x3_bias_act(const void* kp_hi, const void* kp_lo, const void* wt_hi, const void* wt_lo,
                         const float* bias, int act, float act_gain, int B, int Cin, int Cout, int H,
                         int W, float* out, rw_stream_t stream);

@@ -73,6 +73,8 @@ SIGNATURES = {
     'rw_rowgemm': (c_int, [c_p, c_p, c_p, c_p, c_int, c_int, c_int, c_p, c_p]),
     'rw_pixel_norm_nchw': (c_int, [c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p]),
     'rw_nearest_up2': (c_int, [c_p, c_ll, c_int, c_int, c_p, c_p]),
+    'rw_pixel_norm_nchw_bwd': (c_int, [c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p]),
+    'rw_nearest_up2_bwd': (c_int, [c_p, c_ll, c_int, c_int, c_p, c_p]),
     'rw_conv3x3_bias_act': (c_int, [c_p, c_p, c_p, c_p, c_p, c_int, c_f, c_int, c_int, c_int, c_int,
                                     c_int, c_p, c_p]),
     'rw_debug_upconv_profile': (c_int, [c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_ll, c_p, c_p, c_p, c_p,

@@ -389,6 +389,24 @@ int rw_nearest_up2(const float* x, long long planes, int H, int W, float* out, r
   return nearest_up2_launch(x, planes, H, W, out, stream);
 }
 
+int rw_pixel_norm_nchw_bwd(const float* x, const float* gy, int B, int C, int H, int W, int up2,
+                           float* gx, rw_stream_t stream) {
+  if (!x || !gy || !gx) {
+    set_last_error("rw_pixel_norm_nchw_bwd: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  return pixel_norm_nchw_bwd_launch(x, gy, B, C, H, W, up2, gx, stream);
+}
+
+int rw_nearest_up2_bwd(const float* gy, long long planes, int H, int W, float* gx,
+                       rw_stream_t stream) {
+  if (!gy || !gx) {
+    set_last_error("rw_nearest_up2_bwd: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  return nearest_up2_bwd_launch(gy, planes, H, W, gx, stream);
+}
+
 static int modconv_fused_impl(const void* kp_hi, const void* kp_lo, const void* wt_hi,
                               const void* wt_lo, const float* scale_bo, const float* noise,
                               long long noise_bstride, const float* noise_w, const float* bias,

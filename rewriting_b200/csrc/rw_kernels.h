@@ -151,6 +151,10 @@ int pixel_norm_nchw_launch(const float* x, int B, int C, int H, int W, int up2, 
                            cudaStream_t stream);
 int nearest_up2_launch(const float* x, long long planes, int H, int W, float* out,
                        cudaStream_t stream);
+int pixel_norm_nchw_bwd_launch(const float* x, const float* gy, int B, int C, int H, int W, int up2,
+                               float* gx, cudaStream_t stream);
+int nearest_up2_bwd_launch(const float* gy, long long planes, int H, int W, float* gx,
+                           cudaStream_t stream);
 int demod_multi_launch(int B, float eps, int n, const float* const* style,
                        const float* const* wsq, float* const* out, const int* cout,
                        const int* cin, const int* kind, const float* wscale,

@@ -1166,6 +1166,63 @@ nearest_up2_kernel(const float* __restrict__ x, long long n_in, int H, int W,
   *reinterpret_cast<float2*>(d + 2 * W) = make_float2(v, v);
 }
 
+// The 2 x 2 sum of a [2H, 2W] gradient plane at input pixel (y, x): the adjoint of the nearest 2x.
+// `g` points at the plane; the two float2 loads need it 8-byte aligned (2W is even).
+__device__ __forceinline__ float sum_2x2(const float* __restrict__ g, int y, int xx, int W) {
+  const float* r = g + (2LL * y) * (2 * W) + 2 * xx;
+  const float2 a = __ldg(reinterpret_cast<const float2*>(r));
+  const float2 b = __ldg(reinterpret_cast<const float2*>(r + 2 * W));
+  return (a.x + a.y) + (b.x + b.y);
+}
+
+// Backward of pixel_norm_nchw_kernel (and of its fused 2x when up2).  With s = mean_c x^2 + 1e-8
+// and g the incoming gradient (its 2 x 2 sum when up2):
+//   gx[c] = (g[c] - x[c] * (sum_j g[j] x[j]) / (C s)) / sqrt(s)
+// One thread per input pixel, coalesced along x like the forward: pass 1 accumulates sum x^2 and
+// sum g x over the C channels, pass 2 re-reads x and gy and writes gx.
+__global__ void __launch_bounds__(256)
+pixel_norm_nchw_bwd_kernel(const float* __restrict__ x, const float* __restrict__ gy, int B, int C,
+                           int H, int W, int up2, float* __restrict__ gx) {
+  const long long hw = static_cast<long long>(H) * W;
+  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (idx >= static_cast<long long>(B) * hw) return;
+  const int b = static_cast<int>(idx / hw);
+  const long long pix = idx - static_cast<long long>(b) * hw;
+  const int y = static_cast<int>(pix / W), xx = static_cast<int>(pix - static_cast<long long>(y) * W);
+  const long long ghw = up2 ? 4 * hw : hw;
+  const float* xs = x + static_cast<long long>(b) * C * hw + pix;
+  const float* gp = gy + static_cast<long long>(b) * C * ghw + (up2 ? 0 : pix);
+  float ss = 0.f, dot = 0.f;
+  for (int c = 0; c < C; ++c) {
+    const float v = __ldg(xs + c * hw);
+    const float g = up2 ? sum_2x2(gp + c * ghw, y, xx, W) : __ldg(gp + c * ghw);
+    ss = fmaf(v, v, ss);
+    dot = fmaf(g, v, dot);
+  }
+  const float s = ss / static_cast<float>(C) + 1e-8f;
+  const float den = sqrtf(s);
+  const float coef = dot / (static_cast<float>(C) * s);
+  float* dst = gx + static_cast<long long>(b) * C * hw + pix;
+  for (int c = 0; c < C; ++c) {
+    const float v = __ldg(xs + c * hw);
+    const float g = up2 ? sum_2x2(gp + c * ghw, y, xx, W) : __ldg(gp + c * ghw);
+    dst[c * hw] = fmaf(-v, coef, g) / den;
+  }
+}
+
+// Backward of nearest_up2_kernel: gx[plane, y, x] = 2 x 2 sum of gy, one thread per input element
+__global__ void __launch_bounds__(256)
+nearest_up2_bwd_kernel(const float* __restrict__ gy, long long n_in, int H, int W,
+                       float* __restrict__ gx) {
+  const long long idx = static_cast<long long>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (idx >= n_in) return;
+  const long long hw = static_cast<long long>(H) * W;
+  const long long pl = idx / hw;
+  const long long pix = idx - pl * hw;
+  const int y = static_cast<int>(pix / W), xx = static_cast<int>(pix - static_cast<long long>(y) * W);
+  gx[idx] = sum_2x2(gy + pl * 4 * hw, y, xx, W);
+}
+
 inline int grid_for(long long n, int threads, int cap = 132 * 16) {
   long long g = (n + threads - 1) / threads;
   if (g > cap) g = cap;
@@ -1407,6 +1464,30 @@ int nearest_up2_launch(const float* x, long long planes, int H, int W, float* ou
   const long long blocks = (n + 255) / 256;
   nearest_up2_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(x, n, H, W, out);
   return check_cuda(cudaGetLastError(), "nearest_up2 launch");
+}
+
+int pixel_norm_nchw_bwd_launch(const float* x, const float* gy, int B, int C, int H, int W, int up2,
+                               float* gx, cudaStream_t stream) {
+  if (B < 1 || C < 1 || H < 1 || W < 1 || (up2 && (reinterpret_cast<uintptr_t>(gy) & 7u))) {
+    set_last_error("pixel_norm_nchw_bwd: bad shape / alignment");
+    return RW_ERR_BAD_ARG;
+  }
+  const long long blocks = (static_cast<long long>(B) * H * W + 255) / 256;
+  pixel_norm_nchw_bwd_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(x, gy, B, C, H, W,
+                                                                               up2 ? 1 : 0, gx);
+  return check_cuda(cudaGetLastError(), "pixel_norm_nchw_bwd launch");
+}
+
+int nearest_up2_bwd_launch(const float* gy, long long planes, int H, int W, float* gx,
+                           cudaStream_t stream) {
+  if (planes < 1 || H < 1 || W < 1 || (reinterpret_cast<uintptr_t>(gy) & 7u)) {
+    set_last_error("nearest_up2_bwd: bad shape / alignment");
+    return RW_ERR_BAD_ARG;
+  }
+  const long long n = planes * H * W;
+  const long long blocks = (n + 255) / 256;
+  nearest_up2_bwd_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(gy, n, H, W, gx);
+  return check_cuda(cudaGetLastError(), "nearest_up2_bwd launch");
 }
 
 int demod_multi_launch(int B, float eps, int n, const float* const* style,

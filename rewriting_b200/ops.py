@@ -15,6 +15,7 @@ import math
 
 import numpy as np
 import torch
+from torch.autograd.function import once_differentiable
 
 from . import _cabi
 
@@ -594,6 +595,45 @@ def nearest_up2(x):
     out = torch.empty((B, C, 2 * H, 2 * W), dtype=torch.float32, device=x.device)
     _cabi.call('rw_nearest_up2', _p(x), B * C, H, W, _p(out), _stream())
     return out
+
+
+class PixelNormFunction(torch.autograd.Function):
+    """pixel_norm_nchw (the same launch) with its gradient on `rw_pixel_norm_nchw_bwd`."""
+
+    @staticmethod
+    def forward(ctx, x, up2):
+        x = _f32c(x)
+        ctx.save_for_backward(x)
+        ctx.up2 = bool(up2)
+        return pixel_norm_nchw(x, up2=up2)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        (x,) = ctx.saved_tensors
+        B, C, H, W = x.shape
+        gx = torch.empty_like(x)
+        _cabi.call('rw_pixel_norm_nchw_bwd', _p(x), _p(_f32c(gy)), B, C, H, W,
+                   1 if ctx.up2 else 0, _p(gx), _stream())
+        return gx, None
+
+
+class NearestUp2Function(torch.autograd.Function):
+    """nearest_up2 (the same launch) with its gradient, the 2x2 sum, on `rw_nearest_up2_bwd`."""
+
+    @staticmethod
+    def forward(ctx, x):
+        x = _f32c(x)
+        ctx.in_shape = x.shape
+        return nearest_up2(x)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        B, C, H, W = ctx.in_shape
+        gx = torch.empty((B, C, H, W), dtype=torch.float32, device=gy.device)
+        _cabi.call('rw_nearest_up2_bwd', _p(_f32c(gy)), B * C, H, W, _p(gx), _stream())
+        return gx
 
 
 def plain_conv_eligible(weight):

@@ -360,7 +360,9 @@ class ProgressiveGanRewriter(object):
         """G(z) without a graph; through the autograd forward kernels when `apply_overfit` asks
         for pixels that are bit-identical to what its optimisation loop will see."""
         if self._render_like_training:
-            with torch.enable_grad():
+            # the same cuDNN setting as the iteration too: a ProgGAN's 4x4 first layer and ToRGB
+            # run on F.conv2d, where TF32 would leave residuals on every unpasted pixel
+            with torch.enable_grad(), torch.backends.cudnn.flags(allow_tf32=False):
                 return self.model(z).detach()
         with torch.no_grad():
             return self.model(z)

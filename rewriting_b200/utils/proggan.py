@@ -4,7 +4,9 @@
 and `nethook.subsequence` address `layerN.conv` exactly as in the reference.
 
 Where the arithmetic runs (CUDA tensors; there is no CPU fallback for the forward):
-  * PixelNormLayer / DoubleResolutionLayer — `rw_pixel_norm_nchw` / `rw_nearest_up2`;
+  * PixelNormLayer / DoubleResolutionLayer — `rw_pixel_norm_nchw` / `rw_nearest_up2`, and under
+    autograd (grad enabled, input requiring grad) the same launches with their backwards
+    `rw_pixel_norm_nchw_bwd` / `rw_nearest_up2_bwd`, so gradients reach every parameter;
   * every 3x3 conv with Cin % 64 == 0 and Cout % 128 == 0 (all 512/256/128-channel layers, in
     particular every layer a rewriter targets) — the wgmma row-GEMM over bf16 hi/lo key planes
     (`ops.plain_conv`, with autograd for the rewriter's fallback path); an intact, unhooked
@@ -52,13 +54,21 @@ def from_old_pt_dict(parameters):
 
 
 # ------------------------------------------------------------------------------------------ modules
+def _needs_grad(x):
+    return torch.is_grad_enabled() and x.requires_grad
+
+
 class PixelNormLayer(nn.Module):
     def forward(self, x):
+        if _needs_grad(x):
+            return ops.PixelNormFunction.apply(x, False)
         return ops.pixel_norm_nchw(x)
 
 
 class DoubleResolutionLayer(nn.Module):
     def forward(self, x):
+        if _needs_grad(x):
+            return ops.NearestUp2Function.apply(x)
         return ops.nearest_up2(x)
 
 
