@@ -360,6 +360,50 @@ int rw_conv3x3_bias_act(const void* kp_hi, const void* kp_lo, const void* wt_hi,
                         const float* bias, int act, float act_gain, int B, int Cin, int Cout, int H,
                         int W, float* out, rw_stream_t stream);
 
+/* ---- ProgGAN layers off the tensor-core path: fp32 on CUDA cores, fp32 NCHW in and out ----
+ * Every call sums in a fixed order (two calls on the same input give the same bits), neither
+ * allocates nor synchronises, and returns RW_STATUS_BAD_ARG before any launch for a null pointer,
+ * a size < 1, a misaligned pointer where one is required or a short workspace.
+ *
+ * rw_proggan_input_fwd: the 4x4 "dense" first layer, Conv2d(Z, C, 4, padding 3) on z [B,Z]
+ *   (the 1x1 input): out[b,o,y,x] = sum_i z[b,i] w[o,i,3-y,3-x], w [C,Z,4,4], out [B,C,4,4].
+ *   bias == NULL: the bare conv (wscale unused); otherwise the block's epilogue
+ *   leaky_relu(out * wscale + bias[o], 0.2).
+ * rw_proggan_input_bwd: gz [B,Z] = W^T gy and gw [C,Z,4,4] = sum over the batch, in order, of
+ *   gy (x) z; either output may be NULL.  w, gy and gw must be 16-byte aligned.
+ * rw_narrow_conv3x3: 3x3 conv (pad 1, no bias) for any Cin, Cout >= 1 (tuned for <= 64
+ *   channels), x [B,Cin,H,W], w [Cout,Cin,3,3]; bias / wscale as for the input layer.
+ * rw_narrow_conv3x3_dgrad: gx [B,Cin,H,W] from gy [B,Cout,H,W] (the same kernel, weights read
+ *   transposed and flipped).
+ * rw_narrow_conv3x3_wgrad: gw [Cout,Cin,3,3] from x and gy: partial sums over pixel tiles into
+ *   `workspace` (at least rw_narrow_conv3x3_wgrad_workspace_bytes bytes; 0 means the shape is
+ *   refused), then a fixed-order sum.
+ * rw_torgb1x1 / _dgrad / _wgrad: the 1x1 conv of the ToRGB block, Cin -> Cout (1 <= Cout <= 4),
+ *   w [Cout,Cin,1,1]; the wgrad as above with its own workspace query.
+ * rw_proggan_output_block: OutputConvBlock in one kernel: pixel norm -> 1x1 conv -> * wscale +
+ *   bias -> Hardtanh (clamp != 0) or identity; the same bits as the four leaves. */
+int rw_proggan_input_fwd(const float* z, const float* w, const float* bias, float wscale, int B,
+                         int Z, int C, float* out, rw_stream_t stream);
+int rw_proggan_input_bwd(const float* z, const float* w, const float* gy, int B, int Z, int C,
+                         float* gz, float* gw, rw_stream_t stream);
+int rw_narrow_conv3x3(const float* x, const float* w, const float* bias, float wscale, int B,
+                      int Cin, int Cout, int H, int W, float* out, rw_stream_t stream);
+int rw_narrow_conv3x3_dgrad(const float* gy, const float* w, int B, int Cin, int Cout, int H, int W,
+                            float* gx, rw_stream_t stream);
+size_t rw_narrow_conv3x3_wgrad_workspace_bytes(int B, int Cin, int Cout, int H, int W);
+int rw_narrow_conv3x3_wgrad(const float* x, const float* gy, int B, int Cin, int Cout, int H, int W,
+                            float* gw, void* workspace, size_t workspace_bytes, rw_stream_t stream);
+int rw_torgb1x1(const float* x, const float* w, int B, int Cin, int Cout, int H, int W, float* out,
+                rw_stream_t stream);
+int rw_torgb1x1_dgrad(const float* gy, const float* w, int B, int Cin, int Cout, int H, int W,
+                      float* gx, rw_stream_t stream);
+size_t rw_torgb1x1_wgrad_workspace_bytes(int B, int Cin, int Cout, int H, int W);
+int rw_torgb1x1_wgrad(const float* x, const float* gy, int B, int Cin, int Cout, int H, int W,
+                      float* gw, void* workspace, size_t workspace_bytes, rw_stream_t stream);
+int rw_proggan_output_block(const float* x, const float* w, const float* bias, float wscale,
+                            int clamp, int B, int Cin, int Cout, int H, int W, float* out,
+                            rw_stream_t stream);
+
 /* ---- bring-up hooks (tests/tools only) ---- */
 /* rw_modconv_up_fused with demod = next_scale = ones_bo, additionally dumping the raw tap products
  * P[b][y][x][tap][Cout] of the tensor-core stage */

@@ -77,6 +77,19 @@ SIGNATURES = {
     'rw_nearest_up2_bwd': (c_int, [c_p, c_ll, c_int, c_int, c_p, c_p]),
     'rw_conv3x3_bias_act': (c_int, [c_p, c_p, c_p, c_p, c_p, c_int, c_f, c_int, c_int, c_int, c_int,
                                     c_int, c_p, c_p]),
+    'rw_proggan_input_fwd': (c_int, [c_p, c_p, c_p, c_f, c_int, c_int, c_int, c_p, c_p]),
+    'rw_proggan_input_bwd': (c_int, [c_p, c_p, c_p, c_int, c_int, c_int, c_p, c_p, c_p]),
+    'rw_narrow_conv3x3': (c_int, [c_p, c_p, c_p, c_f, c_int, c_int, c_int, c_int, c_int, c_p, c_p]),
+    'rw_narrow_conv3x3_dgrad': (c_int, [c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p]),
+    'rw_narrow_conv3x3_wgrad_workspace_bytes': (c_sz, [c_int, c_int, c_int, c_int, c_int]),
+    'rw_narrow_conv3x3_wgrad': (c_int, [c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p, c_sz,
+                                        c_p]),
+    'rw_torgb1x1': (c_int, [c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p]),
+    'rw_torgb1x1_dgrad': (c_int, [c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p]),
+    'rw_torgb1x1_wgrad_workspace_bytes': (c_sz, [c_int, c_int, c_int, c_int, c_int]),
+    'rw_torgb1x1_wgrad': (c_int, [c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p, c_sz, c_p]),
+    'rw_proggan_output_block': (c_int, [c_p, c_p, c_p, c_f, c_int, c_int, c_int, c_int, c_int, c_int,
+                                        c_p, c_p]),
     'rw_debug_upconv_profile': (c_int, [c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_ll, c_p, c_p, c_p, c_p,
                                         c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p]),
     'rw_debug_conv_profile': (c_int, [c_p, c_p, c_p, c_p, c_p, c_p, c_ll, c_p, c_p, c_int,
@@ -165,7 +178,7 @@ def check(rc, what):
 # kernels launched per entry point (for bench.py's `gpu_launches` claim)
 LAUNCHES_PER_CALL = {
     'rw_second_moment_accum': 2, 'rw_conv_wgrad': 2, 'rw_conv_up_wgrad': 2,
-    'rw_debug_colgemm': 2,
+    'rw_debug_colgemm': 2, 'rw_narrow_conv3x3_wgrad': 2, 'rw_torgb1x1_wgrad': 2,
 }
 launch_count = 0
 

@@ -407,6 +407,98 @@ int rw_nearest_up2_bwd(const float* gy, long long planes, int H, int W, float* g
   return nearest_up2_bwd_launch(gy, planes, H, W, gx, stream);
 }
 
+int rw_proggan_input_fwd(const float* z, const float* w, const float* bias, float wscale, int B,
+                         int Z, int C, float* out, rw_stream_t stream) {
+  if (!z || !w || !out) {
+    set_last_error("rw_proggan_input_fwd: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  return proggan_input_fwd_launch(z, w, bias, wscale, B, Z, C, out, stream);
+}
+
+int rw_proggan_input_bwd(const float* z, const float* w, const float* gy, int B, int Z, int C,
+                         float* gz, float* gw, rw_stream_t stream) {
+  if (!gy || (!gz && !gw) || (gz && !w) || (gw && !z)) {
+    set_last_error("rw_proggan_input_bwd: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  return proggan_input_bwd_launch(z, w, gy, B, Z, C, gz, gw, stream);
+}
+
+int rw_narrow_conv3x3(const float* x, const float* w, const float* bias, float wscale, int B,
+                      int Cin, int Cout, int H, int W, float* out, rw_stream_t stream) {
+  if (!x || !w || !out) {
+    set_last_error("rw_narrow_conv3x3: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  return narrow_conv3x3_launch(x, w, bias, wscale, B, Cin, Cout, H, W, 0, out, stream);
+}
+
+int rw_narrow_conv3x3_dgrad(const float* gy, const float* w, int B, int Cin, int Cout, int H, int W,
+                            float* gx, rw_stream_t stream) {
+  if (!gy || !w || !gx) {
+    set_last_error("rw_narrow_conv3x3_dgrad: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  // conv(gy, W') over Cout input channels to Cin output channels
+  return narrow_conv3x3_launch(gy, w, nullptr, 1.f, B, Cout, Cin, H, W, 1, gx, stream);
+}
+
+size_t rw_narrow_conv3x3_wgrad_workspace_bytes(int B, int Cin, int Cout, int H, int W) {
+  return narrow_conv3x3_wgrad_workspace_bytes(B, Cin, Cout, H, W);
+}
+
+int rw_narrow_conv3x3_wgrad(const float* x, const float* gy, int B, int Cin, int Cout, int H, int W,
+                            float* gw, void* workspace, size_t workspace_bytes, rw_stream_t stream) {
+  if (!x || !gy || !gw || !workspace) {
+    set_last_error("rw_narrow_conv3x3_wgrad: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  return narrow_conv3x3_wgrad_launch(x, gy, B, Cin, Cout, H, W, gw, workspace, workspace_bytes,
+                                     stream);
+}
+
+int rw_torgb1x1(const float* x, const float* w, int B, int Cin, int Cout, int H, int W, float* out,
+                rw_stream_t stream) {
+  if (!x || !w || !out) {
+    set_last_error("rw_torgb1x1: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  return torgb1x1_launch(x, w, nullptr, 1.f, 0, 0, B, Cin, Cout, H, W, out, stream);
+}
+
+int rw_torgb1x1_dgrad(const float* gy, const float* w, int B, int Cin, int Cout, int H, int W,
+                      float* gx, rw_stream_t stream) {
+  if (!gy || !w || !gx) {
+    set_last_error("rw_torgb1x1_dgrad: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  return torgb1x1_dgrad_launch(gy, w, B, Cin, Cout, H, W, gx, stream);
+}
+
+size_t rw_torgb1x1_wgrad_workspace_bytes(int B, int Cin, int Cout, int H, int W) {
+  return torgb1x1_wgrad_workspace_bytes(B, Cin, Cout, H, W);
+}
+
+int rw_torgb1x1_wgrad(const float* x, const float* gy, int B, int Cin, int Cout, int H, int W,
+                      float* gw, void* workspace, size_t workspace_bytes, rw_stream_t stream) {
+  if (!x || !gy || !gw || !workspace) {
+    set_last_error("rw_torgb1x1_wgrad: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  return torgb1x1_wgrad_launch(x, gy, B, Cin, Cout, H, W, gw, workspace, workspace_bytes, stream);
+}
+
+int rw_proggan_output_block(const float* x, const float* w, const float* bias, float wscale,
+                            int clamp, int B, int Cin, int Cout, int H, int W, float* out,
+                            rw_stream_t stream) {
+  if (!x || !w || !bias || !out) {
+    set_last_error("rw_proggan_output_block: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  return torgb1x1_launch(x, w, bias, wscale, clamp ? 1 : 0, 1, B, Cin, Cout, H, W, out, stream);
+}
+
 static int modconv_fused_impl(const void* kp_hi, const void* kp_lo, const void* wt_hi,
                               const void* wt_lo, const float* scale_bo, const float* noise,
                               long long noise_bstride, const float* noise_w, const float* bias,

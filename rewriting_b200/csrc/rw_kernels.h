@@ -240,4 +240,27 @@ int insert_up_launch(const InsertLoopParams& p, const float* blur, void* workspa
 int linear_insert_up_launch(const InsertLoopParams& p, const float* blur, void* workspace,
                             size_t workspace_bytes, cudaStream_t stream);
 
+// ---------------------------------------------------------------------------
+// ProgGAN layers off the tensor-core path (proggan.cu): fp32 CUDA-core kernels
+// ---------------------------------------------------------------------------
+int proggan_input_fwd_launch(const float* z, const float* w, const float* bias, float wscale, int B,
+                             int Z, int C, float* out, cudaStream_t stream);
+int proggan_input_bwd_launch(const float* z, const float* w, const float* gy, int B, int Z, int C,
+                             float* gz, float* gw, cudaStream_t stream);
+// flip = 1: the dgrad (conv with W[i][o][8 - tap]; Cin / Cout are the dgrad's)
+int narrow_conv3x3_launch(const float* x, const float* w, const float* bias, float wscale, int B,
+                          int Cin, int Cout, int H, int W, int flip, float* out, cudaStream_t stream);
+size_t narrow_conv3x3_wgrad_workspace_bytes(int B, int Cin, int Cout, int H, int W);
+int narrow_conv3x3_wgrad_launch(const float* x, const float* gy, int B, int Cin, int Cout, int H,
+                                int W, float* gw, void* workspace, size_t workspace_bytes,
+                                cudaStream_t stream);
+int torgb1x1_launch(const float* x, const float* w, const float* bias, float wscale, int clamp,
+                    int norm, int B, int Cin, int Cout, int H, int W, float* out,
+                    cudaStream_t stream);
+int torgb1x1_dgrad_launch(const float* gy, const float* w, int B, int Cin, int Cout, int H, int W,
+                          float* gx, cudaStream_t stream);
+size_t torgb1x1_wgrad_workspace_bytes(int B, int Cin, int Cout, int H, int W);
+int torgb1x1_wgrad_launch(const float* x, const float* gy, int B, int Cin, int Cout, int H, int W,
+                          float* gw, void* workspace, size_t workspace_bytes, cudaStream_t stream);
+
 }  // namespace rw

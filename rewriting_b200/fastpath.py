@@ -74,7 +74,7 @@ def eligible(model, z):
     from .utils.stylegan2 import models as sg2
     if not isinstance(z, torch.Tensor) or z.dim() != 2 or not z.is_cuda or z.dtype != torch.float32:
         return False
-    if model.bag_input or model.bag_output or model.mconv != 'seq':
+    if getattr(model, 'mconv', None) != 'seq' or model.bag_input or model.bag_output:
         return False
     if torch.is_grad_enabled() and (z.requires_grad or any(p.requires_grad for p in model.parameters())):
         return False

@@ -637,8 +637,10 @@ class NearestUp2Function(torch.autograd.Function):
 
 
 def plain_conv_eligible(weight):
+    """3x3 weights the tensor-core row-GEMM takes: Cin and Cout multiples of 64 (128-column tiles
+    where Cout allows, 64-column tiles otherwise)."""
     return (weight.dim() == 4 and weight.shape[2] == 3 and weight.shape[3] == 3 and
-            weight.shape[0] % 128 == 0 and weight.shape[1] % 64 == 0)
+            weight.shape[0] % 64 == 0 and weight.shape[1] % 64 == 0)
 
 
 def conv3x3_bias_act(x, weight, wscale=1.0, bias=None, act=False, act_gain=1.0):
@@ -691,6 +693,151 @@ class PlainConvFunction(torch.autograd.Function):
 
 def plain_conv(x, weight):
     return PlainConvFunction.apply(x, weight, _WeightHolder(weight))
+
+
+# --------------------------------------------------------------------------- ProgGAN fp32 layers
+# The layers of a ProgGAN the tensor-core row-GEMM does not take, on the fp32 CUDA-core kernels of
+# csrc/proggan.cu: the 4x4 input layer, narrow 3x3 convs and the 1x1 ToRGB.  `wscale` / `bias`
+# select the no-grad fused block epilogue (conv * wscale + bias, then LeakyReLU 0.2 or Hardtanh).
+def input_layer(z, weight, wscale=1.0, bias=None):
+    """Conv2d(Z, C, 4, padding 3) of z [B, Z, 1, 1] (or [B, Z]) -> [B, C, 4, 4]."""
+    z = _f32c(z)
+    w = _f32c(weight.detach())
+    B, Z = z.shape[0], z.shape[1]
+    C = w.shape[0]
+    out = torch.empty((B, C, 4, 4), dtype=torch.float32, device=z.device)
+    _cabi.call('rw_proggan_input_fwd', _p(z), _p(w), _p(_f32c(bias.detach()) if bias is not None
+                                                        else None),
+               float(wscale), B, Z, C, _p(out), _stream())
+    return out
+
+
+def narrow_conv3x3(x, weight, wscale=1.0, bias=None):
+    """3x3 conv (pad 1, no bias) of x [B, Cin, H, W] -> [B, Cout, H, W] for any channel counts."""
+    x = _f32c(x)
+    w = _f32c(weight.detach())
+    B, Cin, H, W = x.shape
+    Cout = w.shape[0]
+    out = torch.empty((B, Cout, H, W), dtype=torch.float32, device=x.device)
+    _cabi.call('rw_narrow_conv3x3', _p(x), _p(w), _p(_f32c(bias.detach()) if bias is not None
+                                                     else None),
+               float(wscale), B, Cin, Cout, H, W, _p(out), _stream())
+    return out
+
+
+def torgb1x1(x, weight):
+    """The ToRGB 1x1 conv of x [B, Cin, H, W] to Cout <= 4 channels."""
+    x = _f32c(x)
+    w = _f32c(weight.detach())
+    B, Cin, H, W = x.shape
+    Cout = w.shape[0]
+    out = torch.empty((B, Cout, H, W), dtype=torch.float32, device=x.device)
+    _cabi.call('rw_torgb1x1', _p(x), _p(w), B, Cin, Cout, H, W, _p(out), _stream())
+    return out
+
+
+def output_block(x, weight, wscale, bias, clamp):
+    """OutputConvBlock in one launch: pixel norm -> 1x1 conv -> * wscale + bias -> Hardtanh
+    (clamp) or identity."""
+    x = _f32c(x)
+    w = _f32c(weight.detach())
+    B, Cin, H, W = x.shape
+    Cout = w.shape[0]
+    out = torch.empty((B, Cout, H, W), dtype=torch.float32, device=x.device)
+    _cabi.call('rw_proggan_output_block', _p(x), _p(w), _p(_f32c(bias.detach())), float(wscale),
+               1 if clamp else 0, B, Cin, Cout, H, W, _p(out), _stream())
+    return out
+
+
+class InputLayerFunction(torch.autograd.Function):
+    """input_layer with its gradients (`rw_proggan_input_bwd`): gz = W^T gy, gW = sum_b gy (x) z."""
+
+    @staticmethod
+    def forward(ctx, x, weight):
+        x = _f32c(x)
+        ctx.save_for_backward(x, weight)
+        return input_layer(x, weight)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        x, weight = ctx.saved_tensors
+        need_x, need_w = ctx.needs_input_grad[:2]
+        B, Z = x.shape[0], x.shape[1]
+        C = weight.shape[0]
+        gx = torch.empty_like(x) if need_x else None
+        gW = torch.empty(weight.shape, dtype=torch.float32, device=x.device) if need_w else None
+        if need_x or need_w:
+            # the kernels read gy and W as float4: copy a view that starts off a 16-byte boundary
+            gy, w = [t if t.data_ptr() % 16 == 0 else t.clone()
+                     for t in (_f32c(gy), _f32c(weight.detach()))]
+            _cabi.call('rw_proggan_input_bwd', _p(x), _p(w), _p(gy), B, Z, C, _p(gx), _p(gW),
+                       _stream())
+        return gx, gW
+
+
+class NarrowConvFunction(torch.autograd.Function):
+    """narrow_conv3x3 with its gradients: the dgrad on the same kernel (weights transposed and
+    flipped), the wgrad as a split reduction over the pixels with a fixed-order final sum."""
+
+    @staticmethod
+    def forward(ctx, x, weight):
+        x = _f32c(x)
+        ctx.save_for_backward(x, weight)
+        return narrow_conv3x3(x, weight)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        x, weight = ctx.saved_tensors
+        need_x, need_w = ctx.needs_input_grad[:2]
+        gy = _f32c(gy)
+        w = _f32c(weight.detach())
+        B, Cin, H, W = x.shape
+        Cout = w.shape[0]
+        gx = gW = None
+        if need_x:
+            gx = torch.empty_like(x)
+            _cabi.call('rw_narrow_conv3x3_dgrad', _p(gy), _p(w), B, Cin, Cout, H, W, _p(gx),
+                       _stream())
+        if need_w:
+            lib = _cabi.load()
+            ws = _workspace(lib.rw_narrow_conv3x3_wgrad_workspace_bytes(B, Cin, Cout, H, W), x.device)
+            gW = torch.empty(weight.shape, dtype=torch.float32, device=x.device)
+            _cabi.call('rw_narrow_conv3x3_wgrad', _p(x), _p(gy), B, Cin, Cout, H, W, _p(gW), _p(ws),
+                       ws.numel() * 4, _stream())
+        return gx, gW
+
+
+class ToRGBFunction(torch.autograd.Function):
+    """torgb1x1 with its gradients (`rw_torgb1x1_dgrad`, `rw_torgb1x1_wgrad`)."""
+
+    @staticmethod
+    def forward(ctx, x, weight):
+        x = _f32c(x)
+        ctx.save_for_backward(x, weight)
+        return torgb1x1(x, weight)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        x, weight = ctx.saved_tensors
+        need_x, need_w = ctx.needs_input_grad[:2]
+        gy = _f32c(gy)
+        w = _f32c(weight.detach())
+        B, Cin, H, W = x.shape
+        Cout = w.shape[0]
+        gx = gW = None
+        if need_x:
+            gx = torch.empty_like(x)
+            _cabi.call('rw_torgb1x1_dgrad', _p(gy), _p(w), B, Cin, Cout, H, W, _p(gx), _stream())
+        if need_w:
+            lib = _cabi.load()
+            ws = _workspace(lib.rw_torgb1x1_wgrad_workspace_bytes(B, Cin, Cout, H, W), x.device)
+            gW = torch.empty(weight.shape, dtype=torch.float32, device=x.device)
+            _cabi.call('rw_torgb1x1_wgrad', _p(x), _p(gy), B, Cin, Cout, H, W, _p(gW), _p(ws),
+                       ws.numel() * 4, _stream())
+        return gx, gW
 
 
 # --------------------------------------------------------------------------- key algebra

@@ -3,19 +3,24 @@
 `layer<i>.wscale.b`, `output_<R>x<R>.*`), so `ProgressiveGanRewriter` (rewrite/ganrewrite.py:25-96)
 and `nethook.subsequence` address `layerN.conv` exactly as in the reference.
 
-Where the arithmetic runs (CUDA tensors; there is no CPU fallback for the forward):
+Where the arithmetic runs (CUDA tensors; every layer of a ProgGAN runs on the package's kernels,
+so the result does not depend on torch's TF32 flags):
   * PixelNormLayer / DoubleResolutionLayer — `rw_pixel_norm_nchw` / `rw_nearest_up2`, and under
     autograd (grad enabled, input requiring grad) the same launches with their backwards
     `rw_pixel_norm_nchw_bwd` / `rw_nearest_up2_bwd`, so gradients reach every parameter;
-  * every 3x3 conv with Cin % 64 == 0 and Cout % 128 == 0 (all 512/256/128-channel layers, in
+  * every 3x3 conv with Cin % 64 == 0 and Cout % 64 == 0 (all 512/256/128/64-channel layers, in
     particular every layer a rewriter targets) — the wgmma row-GEMM over bf16 hi/lo key planes
     (`ops.plain_conv`, with autograd for the rewriter's fallback path); an intact, unhooked
     NormConvBlock runs as pixel-norm(+2x) -> planes -> ONE conv launch whose epilogue applies the
     WScale bias and the leaky-ReLU (the WScale factor is folded into the weight planes);
-  * the 4x4 "dense" first layer (a [Z] -> [C,4,4] GEMM written as a padded conv), the 64/32/16
-    channel tails of the high-resolution generators and the 1x1 ToRGB go through
-    torch.nn.functional.conv2d: they are off the rewrite path (SURVEY.md §8 f-3) and below the
-    128-column tile of the tensor-core kernel.
+  * the other 3x3 convs (the 64 -> 32 -> 16 channel tails of the 256² and 1024² generators) — the
+    fp32 narrow conv (`rw_narrow_conv3x3`, dgrad / wgrad for autograd); fused, its epilogue applies
+    the WScale factor, the bias and the leaky-ReLU;
+  * the 4x4 "dense" first layer (a [Z] -> [C,4,4] GEMM written as a padded conv) — fp32
+    `rw_proggan_input_fwd` / `_bwd`, with the same fused epilogue when the block is intact;
+  * the 1x1 ToRGB — fp32 `rw_torgb1x1` (and its backwards) leaf by leaf; an intact, unhooked
+    OutputConvBlock without grad is one `rw_proggan_output_block` launch with the same bits.
+torch.nn.functional.conv2d is left only for CPU tensors and conv shapes none of these take.
 """
 import itertools
 from collections import OrderedDict
@@ -83,14 +88,39 @@ class WScaleLayer(nn.Module):
         return x * self.scale + self.b.view(1, -1, 1, 1)
 
 
+def _conv_route(conv, in_hw):
+    """Which kernel takes a bias-free, stride-1 RewritableConv2d whose input is `in_hw` pixels:
+    'input' (4x4, padding 3, on 1x1), 'tc' (3x3 on the tensor-core row-GEMM), 'narrow' (any other
+    3x3), 'rgb' (1x1 to at most 4 channels) or None (torch's conv2d)."""
+    if conv.bias is not None or conv.stride != (1, 1) or conv.dilation != (1, 1) or conv.groups != 1:
+        return None
+    if conv.kernel_size == (4, 4) and conv.padding == (3, 3) and tuple(in_hw) == (1, 1):
+        return 'input'
+    if conv.kernel_size == (3, 3) and conv.padding == (1, 1):
+        return 'tc' if ops.plain_conv_eligible(conv.weight) else 'narrow'
+    if conv.kernel_size == (1, 1) and conv.padding == (0, 0) and conv.out_channels <= 4:
+        return 'rgb'
+    return None
+
+
 class RewritableConv2d(nn.Conv2d):
-    """nn.Conv2d (bias-free) whose 3x3 instances run on the tensor-core row-GEMM."""
+    """nn.Conv2d (bias-free) on the package's kernels for CUDA inputs: the 4x4 input layer and
+    the 1x1 ToRGB on fp32 CUDA-core kernels, 3x3 convs on the tensor-core row-GEMM or, when a
+    channel count is not a multiple of 64, on the fp32 narrow conv.  Each route has its
+    gradients."""
 
     def forward(self, x):
-        if x.is_cuda and self.kernel_size == (3, 3) and self.padding == (1, 1) and \
-                self.bias is None and ops.plain_conv_eligible(self.weight):
+        route = _conv_route(self, x.shape[2:]) if x.is_cuda else None
+        if route == 'tc':
             return ops.plain_conv(x, self.weight)
-        return nn.functional.conv2d(x, self.weight, self.bias, self.stride, self.padding)
+        if route == 'narrow':
+            return ops.NarrowConvFunction.apply(x, self.weight)
+        if route == 'input':
+            return ops.InputLayerFunction.apply(x, self.weight)
+        if route == 'rgb':
+            return ops.ToRGBFunction.apply(x, self.weight)
+        return nn.functional.conv2d(x, self.weight, self.bias, self.stride, self.padding,
+                                    self.dilation, self.groups)
 
 
 class _Block(nn.Sequential):
@@ -99,15 +129,20 @@ class _Block(nn.Sequential):
 
     def forward(self, x):
         kids = self._modules
-        conv = kids.get('conv')
-        fused = (tuple(kids) == self._expected and x.is_cuda and not torch.is_grad_enabled() and
-                 not _is_hooked(self) and conv is not None and conv.kernel_size == (3, 3) and
-                 ops.plain_conv_eligible(conv.weight) and kids['relu'].negative_slope == 0.2)
-        if not fused:
+        route = None
+        if (tuple(kids) == self._expected and x.is_cuda and not torch.is_grad_enabled() and
+                not _is_hooked(self) and kids['relu'].negative_slope == 0.2):
+            up = 2 if 'up' in kids else 1
+            route = _conv_route(kids['conv'], (up * x.shape[2], up * x.shape[3]))
+        if route is None or route == 'rgb':
             return nn.Sequential.forward(self, x)
+        w, wscale, b = kids['conv'].weight, float(kids['wscale'].scale), kids['wscale'].b
         y = ops.pixel_norm_nchw(x, up2='up' in kids)
-        return ops.conv3x3_bias_act(y, conv.weight, wscale=float(kids['wscale'].scale),
-                                    bias=kids['wscale'].b, act=True, act_gain=1.0)
+        if route == 'tc':
+            return ops.conv3x3_bias_act(y, w, wscale=wscale, bias=b, act=True, act_gain=1.0)
+        if route == 'narrow':
+            return ops.narrow_conv3x3(y, w, wscale=wscale, bias=b)
+        return ops.input_layer(y, w, wscale=wscale, bias=b)
 
 
 class NormConvBlock(_Block):
@@ -142,6 +177,20 @@ class OutputConvBlock(nn.Sequential):
             ('conv', RewritableConv2d(in_channels, 3, kernel_size=1, padding=0, bias=False)),
             ('wscale', WScaleLayer(3, in_channels, gain=1)),
             ('clamp', nn.Hardtanh() if tanh else nn.Identity())]))
+
+    def forward(self, x):
+        """One kernel (pixel norm, 1x1 conv, WScale, clamp) when intact, unhooked, on CUDA and
+        without grad; child by child otherwise.  Both give the same bits."""
+        kids = self._modules
+        clamp = kids.get('clamp')
+        tanh = isinstance(clamp, nn.Hardtanh) and clamp.min_val == -1.0 and clamp.max_val == 1.0
+        if (tuple(kids) == ('norm', 'conv', 'wscale', 'clamp') and x.is_cuda and
+                not torch.is_grad_enabled() and not _is_hooked(self) and
+                (tanh or type(clamp) is nn.Identity) and
+                _conv_route(kids['conv'], x.shape[2:]) == 'rgb'):
+            return ops.output_block(x, kids['conv'].weight, float(kids['wscale'].scale),
+                                    kids['wscale'].b, clamp=tanh)
+        return nn.Sequential.forward(self, x)
 
 
 class ProgressiveGenerator(nn.Sequential):
