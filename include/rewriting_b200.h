@@ -404,6 +404,28 @@ int rw_proggan_output_block(const float* x, const float* w, const float* bias, f
                             int clamp, int B, int Cin, int Cout, int H, int W, float* out,
                             rw_stream_t stream);
 
+/* ---- VGG feature stack: the passes between its convolutions (HBM-bound, fp32 on CUDA cores) ----
+ * rw_relu_pool: one read of a conv output a [B,C,H,W] fp32 NCHW: v = relu(a + bias[c]) (bias may be
+ *   NULL), then, when pool != 0, the 2x2 / stride-2 max pool with floor semantics (an odd last row
+ *   or column is dropped; H, W >= 2), giving [B,C,Ho,Wo].  Writes the next conv's bf16 planes
+ *   out_hi / out_lo [B*(Ho+1)*(Wo+1)][C] (the layout and split of rw_prep_keys with no style:
+ *   hi = bf16_rn(v), lo = bf16_rn(v - hi), zero pad row / column; C % 64 == 0, 16-byte aligned),
+ *   fp32 NCHW out, or both.  relu keeps a NaN; the pool scans its window in row-major order and
+ *   takes a strictly greater value or a NaN (torch's max_pool2d).
+ * rw_relu_pool_bwd: the gradient with respect to a, from the same a / bias / pool and gy
+ *   [B,C,Ho,Wo] fp32 NCHW: every ReLU gate and pool argmax is re-derived with the forward's
+ *   arithmetic; the argmax element gets 0 + gy, every other element and a dropped row / column get
+ *   0, and an element whose relu output is <= 0 gets 0 (torch's threshold_backward).  Writes
+ *   planes g_hi / g_lo [B*(H+1)*(W+1)][C] (for the conv_tc dgrad), fp32 NCHW g [B,C,H,W], or both.
+ * Outputs must not overlap a or gy.  A null input, a size < 1, a pool on H or W < 2, neither or
+ * only one plane, planes with C % 64 != 0 or a plane pointer that is not 16-byte aligned return
+ * RW_STATUS_BAD_ARG before any launch.  Neither call allocates or synchronises; two calls give the
+ * same bits. */
+int rw_relu_pool(const float* a, const float* bias, int B, int C, int H, int W, int pool,
+                 void* out_hi, void* out_lo, float* out, rw_stream_t stream);
+int rw_relu_pool_bwd(const float* a, const float* bias, const float* gy, int B, int C, int H, int W,
+                     int pool, void* g_hi, void* g_lo, float* g, rw_stream_t stream);
+
 /* ---- bring-up hooks (tests/tools only) ---- */
 /* rw_modconv_up_fused with demod = next_scale = ones_bo, additionally dumping the raw tap products
  * P[b][y][x][tap][Cout] of the tensor-core stage */

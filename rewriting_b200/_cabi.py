@@ -90,6 +90,9 @@ SIGNATURES = {
     'rw_torgb1x1_wgrad': (c_int, [c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p, c_sz, c_p]),
     'rw_proggan_output_block': (c_int, [c_p, c_p, c_p, c_f, c_int, c_int, c_int, c_int, c_int, c_int,
                                         c_p, c_p]),
+    'rw_relu_pool': (c_int, [c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p, c_p, c_p]),
+    'rw_relu_pool_bwd': (c_int, [c_p, c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p, c_p,
+                                 c_p]),
     'rw_debug_upconv_profile': (c_int, [c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_ll, c_p, c_p, c_p, c_p,
                                         c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p]),
     'rw_debug_conv_profile': (c_int, [c_p, c_p, c_p, c_p, c_p, c_p, c_ll, c_p, c_p, c_int,

@@ -489,6 +489,24 @@ int rw_torgb1x1_wgrad(const float* x, const float* gy, int B, int Cin, int Cout,
   return torgb1x1_wgrad_launch(x, gy, B, Cin, Cout, H, W, gw, workspace, workspace_bytes, stream);
 }
 
+int rw_relu_pool(const float* a, const float* bias, int B, int C, int H, int W, int pool,
+                 void* out_hi, void* out_lo, float* out, rw_stream_t stream) {
+  if (!a) {
+    set_last_error("rw_relu_pool: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  return relu_pool_launch(a, bias, nullptr, B, C, H, W, pool, out_hi, out_lo, out, stream);
+}
+
+int rw_relu_pool_bwd(const float* a, const float* bias, const float* gy, int B, int C, int H, int W,
+                     int pool, void* g_hi, void* g_lo, float* g, rw_stream_t stream) {
+  if (!a || !gy) {
+    set_last_error("rw_relu_pool_bwd: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  return relu_pool_launch(a, bias, gy, B, C, H, W, pool, g_hi, g_lo, g, stream);
+}
+
 int rw_proggan_output_block(const float* x, const float* w, const float* bias, float wscale,
                             int clamp, int B, int Cin, int Cout, int H, int W, float* out,
                             rw_stream_t stream) {

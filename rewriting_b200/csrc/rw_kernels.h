@@ -263,4 +263,10 @@ size_t torgb1x1_wgrad_workspace_bytes(int B, int Cin, int Cout, int H, int W);
 int torgb1x1_wgrad_launch(const float* x, const float* gy, int B, int Cin, int Cout, int H, int W,
                           float* gw, void* workspace, size_t workspace_bytes, cudaStream_t stream);
 
+// ---------------------------------------------------------------------------
+// VGG feature stack (vgg.cu): bias + ReLU + optional 2x2 max pool, and its backward (gy != null)
+// ---------------------------------------------------------------------------
+int relu_pool_launch(const float* a, const float* bias, const float* gy, int B, int C, int H, int W,
+                     int pool, void* hi, void* lo, float* out, cudaStream_t stream);
+
 }  // namespace rw

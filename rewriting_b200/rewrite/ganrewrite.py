@@ -33,7 +33,7 @@ import time
 
 import torch
 
-from .. import _cabi, ops
+from .. import _cabi, ops, perceptual
 from ..utils import imgviz, nethook, nvtx, pbar, renormalize, tally
 from ..utils.stylegan2 import models as sg2
 
@@ -370,7 +370,12 @@ class ProgressiveGanRewriter(object):
     def perceptual_features(self, feature_net=None):
         """VGG-16 `features` through index 20 (ganrewrite.py:303-304).  `feature_net` (a
         torchvision VGG-16, e.g. rewriting_b200.synthetic.seeded_vgg16() where the ImageNet weights
-        cannot be downloaded) replaces the pretrained network the reference fetches."""
+        cannot be downloaded) replaces the pretrained network the reference fetches.
+
+        A recognised VGG slice (Conv2d 3x3 -> ReLU [-> MaxPool2d(2, 2)] units, as in VGG-16 and
+        VGG-19) comes back as `perceptual.KernelVGGFeatures`, which runs CUDA fp32 inputs on this
+        package's kernels and anything else on the Sequential itself; RW_VGG_KERNELS=0 returns the
+        Sequential."""
         if feature_net is None:
             import torchvision
             try:
@@ -382,7 +387,8 @@ class ProgressiveGanRewriter(object):
         features = getattr(feature_net, 'features', feature_net)
         VF = nethook.subsequence(features, last_layer='20').to(self.device)
         nethook.set_requires_grad(False, VF)
-        return VF
+        kernel_vf = perceptual.kernel_features(VF)
+        return VF if kernel_vf is None else kernel_vf
 
     GRAPH_MIN_ITERS = 16       # whole-iteration CUDA graph for all_weights_insert above this
 
@@ -391,7 +397,9 @@ class ProgressiveGanRewriter(object):
         """Adam over all parameters of the generator on L1 + 1e-2 * MSE of VGG features between the
         target image `x` and G(z), inside `bounds` (ganrewrite.py:300-331).  The generator's
         forward and backward run on this package's kernels (the layer-level autograd ops of
-        BASELINE config 2); the VGG network is torch's own convolution, as in the reference.
+        BASELINE config 2), and so does a recognised VGG network (`perceptual_features`).  On that
+        path the features of the detached target, which are the same every iteration, are computed
+        once before the loop.
 
         At batch 1 an iteration is ~600 kernel launches and launch-bound (19 ms): after three eager
         iterations the WHOLE iteration — forward, backward, Adam step, weight-plane refresh — is
@@ -400,26 +408,36 @@ class ProgressiveGanRewriter(object):
         x, z = [self.detach(d) for d in [x, z]]
         VF = self.perceptual_features(feature_net)
 
+        def crop(d):
+            if bounds is None:
+                return d
+            t, l, b, r = bounds
+            return d[:, :, t:b, l:r]
+        gt_features = None
+        if isinstance(VF, perceptual.KernelVGGFeatures) and VF.kernel_path(crop(x)):
+            with torch.no_grad():
+                gt_features = VF(crop(x))
+
         def compute_loss():
             out = self.model(z)
-            if bounds is None:
-                gt, pred = x, out
-            else:
-                t, l, b, r = bounds
-                gt, pred = [d[:, :, t:b, l:r] for d in [x, out]]
+            gt, pred = crop(x), crop(out)
             return torch.nn.functional.l1_loss(gt, pred) + (
-                1e-2 * torch.nn.functional.mse_loss(VF(gt), VF(pred)))
+                1e-2 * torch.nn.functional.mse_loss(VF(gt) if gt_features is None else gt_features,
+                                                    VF(pred)))
 
         nethook.set_requires_grad(False, self.model)
         params = list(self.model.parameters())
         nethook.set_requires_grad(True, *params)
         if use_graph is None:
             use_graph = x.is_cuda and niter >= self.GRAPH_MIN_ITERS
-        optimizer = torch.optim.Adam(params, lr=lr, capturable=bool(use_graph))
+        # capturable Adam (its step count and bias corrections on the device) for the eager loop
+        # too, on CUDA: an eager run and a graph-replayed run then take the same Adam arithmetic,
+        # so their results do not depend on which side of GRAPH_MIN_ITERS `niter` falls
+        optimizer = torch.optim.Adam(params, lr=lr, capturable=bool(use_graph) or x.is_cuda)
 
         def iteration():
             # fp32 like the reference: cuDNN's TF32 convolutions (torch's default on this hardware)
-            # put ~1 % of error into the VGG term's gradient
+            # put ~1 % of error into the VGG term's gradient wherever the VGG runs on torch
             with torch.enable_grad(), torch.backends.cudnn.flags(allow_tf32=False):
                 loss = compute_loss()
                 optimizer.zero_grad()
