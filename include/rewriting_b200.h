@@ -426,6 +426,42 @@ int rw_relu_pool(const float* a, const float* bias, int B, int C, int H, int W, 
 int rw_relu_pool_bwd(const float* a, const float* bias, const float* gy, int B, int C, int H, int W,
                      int pool, void* g_hi, void* g_lo, float* g, rw_stream_t stream);
 
+/* ---- edit distances: spatial LPIPS v0.1 (VGG-16, "net-lin") and the masked L1 (HBM-bound) ----
+ * rw_lpips_input: im0, im1 as fp32 NCHW [B,3,H,W] in [-1, 1] (u8 == 0) or uint8 NHWC [B,H,W,3]
+ *   (u8 == 1, decoded as (u / 255 - 0.5) / 0.5, each step one IEEE fp32 operation) through the
+ *   scaling layer (x - shift[c]) / scale[c], shift = (-.030, -.088, -.188), scale = (.458, .448,
+ *   .450): out [2B,3,H,W] fp32, images 0..B-1 from im0, B..2B-1 from im1.  The same bits as torch's
+ *   elementwise ops.
+ * rw_lpips_head: one tap.  a [2B,C,h,w] fp32 is the tap conv's output for both halves of the batch
+ *   (bias [C] added here when the conv left it out, else NULL); f = relu(a + bias) and
+ *   d[b,y,x] = sum_c lin_w[c] (f0 / (|f0| + 1e-10) - f1 / (|f1| + 1e-10))^2 over the channel vector
+ *   at (y, x), f0 from image b and f1 from image b + B; d [B,h,w] fp32, formed in float64.
+ * rw_lpips_combine: D[b,0,y,x] = sum over the nmaps (1..8) maps, in order, of maps[l] [B,h_l,w_l]
+ *   bilinearly resized to H x W (torch's align_corners=False with the output size given), in
+ *   float64; map_hw is a host array {h_0, w_0, h_1, w_1, ...} and maps a host array of device
+ *   pointers.  D [B,1,H,W] is written when not NULL.  With num / den (float64 [B]):
+ *   num[b] = sum D * mask, den[b] = sum mask, mask [mask_b,1,H,W] fp32 with mask_b 1 or B, or NULL
+ *   for a mask of ones; partial sums over 1024-pixel tiles go to `workspace` (8-byte aligned, at
+ *   least rw_lpips_combine_workspace_bytes bytes; 0 means the shape is refused) and a fixed-order
+ *   finish adds them per image.
+ * rw_masked_l1: the same reduction of sum_c |im1 - im0| per pixel (images as for rw_lpips_input, in
+ *   [-1, 1] units), channels added in order in fp32; num and den are required.
+ * A null required pointer, a size < 1, B > 65535, an unknown format, a mask batch other than 1 or
+ * B, only one of num / den, or a short workspace return RW_STATUS_BAD_ARG before any launch.  No
+ * call allocates or synchronises, and none uses atomics: two calls give the same bits, and image
+ * b's results do not depend on the other images of the batch. */
+int rw_lpips_input(const void* im0, const void* im1, int u8, int B, int H, int W, float* out,
+                   rw_stream_t stream);
+int rw_lpips_head(const float* a, const float* bias, const float* lin_w, int B, int C, int h, int w,
+                  float* d, rw_stream_t stream);
+size_t rw_lpips_combine_workspace_bytes(int B, int H, int W);
+int rw_lpips_combine(int nmaps, const float* const* maps, const int* map_hw, int B, int H, int W,
+                     const float* mask, int mask_b, float* D, double* num, double* den,
+                     void* workspace, size_t workspace_bytes, rw_stream_t stream);
+int rw_masked_l1(const void* im0, const void* im1, int u8, int B, int H, int W, const float* mask,
+                 int mask_b, double* num, double* den, void* workspace, size_t workspace_bytes,
+                 rw_stream_t stream);
+
 /* ---- bring-up hooks (tests/tools only) ---- */
 /* rw_modconv_up_fused with demod = next_scale = ones_bo, additionally dumping the raw tap products
  * P[b][y][x][tap][Cout] of the tensor-core stage */

@@ -93,6 +93,13 @@ SIGNATURES = {
     'rw_relu_pool': (c_int, [c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p, c_p, c_p]),
     'rw_relu_pool_bwd': (c_int, [c_p, c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p, c_p,
                                  c_p]),
+    'rw_lpips_input': (c_int, [c_p, c_p, c_int, c_int, c_int, c_int, c_p, c_p]),
+    'rw_lpips_head': (c_int, [c_p, c_p, c_p, c_int, c_int, c_int, c_int, c_p, c_p]),
+    'rw_lpips_combine_workspace_bytes': (c_sz, [c_int, c_int, c_int]),
+    'rw_lpips_combine': (c_int, [c_int, c_p, c_p, c_int, c_int, c_int, c_p, c_int, c_p, c_p, c_p,
+                                 c_p, c_sz, c_p]),
+    'rw_masked_l1': (c_int, [c_p, c_p, c_int, c_int, c_int, c_int, c_p, c_int, c_p, c_p, c_p, c_sz,
+                             c_p]),
     'rw_debug_upconv_profile': (c_int, [c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_ll, c_p, c_p, c_p, c_p,
                                         c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p]),
     'rw_debug_conv_profile': (c_int, [c_p, c_p, c_p, c_p, c_p, c_p, c_ll, c_p, c_p, c_int,

@@ -507,6 +507,50 @@ int rw_relu_pool_bwd(const float* a, const float* bias, const float* gy, int B, 
   return relu_pool_launch(a, bias, gy, B, C, H, W, pool, g_hi, g_lo, g, stream);
 }
 
+int rw_lpips_input(const void* im0, const void* im1, int u8, int B, int H, int W, float* out,
+                   rw_stream_t stream) {
+  if (!im0 || !im1 || !out) {
+    set_last_error("rw_lpips_input: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  return lpips_input_launch(im0, im1, u8, B, H, W, out, stream);
+}
+
+int rw_lpips_head(const float* a, const float* bias, const float* lin_w, int B, int C, int h, int w,
+                  float* d, rw_stream_t stream) {
+  if (!a || !lin_w || !d) {
+    set_last_error("rw_lpips_head: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  return lpips_head_launch(a, bias, lin_w, B, C, h, w, d, stream);
+}
+
+size_t rw_lpips_combine_workspace_bytes(int B, int H, int W) {
+  return lpips_combine_workspace_bytes(B, H, W);
+}
+
+int rw_lpips_combine(int nmaps, const float* const* maps, const int* map_hw, int B, int H, int W,
+                     const float* mask, int mask_b, float* D, double* num, double* den,
+                     void* workspace, size_t workspace_bytes, rw_stream_t stream) {
+  if (!maps || !map_hw) {
+    set_last_error("rw_lpips_combine: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  return lpips_combine_launch(nmaps, maps, map_hw, B, H, W, mask, mask_b, D, num, den, workspace,
+                              workspace_bytes, stream);
+}
+
+int rw_masked_l1(const void* im0, const void* im1, int u8, int B, int H, int W, const float* mask,
+                 int mask_b, double* num, double* den, void* workspace, size_t workspace_bytes,
+                 rw_stream_t stream) {
+  if (!im0 || !im1) {
+    set_last_error("rw_masked_l1: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  return masked_l1_launch(im0, im1, u8, B, H, W, mask, mask_b, num, den, workspace, workspace_bytes,
+                          stream);
+}
+
 int rw_proggan_output_block(const float* x, const float* w, const float* bias, float wscale,
                             int clamp, int B, int Cin, int Cout, int H, int W, float* out,
                             rw_stream_t stream) {

@@ -269,4 +269,19 @@ int torgb1x1_wgrad_launch(const float* x, const float* gy, int B, int Cin, int C
 int relu_pool_launch(const float* a, const float* bias, const float* gy, int B, int C, int H, int W,
                      int pool, void* hi, void* lo, float* out, cudaStream_t stream);
 
+// ---------------------------------------------------------------------------
+// LPIPS and masked L1 edit distances (lpips.cu)
+// ---------------------------------------------------------------------------
+int lpips_input_launch(const void* im0, const void* im1, int u8, int B, int H, int W, float* out,
+                       cudaStream_t stream);
+int lpips_head_launch(const float* a, const float* bias, const float* lin_w, int B, int C, int h,
+                      int w, float* d, cudaStream_t stream);
+size_t lpips_combine_workspace_bytes(int B, int H, int W);
+int lpips_combine_launch(int nmaps, const float* const* maps, const int* map_hw, int B, int H, int W,
+                         const float* mask, int mask_b, float* D, double* num, double* den,
+                         void* workspace, size_t workspace_bytes, cudaStream_t stream);
+int masked_l1_launch(const void* im0, const void* im1, int u8, int B, int H, int W, const float* mask,
+                     int mask_b, double* num, double* den, void* workspace, size_t workspace_bytes,
+                     cudaStream_t stream);
+
 }  // namespace rw

@@ -87,13 +87,20 @@ def _relu_pool(a, bias, pool, planes, fp32):
     return (ops.KeyPlanes(hi, lo, B, C, Ho, Wo) if planes else None), out
 
 
-def _forward(units, x, keep):
-    """The stack's output; with `keep`, also every conv output (what the backward re-reads)."""
+def _forward(units, x, keep, taps=None, on_tap=None):
+    """The stack's output; with `keep`, also every conv output (what the backward re-reads).
+    With `taps` (sorted unit indices), `saved` is instead one (conv output, bias) per tap — the
+    pre-activation output, its bias None where conv_tc added it, else the bias still to add — and
+    the stack stops after the last tap's conv (no ReLU pass for it, no output).  With `on_tap`,
+    `saved` holds on_tap(conv output, bias) instead, called as soon as the tap is formed, so a
+    tap's conv output need not outlive the next unit."""
     x = ops._f32c(x)
     B, _, H, W = x.shape
     planes = ops.prep_keys(x, None)[0] if units[0].tc else None
     act = x
     saved = []
+    if taps is not None:
+        units = units[:taps[-1] + 1]
     for k, u in enumerate(units):
         conv = u.conv
         Cin, Cout = conv.in_channels, conv.out_channels
@@ -107,6 +114,11 @@ def _forward(units, x, keep):
         else:
             a = ops.narrow_conv3x3(act, conv.weight)
             bias = ops._f32c(conv.bias.detach())
+        if taps is not None:
+            if k in taps:
+                saved.append(on_tap(a, bias) if on_tap else (a, bias))
+            if k == taps[-1]:
+                return None, saved
         nxt = units[k + 1] if k + 1 < len(units) else None
         planes, act = _relu_pool(a, bias, u.pool, planes=nxt is not None and nxt.tc,
                                  fp32=nxt is None or not nxt.tc)
