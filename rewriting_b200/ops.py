@@ -271,6 +271,15 @@ def fused_bias_act_raw(x, bias, ref, act, grad, alpha, scale):
     return y
 
 
+def _upfirdn2d_out_len(n, down):
+    """The reference's output length (upfirdn2d_kernel.cu:170-171): `(n + down) / down` in C
+    integer division, which truncates toward zero.  It equals `n // down + 1` for n >= -down;
+    for -2*down < n < -down (a signal shorter than the kernel, decimated) it is 0, where the floor
+    would give -1."""
+    q = n + down
+    return q // down if q >= 0 else -(-q // down)
+
+
 def upfirdn2d_raw(inp, kernel, up_x, up_y, down_x, down_y, px0, px1, py0, py1):
     """The reference's `upfirdn2d_op.upfirdn2d` on a [major, H, W, 1] view
     (op/upfirdn2d.cpp:4-22)."""
@@ -281,12 +290,16 @@ def upfirdn2d_raw(inp, kernel, up_x, up_y, down_x, down_y, px0, px1, py0, py1):
         major_eff = major * minor
     else:
         major_eff = major
+    kernel = _f32c(kernel)
     kh, kw = kernel.shape
-    out_h = (in_h * up_y + py0 + py1 - kh) // down_y + 1
-    out_w = (in_w * up_x + px0 + px1 - kw) // down_x + 1
+    out_h = _upfirdn2d_out_len(in_h * up_y + py0 + py1 - kh, down_y)
+    out_w = _upfirdn2d_out_len(in_w * up_x + px0 + px1 - kw, down_x)
+    if out_h < 0 or out_w < 0:
+        raise _cabi.RwError('upfirdn2d: negative output size %dx%d' % (out_h, out_w))
     out = torch.empty((major_eff, out_h, out_w), dtype=torch.float32, device=inp.device)
-    _cabi.call('rw_upfirdn2d', _p(inp), _p(_f32c(kernel)), major_eff, in_h, in_w, kh, kw, up_x,
-               up_y, down_x, down_y, px0, px1, py0, py1, _p(out), out_h, out_w, _stream())
+    if out.numel():                       # an empty output has no storage to hand the kernel
+        _cabi.call('rw_upfirdn2d', _p(inp), _p(kernel), major_eff, in_h, in_w, kh, kw, up_x,
+                   up_y, down_x, down_y, px0, px1, py0, py1, _p(out), out_h, out_w, _stream())
     if minor != 1:
         return out.view(major, minor, out_h, out_w).permute(0, 2, 3, 1).contiguous()
     return out.view(major, out_h, out_w, 1)
