@@ -51,10 +51,13 @@ constexpr uint32_t kProducerRegs = 40;
 constexpr uint32_t kConsumerRegs = 232;
 // CTAs per cluster: they share (multicast) the weight tile of a k-block
 constexpr int kCluster = 2;
-// The tensor core's fp32 accumulate truncates (round-toward-zero) on every MMA, a relative bias of
-// ~ -2^-25 per accumulation, i.e. 1.6e-5 after the 864 accumulations of a K=4608 tile.  So the
-// wgmma accumulator only ever holds a CHUNK of kChunkKB k-blocks (K=512: 96 accumulations); the
-// chunks are added in fp32 registers with round-to-nearest.
+// The tensor core's fp32 accumulate truncates (round-toward-zero) on every MMA: a chain of n
+// accumulations whose partial sums grow linearly shrinks by about n/2 * 2^-25 (measured: 1-1.3x
+// that with chunks, up to 1.9x for one long chain).  So the wgmma accumulator only ever holds
+// a CHUNK of kChunkKB k-blocks (K=512: 96 accumulations); the chunks are added in fp32 registers
+// with round-to-nearest.  Measured on an H100 at K=4608 (DESIGN.md §4): 1.65e-6 with one-signed
+// operands, 1.4e-6 with mean-zero ones (tests/test_gpu_tc_accumulation.py); with kChunkKB = 256
+// (one chain) 2.2e-5..2.5e-5 and 1.2e-5..1.4e-5.
 // (K=512 -> pixel error 5.2e-4, K=1024 -> 8.1e-4, K >= 2304 fails the 1e-3 bound)
 constexpr int kChunkKB = 16;
 

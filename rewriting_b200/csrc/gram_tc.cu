@@ -29,7 +29,8 @@ constexpr int MMA_K = 16;
 constexpr int kStages = 3;
 // fp32 accumulation in the tensor core truncates (see conv_tc.cu): the wgmma accumulator holds
 // at most kChunkRB row-blocks (1024 rows = 192 accumulations); chunks are summed in fp32
-// registers (round-to-nearest).
+// registers (round-to-nearest).  Measured on an H100 at 135 200 rows (DESIGN.md §4): a shrinkage
+// of 2.7e-6..4.2e-6, 1.0-1.5x the chunk model's n/2 * 2^-25 over each split's chunks.
 constexpr int kChunkRB = 16;
 constexpr int kBlockBytes = 64 * RB * 2;       // one 64-channel x RB-row box
 template <int TM, int TN>
