@@ -92,28 +92,47 @@ def blur_case(name):
     raise ValueError(name)
 
 
-def noise_table(batch, hw, dtype=torch.float32):
+def gated_leaky_relu(x, bias, gate, negative_slope=0.2, scale=SQRT2):
+    """fused_leaky_relu with the sign decision taken from `gate` (bool, x's shape) instead of
+    x + b: where(gate, x + b, 0.2 (x + b)) * scale.  Where gate == (x + b > 0) this is
+    fused_leaky_relu bit for bit, forward and backward; a float64 run given a float32 kernel's
+    gates differentiates through the kernel's own branch of every kink."""
+    shape = [1, -1] + [1] * (x.dim() - 2)
+    pre = x + bias.view(*shape)
+    return torch.where(gate, pre, negative_slope * pre) * scale
+
+
+def noise_table(batch, hw, dtype=torch.float32, device='cpu'):
     """models.py:542-545: RandomState(0).randn(batch, H*W) on every call."""
-    return torch.from_numpy(np.random.RandomState(0).randn(batch, hw).astype('float32')).to(dtype)
+    return torch.from_numpy(np.random.RandomState(0).randn(batch, hw).astype('float32')).to(
+        device=device, dtype=dtype)
 
 
 # ---------------------------------------------------------------------------------------
 # model level
 # ---------------------------------------------------------------------------------------
-def equal_linear(x, weight, bias, lr_mul=1.0, activation=False):
-    """models.py:487-511."""
+def equal_linear(x, weight, bias, lr_mul=1.0, activation=False, gate=None, record_pre=None):
+    """models.py:487-511.  With `activation`, `gate` replaces the leaky ReLU's sign decision
+    (gated_leaky_relu) and `record_pre` (a list) receives its argument x W^T + b."""
     scale = (1 / math.sqrt(weight.shape[1])) * lr_mul
     if activation:
-        return fused_leaky_relu(F.linear(x, weight * scale), bias * lr_mul)
+        x = F.linear(x, weight * scale)
+        if record_pre is not None:
+            record_pre.append(x + bias * lr_mul)
+        if gate is not None:
+            return gated_leaky_relu(x, bias * lr_mul, gate)
+        return fused_leaky_relu(x, bias * lr_mul)
     return F.linear(x, weight * scale, bias=bias * lr_mul)
 
 
-def mapping(sd, z, n_mlp=8, lr_mlp=0.01):
-    """PixelNormL + n_mlp EqualLinearL(fused_lrelu)   (models.py:59-65,609-614)."""
+def mapping(sd, z, n_mlp=8, lr_mlp=0.01, gates=None, record_pre=None):
+    """PixelNormL + n_mlp EqualLinearL(fused_lrelu)   (models.py:59-65,609-614).  `gates`: one
+    per layer (gated_leaky_relu); `record_pre` (a list) receives each pre-activation."""
     w = z * torch.rsqrt(torch.mean(z ** 2, dim=1, keepdim=True) + 1e-8)
     for i in range(1, n_mlp + 1):
         w = equal_linear(w, sd['style.%d.weight' % i], sd['style.%d.bias' % i], lr_mul=lr_mlp,
-                         activation=True)
+                         activation=True, gate=None if gates is None else gates[i - 1],
+                         record_pre=record_pre)
     return w
 
 
@@ -135,21 +154,26 @@ def demod_conv(k, style, weight, upsample):
     return out * demod[:, :, None, None]
 
 
-def styled_conv(x, w_lat, p, upsample, blur_kernel=(1, 3, 3, 1)):
+def styled_conv(x, w_lat, p, upsample, blur_kernel=(1, 3, 3, 1), gate=None):
     """StyledConvSeq with mconv='seq' (models.py:232-289): returns dict with the key `k`
-    (adain output), the dconv output `t`, and the activated output `y`.
-    p: dict(mod_w, mod_b, weight, noise_w, bias)."""
+    (adain output), the dconv output `t`, the leaky ReLU's argument `pre` (t + noise + bias) and
+    the activated output `y`.  p: dict(mod_w, mod_b, weight, noise_w, bias); `gate` replaces the
+    leaky ReLU's sign decision (gated_leaky_relu)."""
     style = modulate(w_lat, p['mod_w'], p['mod_b'])
     k = style[:, :, None, None] * x                                   # ApplyStyle :616-620
     t = demod_conv(k, style, p['weight'], upsample)
     if upsample:                                                      # BlurF :275-281
-        kern = (make_kernel(list(blur_kernel)) * 4).to(t.dtype)
+        kern = (make_kernel(list(blur_kernel)) * 4).to(device=t.device, dtype=t.dtype)
         t = upfirdn2d(t, kern, pad=blur_pads(len(blur_kernel)))
     b, _, h, w = t.shape
-    n = noise_table(b, h * w, t.dtype).view(b, 1, h, w)               # NoiseInjectionF :535-546
-    pre = t + p['noise_w'] * n
-    y = fused_leaky_relu(pre, p['bias'])                              # FusedLeakyReLUF :622-626
-    return dict(style=style, k=k, t=t, y=y)
+    n = noise_table(b, h * w, t.dtype, t.device).view(b, 1, h, w)     # NoiseInjectionF :535-546
+    # FusedLeakyReLUF :622-626 (fused_leaky_relu, with its argument kept for `pre`)
+    pre = t + p['noise_w'] * n + p['bias'].view(1, -1, 1, 1)
+    if gate is None:
+        y = F.leaky_relu(pre, 0.2) * SQRT2
+    else:
+        y = torch.where(gate, pre, 0.2 * pre) * SQRT2
+    return dict(style=style, k=k, t=t, pre=pre, y=y)
 
 
 def to_rgb(x, w_lat, p, skip):
@@ -177,23 +201,34 @@ def _rgb_params(sd, name):
 
 
 def generator_forward(sd, z, size=256, upto_key_layer=None, record=None,
-                      blur_kernel=(1, 3, 3, 1)):
+                      blur_kernel=(1, 3, 3, 1), gates=None):
     """SeqStyleGAN2.forward for mconv='seq', truncation=1 (models.py:92-141).
     `upto_key_layer=N` stops after layerN's adain and returns its key (the context model of
-    ganrewrite.py:48-50).  `record` (dict) receives per-layer activations.  `blur_kernel` is the
-    odd layers' blur; the RGB skip's UpsampleO keeps [1, 3, 3, 1] whatever it is (models.py:117)."""
+    ganrewrite.py:48-50).  `record` (dict) receives per-layer activations (layerN['pre'] is the
+    leaky ReLU's argument) and, under 'mapping_pre', the 8 mapping layers' pre-activations.
+    `blur_kernel` is the odd layers' blur; the RGB skip's UpsampleO keeps [1, 3, 3, 1] whatever
+    it is (models.py:117).  `gates`: one bool tensor per leaky ReLU, the 8 of the mapping network
+    then one per styled conv (layer2, layer3, ...), each replacing that activation's sign decision
+    (gated_leaky_relu); None keeps the plain forward."""
     log_size = int(math.log(size, 2))
-    w = mapping(sd, z)
+    n_conv = 2 * log_size - 3
+    if gates is not None and len(gates) != 8 + n_conv:
+        raise ValueError('generator_forward: %d gates for 8 + %d leaky ReLUs' % (len(gates), n_conv))
+    mapping_pre = [] if record is not None else None
+    w = mapping(sd, z, gates=None if gates is None else gates[:8], record_pre=mapping_pre)
+    if record is not None:
+        record['mapping_pre'] = mapping_pre
     batch = z.shape[0]
     fmap = sd['input.input'].repeat(batch, 1, 1, 1)
-    upk = make_kernel([1, 3, 3, 1]) * 4
+    upk = (make_kernel([1, 3, 3, 1]) * 4).to(fmap.device)
 
     def run_layer(n, x, upsample):
         p = _layer_params(sd, 'layer%d' % n)
         if upto_key_layer == n:
             style = modulate(w, p['mod_w'], p['mod_b'])
             return None, style[:, :, None, None] * x
-        r = styled_conv(x, w, p, upsample, blur_kernel)
+        r = styled_conv(x, w, p, upsample, blur_kernel,
+                        gate=None if gates is None else gates[8 + n - 2])
         if record is not None:
             record['layer%d' % n] = r
         return r['y'], None

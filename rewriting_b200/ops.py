@@ -521,9 +521,11 @@ class ConvTransposeLeafFunction(torch.autograd.Function):
     """t = conv_transpose2d(k, scale*W^T, stride 2) * demod(W, style) on an already-modulated key
     — the `dconv` LEAF of an upsampling layer when nethook has split the layer at it (the blur
     is then the next leaf): reference DemodulatedConv2dF.forward, models.py:313-329, upsample
-    branch.  Differentiable in the weight (incl. the demodulation term) and in the key, which is
-    what the rewriter's edit of an odd layer needs (ganrewrite.py:254-298); the style enters only
-    through demod and gets no gradient here (the rewriter detaches it)."""
+    branch.  Differentiable in the key, in the weight (incl. the demodulation term) and, with
+    demodulation, in the style: the style enters here only through demod, so its gradient is the
+    demodulation term alone (the key's own dependence on the style is ApplyStyle's, upstream).
+    The rewriter's edit of an odd layer (ganrewrite.py:254-298) detaches the style and launches
+    nothing for it."""
 
     @staticmethod
     def forward(ctx, k, style, weight, demodulate, wholder):
@@ -545,16 +547,21 @@ class ConvTransposeLeafFunction(torch.autograd.Function):
     def backward(ctx, gt):
         style, weight, out, dm = ctx.saved_tensors
         B, Cin, Cout, H, W = ctx.shape
-        need_k, _, need_w = ctx.needs_input_grad[:3]
+        need_k, need_style, need_w = ctx.needs_input_grad[:3]
+        need_style = need_style and dm is not None
         gt = _f32c(gt)
         dev = gt.device
+        # dL/d(demod) * demod = sum_pixels g_t * t  (t is the saved, demodulated output)
+        s_dot = None
+        if dm is not None and (need_w or need_style):
+            s_dot = (gt * out).sum(dim=(2, 3)).contiguous()
         rows = B * (H + 1) * (W + 1)
         gph_hi = torch.empty((rows, 4 * Cout), dtype=torch.bfloat16, device=dev)
         gph_lo = torch.empty_like(gph_hi)
         # phase planes of g_t * demod over the input-resolution padded grid
         _cabi.call('rw_prep_phase_keys', _p(gt), _p(dm), B, Cout, H, W, _p(gph_hi), _p(gph_lo),
                    _stream())
-        gk = gW = None
+        gk = g_style = gW = None
         if need_k:
             wd_hi, wd_lo, _ = ctx.wholder.planes('dgrad_up')
             gk = torch.empty((B, Cin, H, W), dtype=torch.float32, device=dev)
@@ -567,12 +574,15 @@ class ConvTransposeLeafFunction(torch.autograd.Function):
             _cabi.call('rw_conv_up_wgrad', _p(gph_hi), _p(gph_lo), _p(ctx.planes.hi),
                        _p(ctx.planes.lo), rows, Cout, Cin, W + 1, _p(dwt), _p(ws), ws.numel() * 4,
                        _stream())
-            # dL/d(demod) * demod = sum_pixels g_t * t  (t is the saved, demodulated output)
-            s_dot = (gt * out).sum(dim=(2, 3)).contiguous() if dm is not None else None
             gW = torch.empty(weight.shape, dtype=torch.float32, device=dev)
             _cabi.call('rw_wgrad_finish', _p(dwt), _p(_f32c(weight.detach())), _p(s_dot), _p(dm),
                        _p(style), B, Cout, Cin, 1.0 / math.sqrt(Cin * 9), _p(gW), _stream())
-        return gk, None, gW, None, None
+        if need_style:
+            # the demodulation term only (no gs_raw: the key arrives modulated)
+            g_style = torch.empty((B, Cin), dtype=torch.float32, device=dev)
+            _cabi.call('rw_style_grad_finish', None, _p(style), _p(s_dot), _p(dm),
+                       _p(ctx.wholder.planes('fwd')[2]), B, Cout, Cin, _p(g_style), _stream())
+        return gk, g_style, gW, None, None
 
 
 def conv_transpose_leaf(k, style, weight, demodulate=True):
