@@ -462,20 +462,7 @@ int rw_masked_l1(const void* im0, const void* im1, int u8, int B, int H, int W, 
                  int mask_b, double* num, double* den, void* workspace, size_t workspace_bytes,
                  rw_stream_t stream);
 
-/* ---- bring-up hooks (tests/tools only) ---- */
-/* rw_modconv_up_fused with demod = next_scale = ones_bo, additionally dumping the raw tap products
- * P[b][y][x][tap][Cout] of the tensor-core stage */
-int rw_debug_upconv_taps(const void* kp_hi, const void* kp_lo, const void* wt_hi, const void* wt_lo,
-                         const float* ones_bo, const float* kernel4x4, const float* noise,
-                         long long noise_bstride, const float* noise_w, const float* bias,
-                         void* next_hi, void* next_lo, int B, int Cin, int Cout, int H, int W,
-                         float* taps_out, rw_stream_t stream);
-int rw_debug_rowgemm(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo,
-                     int rows, int K, int N, float* out, rw_stream_t stream);
-int rw_debug_colgemm(const void* a_hi, const void* a_lo, const void* b_hi, const void* b_lo,
-                     int rows, int Cm, int Cn, int lbo_bytes, int sbo_bytes, float* out,
-                     void* workspace, size_t workspace_bytes, rw_stream_t stream);
-
+/* ---- per-phase profiles (tools/prof_upconv.py, tools/prof_conv.py) ---- */
 /* rw_modconv_up_fused instrumented with clock64(): prof_out[grid][8 epilogue warps][16] = cycles in
  * {wait for the MMAs, accumulator exchange, combine + mailbox + barrier, shuffles, edge-lane fix-ups,
  * horizontal FIR, vertical FIR + activation + stores}, the step count, and the last phase split into

@@ -68,8 +68,6 @@ SIGNATURES = {
                                     c_int, c_int, c_int, c_int, c_int, c_p]),
     'rw_modconv_up_fused_y': (c_int, [c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_ll, c_p, c_p, c_int, c_p,
                                       c_int, c_int, c_int, c_int, c_int, c_p]),
-    'rw_debug_upconv_taps': (c_int, [c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_ll, c_p, c_p, c_p, c_p,
-                                     c_int, c_int, c_int, c_int, c_int, c_p, c_p]),
     'rw_rowgemm': (c_int, [c_p, c_p, c_p, c_p, c_int, c_int, c_int, c_p, c_p]),
     'rw_pixel_norm_nchw': (c_int, [c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p]),
     'rw_nearest_up2': (c_int, [c_p, c_ll, c_int, c_int, c_p, c_p]),
@@ -145,9 +143,6 @@ SIGNATURES = {
     'rw_insert_up_workspace_bytes': (c_sz, [c_int, c_int, c_int, c_int]),
     'rw_insert_loop_up': (c_int, [ctypes.POINTER(InsertArgs), c_p, c_p, c_sz, c_p]),
     'rw_linear_insert_loop_up': (c_int, [ctypes.POINTER(LinearInsertArgs), c_p, c_p, c_sz, c_p]),
-    'rw_debug_rowgemm': (c_int, [c_p, c_p, c_p, c_p, c_int, c_int, c_int, c_p, c_p]),
-    'rw_debug_colgemm': (c_int, [c_p, c_p, c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_p,
-                                 c_p, c_sz, c_p]),
 }
 
 _lib = None
@@ -188,7 +183,7 @@ def check(rc, what):
 # kernels launched per entry point (for bench.py's `gpu_launches` claim)
 LAUNCHES_PER_CALL = {
     'rw_second_moment_accum': 2, 'rw_conv_wgrad': 2, 'rw_conv_up_wgrad': 2,
-    'rw_debug_colgemm': 2, 'rw_narrow_conv3x3_wgrad': 2, 'rw_torgb1x1_wgrad': 2,
+    'rw_narrow_conv3x3_wgrad': 2, 'rw_torgb1x1_wgrad': 2,
 }
 launch_count = 0
 

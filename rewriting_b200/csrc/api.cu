@@ -2,7 +2,6 @@
 // small host-side utilities shared by the kernel translation units.
 #include <cstdarg>
 #include <cstdio>
-#include <cstdlib>
 #include <cstring>
 #include <mutex>
 
@@ -151,16 +150,87 @@ int make_tmap_nd_bf16(CUtensorMap* out, const void* base, int rank, const uint64
   return RW_OK;
 }
 
-// split heuristic shared by the workspace query and the launches
-static int gram_splits(int tiles, long long rows, int ntaps) {
+// split heuristic shared by the workspace query and the launches; upper_only (symmetric output)
+// runs only the tiles on and above the diagonal
+static int gram_splits(int Cm, int Cn, long long rows, int ntaps, bool upper_only) {
+  const int mt = Cm / gram_tile_width(Cm);
+  const int tiles = upper_only ? mt * (mt + 1) / 2 : gram_tiles(Cm, Cn);
   const long long total_rb = (rows + 63) / 64;
   const int sms = device_sm_count();
   long long s = (sms + static_cast<long long>(tiles) * ntaps - 1) / (static_cast<long long>(tiles) * ntaps);
   if (s > total_rb) s = total_rb;
   if (s < 1) s = 1;
   if (s > 64) s = 64;
-  (void)0;
   return static_cast<int>(s);
+}
+
+// The col-GEMM behind every gram entry point.  p holds the shape (Cm, Cn, ntaps, upper_only,
+// a_cols) and the tap tables; this sets the row range, the splits and the partials' layout, checks
+// the workspace, launches, and reduces the partials into out [Cm][ntaps * Cn] (+= when accumulate,
+// mirrored into the lower triangle when upper_only).
+static int gram_run(const char* who, GramTcParams& p, long long rows, const void* a_hi,
+                    const void* a_lo, const void* b_hi, const void* b_lo, float* out, int accumulate,
+                    void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  p.rows = p.rows_a = p.rows_b = static_cast<int>(rows);
+  p.splits = gram_splits(p.Cm, p.Cn, rows, p.ntaps, p.upper_only != 0);
+  p.ldp = static_cast<long long>(p.ntaps) * p.Cn;
+  p.partial = static_cast<float*>(workspace);
+  const size_t need = static_cast<size_t>(p.splits) * p.Cm * p.ldp * sizeof(float);
+  if (workspace_bytes < need) {
+    set_last_error("%s: workspace %zu < %zu bytes", who, workspace_bytes, need);
+    return RW_ERR_BAD_ARG;
+  }
+  int rc = gram_tc_launch(p, a_hi, a_lo, b_hi, b_lo, stream);
+  if (rc) return rc;
+  return reduce_partials_launch(p.partial, p.splits, p.Cm, static_cast<int>(p.ldp), p.ldp, out,
+                                p.ldp, accumulate, p.upper_only, stream);
+}
+
+// the 3x3 same-size conv over the padded-flat grid of B images H x W: one phase of 9 taps,
+// NCHW output strides
+static int fill_conv3x3(ConvTcParams& p, const char* who, int B, int Cin, int Cout, int H, int W) {
+  memset(&p, 0, sizeof(p));
+  p.Hp = H + 1;
+  p.Wp = W + 1;
+  p.B = B;
+  p.nphase = 1;
+  p.ph_Hv[0] = H;
+  p.ph_Wv[0] = W;
+  const long long rows = static_cast<long long>(B) * p.Hp * p.Wp;
+  if (rows > 0x7fffffffLL) {
+    set_last_error("%s: too many rows", who);
+    return RW_ERR_BAD_ARG;
+  }
+  p.rows = static_cast<int>(rows);
+  p.Cin = Cin;
+  p.Cout = Cout;
+  p.ph_ntaps[0] = 9;
+  for (int u = 0; u < 3; ++u)
+    for (int v = 0; v < 3; ++v) {
+      p.ph_shift[0][u * 3 + v] = (u - 1) * p.Wp + (v - 1);
+      p.ph_kofs[0][u * 3 + v] = (u * 3 + v) * Cin;
+    }
+  p.out_sb = static_cast<long long>(Cout) * H * W;
+  p.out_sc = static_cast<long long>(H) * W;
+  p.out_sy = W;
+  p.out_sx = 1;
+  return RW_OK;
+}
+
+// the fused upsampling conv's parameters common to its entry points; next_* are null in
+// layer-level mode (y_out)
+static UpFusedParams up_fused_params(int B, int Cin, int Cout, int H, int W, const float* demod,
+                                     const float* kernel4x4, const float* noise,
+                                     long long noise_bstride, const float* noise_w,
+                                     const float* bias, const float* next_scale, void* next_hi,
+                                     void* next_lo) {
+  UpFusedParams p;
+  memset(&p, 0, sizeof(p));
+  p.B = B; p.Cin = Cin; p.Cout = Cout; p.H = H; p.W = W;
+  p.demod = demod; p.bias = bias; p.noise = noise; p.noise_bstride = noise_bstride;
+  p.noise_w = noise_w; p.k4 = kernel4x4; p.next_scale = next_scale;
+  p.next_hi = next_hi; p.next_lo = next_lo;
+  return p;
 }
 
 }  // namespace rw
@@ -220,27 +290,8 @@ int rw_modconv_fwd(const void* kp_hi, const void* kp_lo, const void* wt_hi, cons
     return RW_ERR_BAD_ARG;
   }
   ConvTcParams p;
-  memset(&p, 0, sizeof(p));
-  p.Hp = H + 1;
-  p.Wp = W + 1;
-  p.B = B;
-  p.nphase = 1;
-  p.ph_Hv[0] = H;
-  p.ph_Wv[0] = W;
-  const long long rows = static_cast<long long>(B) * p.Hp * p.Wp;
-  if (rows > 0x7fffffffLL) {
-    set_last_error("rw_modconv_fwd: too many rows");
-    return RW_ERR_BAD_ARG;
-  }
-  p.rows = static_cast<int>(rows);
-  p.Cin = Cin;
-  p.Cout = Cout;
-  p.ph_ntaps[0] = 9;
-  for (int u = 0; u < 3; ++u)
-    for (int v = 0; v < 3; ++v) {
-      p.ph_shift[0][u * 3 + v] = (u - 1) * p.Wp + (v - 1);
-      p.ph_kofs[0][u * 3 + v] = (u * 3 + v) * Cin;
-    }
+  int rc = fill_conv3x3(p, "rw_modconv_fwd", B, Cin, Cout, H, W);
+  if (rc) return rc;
   p.scale_bo = scale_bo;
   p.bias = bias;
   p.noise = noise;
@@ -248,10 +299,6 @@ int rw_modconv_fwd(const void* kp_hi, const void* kp_lo, const void* wt_hi, cons
   p.noise_w = noise_w;
   p.act = act;
   p.out = out;
-  p.out_sb = static_cast<long long>(Cout) * H * W;
-  p.out_sc = static_cast<long long>(H) * W;
-  p.out_sy = W;
-  p.out_sx = 1;
   return conv_tc_launch(p, kp_hi, kp_lo, wt_hi, wt_lo, 9 * Cin, stream);
 }
 
@@ -326,35 +373,6 @@ int rw_modconv_up_fwd_cl(const void* kp_hi, const void* kp_lo, const void* wt_hi
   return modconv_up_impl(kp_hi, kp_lo, wt_hi, wt_lo, scale_bo, B, Cin, Cout, H, W, t_cl, 1, stream);
 }
 
-static int fill_conv3x3(ConvTcParams& p, int B, int Cin, int Cout, int H, int W) {
-  memset(&p, 0, sizeof(p));
-  p.Hp = H + 1;
-  p.Wp = W + 1;
-  p.B = B;
-  p.nphase = 1;
-  p.ph_Hv[0] = H;
-  p.ph_Wv[0] = W;
-  const long long rows = static_cast<long long>(B) * p.Hp * p.Wp;
-  if (rows > 0x7fffffffLL) {
-    set_last_error("conv: too many rows");
-    return RW_ERR_BAD_ARG;
-  }
-  p.rows = static_cast<int>(rows);
-  p.Cin = Cin;
-  p.Cout = Cout;
-  p.ph_ntaps[0] = 9;
-  for (int u = 0; u < 3; ++u)
-    for (int v = 0; v < 3; ++v) {
-      p.ph_shift[0][u * 3 + v] = (u - 1) * p.Wp + (v - 1);
-      p.ph_kofs[0][u * 3 + v] = (u * 3 + v) * Cin;
-    }
-  p.out_sb = static_cast<long long>(Cout) * H * W;
-  p.out_sc = static_cast<long long>(H) * W;
-  p.out_sy = W;
-  p.out_sx = 1;
-  return RW_OK;
-}
-
 int rw_conv3x3_bias_act(const void* kp_hi, const void* kp_lo, const void* wt_hi, const void* wt_lo,
                         const float* bias, int act, float act_gain, int B, int Cin, int Cout, int H,
                         int W, float* out, rw_stream_t stream) {
@@ -363,7 +381,7 @@ int rw_conv3x3_bias_act(const void* kp_hi, const void* kp_lo, const void* wt_hi,
     return RW_ERR_BAD_ARG;
   }
   ConvTcParams p;
-  int rc = fill_conv3x3(p, B, Cin, Cout, H, W);
+  int rc = fill_conv3x3(p, "rw_conv3x3_bias_act", B, Cin, Cout, H, W);
   if (rc) return rc;
   p.bias = bias;
   p.act = act;
@@ -575,7 +593,7 @@ static int modconv_fused_impl(const void* kp_hi, const void* kp_lo, const void* 
     return RW_ERR_BAD_ARG;
   }
   ConvTcParams p;
-  int rc = fill_conv3x3(p, B, Cin, Cout, H, W);
+  int rc = fill_conv3x3(p, "rw_modconv_fwd_fused", B, Cin, Cout, H, W);
   if (rc) return rc;
   p.scale_bo = scale_bo;
   p.bias = bias;
@@ -630,12 +648,8 @@ int rw_modconv_up_fused(const void* kp_hi, const void* kp_lo, const void* wt_hi,
     set_last_error("rw_modconv_up_fused: bad argument");
     return RW_ERR_BAD_ARG;
   }
-  UpFusedParams p;
-  memset(&p, 0, sizeof(p));
-  p.B = B; p.Cin = Cin; p.Cout = Cout; p.H = H; p.W = W;
-  p.demod = demod; p.bias = bias; p.noise = noise; p.noise_bstride = noise_bstride;
-  p.noise_w = noise_w; p.k4 = kernel4x4; p.next_scale = next_scale;
-  p.next_hi = next_hi; p.next_lo = next_lo;
+  const UpFusedParams p = up_fused_params(B, Cin, Cout, H, W, demod, kernel4x4, noise,
+                                          noise_bstride, noise_w, bias, next_scale, next_hi, next_lo);
   return upconv_fused_launch(p, kp_hi, kp_lo, wt_hi, wt_lo, stream);
 }
 
@@ -648,28 +662,10 @@ int rw_modconv_up_fused_y(const void* kp_hi, const void* kp_lo, const void* wt_h
     set_last_error("rw_modconv_up_fused_y: bad argument");
     return RW_ERR_BAD_ARG;
   }
-  UpFusedParams p;
-  memset(&p, 0, sizeof(p));
-  p.B = B; p.Cin = Cin; p.Cout = Cout; p.H = H; p.W = W;
-  p.demod = demod; p.bias = bias; p.noise = noise; p.noise_bstride = noise_bstride;
-  p.noise_w = noise_w; p.k4 = kernel4x4;
+  UpFusedParams p = up_fused_params(B, Cin, Cout, H, W, demod, kernel4x4, noise, noise_bstride,
+                                    noise_w, bias, nullptr, nullptr, nullptr);
   p.y_out = y;
   p.act = act;
-  return upconv_fused_launch(p, kp_hi, kp_lo, wt_hi, wt_lo, stream);
-}
-
-int rw_debug_upconv_taps(const void* kp_hi, const void* kp_lo, const void* wt_hi, const void* wt_lo,
-                         const float* ones_bo, const float* kernel4x4, const float* noise,
-                         long long noise_bstride, const float* noise_w, const float* bias,
-                         void* next_hi, void* next_lo, int B, int Cin, int Cout, int H, int W,
-                         float* taps_out, rw_stream_t stream) {
-  UpFusedParams p;
-  memset(&p, 0, sizeof(p));
-  p.B = B; p.Cin = Cin; p.Cout = Cout; p.H = H; p.W = W;
-  p.demod = ones_bo; p.bias = bias; p.noise = noise; p.noise_bstride = noise_bstride;
-  p.noise_w = noise_w; p.k4 = kernel4x4; p.next_scale = ones_bo;
-  p.next_hi = next_hi; p.next_lo = next_lo;
-  p.debug_p = taps_out;
   return upconv_fused_launch(p, kp_hi, kp_lo, wt_hi, wt_lo, stream);
 }
 
@@ -679,14 +675,9 @@ int rw_debug_upconv_profile(const void* kp_hi, const void* kp_lo, const void* wt
                             const float* bias, const float* next_scale, void* next_hi, void* next_lo,
                             int B, int Cin, int Cout, int H, int W, long long* prof_out,
                             rw_stream_t stream) {
-  UpFusedParams p;
-  memset(&p, 0, sizeof(p));
-  p.B = B; p.Cin = Cin; p.Cout = Cout; p.H = H; p.W = W;
-  p.demod = demod; p.bias = bias; p.noise = noise; p.noise_bstride = noise_bstride;
-  p.noise_w = noise_w; p.k4 = kernel4x4; p.next_scale = next_scale;
-  p.next_hi = next_hi; p.next_lo = next_lo;
+  UpFusedParams p = up_fused_params(B, Cin, Cout, H, W, demod, kernel4x4, noise, noise_bstride,
+                                    noise_w, bias, next_scale, next_hi, next_lo);
   p.debug_prof = prof_out;
-  p.debug_nostore = getenv("RW_UP_NOSTORE") != nullptr;
   return upconv_fused_launch(p, kp_hi, kp_lo, wt_hi, wt_lo, stream);
 }
 
@@ -814,12 +805,9 @@ int rw_upfirdn2d(const float* in, const float* kernel, int major, int in_h, int 
 
 size_t rw_gram_workspace_bytes(int Cm, int Cn, long long rows, int ntaps) {
   if (Cm < 64 || Cn < 64 || Cm % 64 != 0 || Cn % 64 != 0 || ntaps < 1) return 0;
-  const int mt = Cm / gram_tile_width(Cm);
-  const int tiles_full = gram_tiles(Cm, Cn);
   // the symmetric path uses fewer tiles -> more splits; size for the larger of the two
-  const int tiles_sym = (Cm == Cn) ? mt * (mt + 1) / 2 : tiles_full;
-  const int s1 = gram_splits(tiles_full, rows, ntaps);
-  const int s2 = gram_splits(tiles_sym, rows, ntaps);
+  const int s1 = gram_splits(Cm, Cn, rows, ntaps, false);
+  const int s2 = gram_splits(Cm, Cn, rows, ntaps, Cm == Cn);
   const int s = s1 > s2 ? s1 : s2;
   return static_cast<size_t>(s) * Cm * static_cast<size_t>(Cn) * ntaps * sizeof(float);
 }
@@ -833,24 +821,11 @@ int rw_second_moment_accum(const void* hi, const void* lo, long long rows, int C
   }
   GramTcParams p;
   memset(&p, 0, sizeof(p));
-  p.rows = static_cast<int>(rows);
-  p.rows_a = p.rows_b = static_cast<int>(rows);
   p.Cm = p.Cn = C;
   p.ntaps = 1;
   p.upper_only = 1;
-  const int mt = C / gram_tile_width(C);
-  p.splits = gram_splits(mt * (mt + 1) / 2, rows, 1);
-  p.ldp = C;
-  p.partial = static_cast<float*>(workspace);
-  const size_t need = static_cast<size_t>(p.splits) * C * C * sizeof(float);
-  if (workspace_bytes < need) {
-    set_last_error("rw_second_moment_accum: workspace %zu < %zu bytes", workspace_bytes, need);
-    return RW_ERR_BAD_ARG;
-  }
-  int rc = gram_tc_launch(p, hi, lo, hi, lo, stream);
-  if (rc) return rc;
-  return reduce_partials_launch(p.partial, p.splits, C, C, p.ldp, mom2, C, /*accumulate=*/1,
-                                /*mirror_upper=*/1, stream);
+  return gram_run("rw_second_moment_accum", p, rows, hi, lo, hi, lo, mom2, /*accumulate=*/1,
+                  workspace, workspace_bytes, stream);
 }
 
 int rw_conv_wgrad(const void* g_hi, const void* g_lo, const void* kp_hi, const void* kp_lo,
@@ -863,8 +838,6 @@ int rw_conv_wgrad(const void* g_hi, const void* g_lo, const void* kp_hi, const v
   }
   GramTcParams p;
   memset(&p, 0, sizeof(p));
-  p.rows = static_cast<int>(rows);
-  p.rows_a = p.rows_b = static_cast<int>(rows);
   p.Cm = Cout;
   p.Cn = Cin;
   p.ntaps = 9;
@@ -873,19 +846,8 @@ int rw_conv_wgrad(const void* g_hi, const void* g_lo, const void* kp_hi, const v
       p.tap_shift_b[u * 3 + v] = (u - 1) * Wp + (v - 1);
       p.tap_col_ofs[u * 3 + v] = (u * 3 + v) * Cin;
     }
-  p.upper_only = 0;
-  p.splits = gram_splits(gram_tiles(Cout, Cin), rows, 9);
-  p.ldp = 9LL * Cin;
-  p.partial = static_cast<float*>(workspace);
-  const size_t need = static_cast<size_t>(p.splits) * Cout * 9 * Cin * sizeof(float);
-  if (workspace_bytes < need) {
-    set_last_error("rw_conv_wgrad: workspace %zu < %zu bytes", workspace_bytes, need);
-    return RW_ERR_BAD_ARG;
-  }
-  int rc = gram_tc_launch(p, g_hi, g_lo, kp_hi, kp_lo, stream);
-  if (rc) return rc;
-  return reduce_partials_launch(p.partial, p.splits, Cout, 9 * Cin, p.ldp, dw_toi, 9LL * Cin,
-                                /*accumulate=*/0, /*mirror_upper=*/0, stream);
+  return gram_run("rw_conv_wgrad", p, rows, g_hi, g_lo, kp_hi, kp_lo, dw_toi, /*accumulate=*/0,
+                  workspace, workspace_bytes, stream);
 }
 
 int rw_prep_phase_keys(const float* g, const float* scale_bc, int B, int C, int H, int W,
@@ -908,7 +870,7 @@ int rw_modconv_up_dgrad(const void* gph_hi, const void* gph_lo, const void* wt_h
   }
   // GEMM: M = input pixels, K = 9 taps x Cout (gradient channels), N = Cin
   ConvTcParams p;
-  int rc = fill_conv3x3(p, B, /*Cin(K)=*/Cout, /*Cout(N)=*/Cin, H, W);
+  int rc = fill_conv3x3(p, "rw_modconv_up_dgrad", B, /*Cin(K)=*/Cout, /*Cout(N)=*/Cin, H, W);
   if (rc) return rc;
   p.a_cols = 4 * Cout;
   for (int u = 0; u < 3; ++u)
@@ -933,8 +895,6 @@ int rw_conv_up_wgrad(const void* gph_hi, const void* gph_lo, const void* kp_hi, 
   }
   GramTcParams p;
   memset(&p, 0, sizeof(p));
-  p.rows = static_cast<int>(rows);
-  p.rows_a = p.rows_b = static_cast<int>(rows);
   p.Cm = Cout;
   p.Cn = Cin;
   p.a_cols = 4 * Cout;
@@ -946,18 +906,8 @@ int rw_conv_up_wgrad(const void* gph_hi, const void* gph_lo, const void* kp_hi, 
       p.tap_acol[t] = ((u & 1) * 2 + (v & 1)) * Cout;
       p.tap_col_ofs[t] = t * Cin;
     }
-  p.splits = gram_splits(gram_tiles(Cout, Cin), rows, 9);
-  p.ldp = 9LL * Cin;
-  p.partial = static_cast<float*>(workspace);
-  const size_t need = static_cast<size_t>(p.splits) * Cout * 9 * Cin * sizeof(float);
-  if (workspace_bytes < need) {
-    set_last_error("rw_conv_up_wgrad: workspace %zu < %zu bytes", workspace_bytes, need);
-    return RW_ERR_BAD_ARG;
-  }
-  int rc = gram_tc_launch(p, gph_hi, gph_lo, kp_hi, kp_lo, stream);
-  if (rc) return rc;
-  return reduce_partials_launch(p.partial, p.splits, Cout, 9 * Cin, p.ldp, dw_toi, 9LL * Cin, 0, 0,
-                                stream);
+  return gram_run("rw_conv_up_wgrad", p, rows, gph_hi, gph_lo, kp_hi, kp_lo, dw_toi,
+                  /*accumulate=*/0, workspace, workspace_bytes, stream);
 }
 
 int rw_act_grad_reduce(const float* gy, const float* y, const float* noise,
@@ -1126,43 +1076,18 @@ int rw_linear_insert_loop_up(const rw_linear_insert_args* a, const float blur[16
   return linear_insert_up_launch(p, blur, workspace, workspace_bytes, stream);
 }
 
-int rw_debug_rowgemm(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo,
-                     int rows, int K, int N, float* out, rw_stream_t stream) {
-  ConvTcParams p;
-  memset(&p, 0, sizeof(p));
-  p.rows = rows; p.Cin = K; p.Cout = N; p.nphase = 1; p.ph_ntaps[0] = 1;
-  p.Hp = 1; p.Wp = rows; p.ph_Hv[0] = 1; p.ph_Wv[0] = rows;   // one "image" = all rows
-  p.out = out; p.out_sb = 0; p.out_sc = 1; p.out_sy = 0; p.out_sx = N;  // row-major [rows][N]
-  return conv_tc_launch(p, a_hi, a_lo, w_hi, w_lo, K, stream);
-}
-
 int rw_rowgemm(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo, int rows, int K,
                int N, float* out, rw_stream_t stream) {
   if (!a_hi || !a_lo || !w_hi || !w_lo || !out || rows < 1 || K % 64 != 0 || N % 64 != 0) {
     set_last_error("rw_rowgemm: bad argument (rows=%d K=%d N=%d)", rows, K, N);
     return RW_ERR_BAD_ARG;
   }
-  return rw_debug_rowgemm(a_hi, a_lo, w_hi, w_lo, rows, K, N, out, stream);
-}
-
-int rw_debug_colgemm(const void* a_hi, const void* a_lo, const void* b_hi, const void* b_lo,
-                     int rows, int Cm, int Cn, int lbo_bytes, int sbo_bytes, float* out,
-                     void* workspace, size_t workspace_bytes, rw_stream_t stream) {
-  GramTcParams p;
+  ConvTcParams p;
   memset(&p, 0, sizeof(p));
-  p.rows = rows; p.rows_a = p.rows_b = rows; p.Cm = Cm; p.Cn = Cn; p.ntaps = 1;
-  p.splits = gram_splits(gram_tiles(Cm, Cn), rows, 1);
-  p.ldp = Cn;
-  p.partial = static_cast<float*>(workspace);
-  const size_t need = static_cast<size_t>(p.splits) * Cm * Cn * sizeof(float);
-  if (workspace_bytes < need) {
-    set_last_error("rw_debug_colgemm: workspace %zu < %zu bytes", workspace_bytes, need);
-    return RW_ERR_BAD_ARG;
-  }
-  if (lbo_bytes > 0 && sbo_bytes > 0) gram_tc_set_desc(lbo_bytes, sbo_bytes);
-  int rc = gram_tc_launch(p, a_hi, a_lo, b_hi, b_lo, stream);
-  if (rc) return rc;
-  return reduce_partials_launch(p.partial, p.splits, Cm, Cn, p.ldp, out, Cn, 0, 0, stream);
+  p.rows = rows; p.Cin = K; p.Cout = N; p.nphase = 1; p.ph_ntaps[0] = 1;
+  p.Hp = 1; p.Wp = rows; p.ph_Hv[0] = 1; p.ph_Wv[0] = rows;   // one "image" = all rows
+  p.out = out; p.out_sb = 0; p.out_sc = 1; p.out_sy = 0; p.out_sx = N;  // row-major [rows][N]
+  return conv_tc_launch(p, a_hi, a_lo, w_hi, w_lo, K, stream);
 }
 
 }  // extern "C"

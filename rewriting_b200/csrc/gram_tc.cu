@@ -11,10 +11,11 @@
 // Operands are the bf16 hi/lo planes [rows][C] (channels contiguous), i.e. the
 // contraction index is the *slow* one: both operands are MN-major for the
 // tensor core.  TMA boxes of 64 channels x 64 rows land as 128-byte swizzled
-// rows; the wgmma descriptor walks 8-row groups with SBO and 64-channel blocks
-// with LBO.  Three MMAs per k-step (hi*hi + lo*hi + hi*lo), fp32 accumulate in
-// registers.  Row ranges are split across CTAs; partial tiles go to a workspace that
-// a second kernel reduces in a fixed order (bit-reproducible, unlike atomics).
+// rows; the wgmma descriptor walks 8-row groups with SBO = 1024 B and 64-channel
+// blocks with LBO = one box (kBlockBytes).  Three MMAs per k-step (hi*hi + lo*hi
+// + hi*lo), fp32 accumulate in registers.  Row ranges are split across CTAs;
+// partial tiles go to a workspace that a second kernel reduces in a fixed order
+// (bit-reproducible, unlike atomics).
 #include "rw_common.cuh"
 #include "rw_kernels.h"
 
@@ -55,8 +56,7 @@ __global__ void __launch_bounds__(GramCfg<TM, TN>::kNumThreads, 1)
 gram_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
                const __grid_constant__ CUtensorMap map_a_lo,
                const __grid_constant__ CUtensorMap map_b_hi,
-               const __grid_constant__ CUtensorMap map_b_lo, const GramTcParams p,
-               const int lbo_bytes, const int sbo_bytes) {
+               const __grid_constant__ CUtensorMap map_b_lo, const GramTcParams p) {
   using G = GramCfg<TM, TN>;
   constexpr int kTmaWarp = G::kTmaWarp, kStageBytes = G::kStageBytes;
   constexpr int kAPlane = G::kAPlaneBytes, kBPlane = G::kBPlaneBytes;
@@ -152,10 +152,10 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
     for (int i = i0; i < i_end; ++i) {
       mbar_wait(&bars->full[stage], phase);
       const uint32_t sa = smem_u32(smem + stage * kStageBytes);
-      const uint64_t da_hi = make_smem_desc(sa + wg * kBlockBytes, lbo_bytes, sbo_bytes);
-      const uint64_t da_lo = make_smem_desc(sa + kAPlane + wg * kBlockBytes, lbo_bytes, sbo_bytes);
-      const uint64_t db_hi = make_smem_desc(sa + 2 * kAPlane, lbo_bytes, sbo_bytes);
-      const uint64_t db_lo = make_smem_desc(sa + 2 * kAPlane + kBPlane, lbo_bytes, sbo_bytes);
+      const uint64_t da_hi = make_smem_desc(sa + wg * kBlockBytes, kBlockBytes, 1024);
+      const uint64_t da_lo = make_smem_desc(sa + kAPlane + wg * kBlockBytes, kBlockBytes, 1024);
+      const uint64_t db_hi = make_smem_desc(sa + 2 * kAPlane, kBlockBytes, 1024);
+      const uint64_t db_lo = make_smem_desc(sa + 2 * kAPlane + kBPlane, kBlockBytes, 1024);
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < RB / MMA_K; ++kk) {
@@ -242,12 +242,6 @@ reduce_partials_kernel(const float* __restrict__ partial, int splits, int M, int
 
 }  // namespace
 
-// test hook: descriptor geometry can be overridden to pin the MN-major LBO/SBO convention on
-// hardware.
-static int g_gram_lbo = kBlockBytes;
-static int g_gram_sbo = 1024;
-void gram_tc_set_desc(int lbo, int sbo) { g_gram_lbo = lbo; g_gram_sbo = sbo; }
-
 template <int TM, int TN>
 static int gram_tc_launch_tile(const GramTcParams& p, const CUtensorMap& ma_hi,
                                const CUtensorMap& ma_lo, const CUtensorMap& mb_hi,
@@ -266,7 +260,7 @@ static int gram_tc_launch_tile(const GramTcParams& p, const CUtensorMap& ma_hi,
   const int tiles = p.upper_only ? mt * (mt + 1) / 2 : mt * nt;
   dim3 grid(tiles, p.splits, p.ntaps);
   gram_tc_kernel<TM, TN><<<grid, G::kNumThreads, G::kSmemTotal, stream>>>(
-      ma_hi, ma_lo, mb_hi, mb_lo, p, g_gram_lbo, g_gram_sbo);
+      ma_hi, ma_lo, mb_hi, mb_lo, p);
   return check_cuda(cudaGetLastError(), "gram_tc launch");
 }
 

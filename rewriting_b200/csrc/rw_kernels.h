@@ -79,9 +79,8 @@ struct UpFusedParams {
   float* y_out;
   int act;
   int ncg, nbands, nitems;     // filled by the launcher
-  float* debug_p;              // bring-up: raw tap products P[b][y][x][tap][Cout] (y < H), or null
-  int debug_nostore;           // bring-up (profiling variant only): skip the plane stores
-  long long* debug_prof;       // bring-up: per (CTA, epilogue warp) cycle counters [grid][8][16], or null
+  long long* debug_prof;       // per (CTA, epilogue warp) cycle counters [grid][8][16], or null
+                               // (rw_debug_upconv_profile)
 };
 // weights: bf16 hi/lo planes [Cout/16][channel half][9 taps][8][Cin]  (rw_prep_weights, transpose_io = 2)
 int upconv_fused_launch(const UpFusedParams& p, const void* a_hi, const void* a_lo,
@@ -191,7 +190,6 @@ int style_grad_finish_launch(const float* gs_raw, const float* style, const floa
 int project_rank_launch_signed(const float* w, const float* base, const float* d, int rank,
                                int Cout, int Cin, int taps, float sign, float* out,
                                cudaStream_t stream);
-void gram_tc_set_desc(int lbo, int sbo);
 
 struct InsertLoopParams {
   float* W;             // [Cout, Cin, 3, 3] updated in place

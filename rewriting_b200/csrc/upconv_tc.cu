@@ -376,14 +376,6 @@ upconv_fused_kernel(const __grid_constant__ CUtensorMap map_a_hi,
           named_bar_sync(kBarPair + q, 64);          // the slot is free for the next step
         }
         if constexpr (PROF) tq[2] = clock64();
-        if (p.debug_p != nullptr && img_ok && y < p.H && y >= it.y_emit - 1) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            float* dp = p.debug_p + ((static_cast<size_t>(b) * p.H + y) * W + x0 + j) * 9 * p.Cout + c0;
-#pragma unroll
-            for (int t = 0; t < 9; ++t) *reinterpret_cast<float2*>(dp + t * p.Cout) = P[t][j];
-          }
-        }
 
         // t rows E = 2y, O = 2y+1 in pixel-local pieces (see the header comment):
         //   E.e[x] = leE[x] + rE[x-1], E.o[x] = oE[x];   O.e[x] = leO[x] + rO[x-1], O.o[x] = oO[x]
@@ -550,8 +542,7 @@ upconv_fused_kernel(const __grid_constant__ CUtensorMap map_a_hi,
             if constexpr (PROF) te[3] = clock64();
             // warp (q, h) issues plane h's store.  (Two dedicated store warps instead, fed through
             // arrive/sync barrier pairs, were slower: 922 vs 830 us at layer 13.)
-            if (lane == 0 && (!PROF || p.debug_nostore == 0))
-              tma_store_5d(omap, my_slot, it.cg * UNC, o_xg, 0, Y, b0 + o_img);
+            if (lane == 0) tma_store_5d(omap, my_slot, it.cg * UNC, o_xg, 0, Y, b0 + o_img);
             if constexpr (PROF) {
               te[4] = clock64();
 #pragma unroll

@@ -78,7 +78,6 @@ def wide_insert_work(B, Cin, h, w):
     warps idle and takes as long as at 256.  A CTA owns 4 output channels and there is at most one
     CTA per SM, so up to Cout = 512 the time does not depend on Cout."""
     return max(Cin, 256) * B * h * (-(-w // 16) * 16)
-    return None
 
 
 def fused_insert_up_kernel(B, Cin, Cout, h, w, linear=False):

@@ -25,6 +25,7 @@ def test_cabi_loads_and_exports_every_declared_symbol():
     for name in sorted(declared):
         assert hasattr(lib, name), 'missing export ' + name
         assert name in _cabi.SIGNATURES, 'no ctypes prototype for ' + name
+    assert set(_cabi.SIGNATURES) == declared, sorted(set(_cabi.SIGNATURES) ^ declared)
     assert lib.rw_gram_workspace_bytes(512, 512, 10890, 1) > 0
 
 
