@@ -38,6 +38,7 @@ import torch
 import torch.nn.functional as F
 
 from oracle import sg2_oracle as orc
+from oracle.exact_operands import bf16_split, bits_equal, key64, three, wfwd64, wupf64
 from test_gpu_conv_tc_tiles import _guard_intact, _guarded
 from test_gpu_persistent_paths import _gram_splits, _nan_workspace, _planes, _shift_rows
 
@@ -77,14 +78,6 @@ def _operands(kind, shape_a, shape_w, seed):
     a = torch.randn(shape_a, device='cuda', generator=g)
     w = torch.randn(shape_w, device='cuda', generator=g)
     return (a.relu() if kind == 'relu' else a), w
-
-
-def _three(f, a, w):
-    """float64 (ref, scale) of the kernel's three products, from (hi, lo) float64 pairs."""
-    (ah, al), (wh, wl) = a, w
-    ref = f(ah, wh) + f(al, wh) + f(ah, wl)
-    scale = f((ah + al).abs(), (wh + wl).abs())
-    return ref, scale
 
 
 def _stats(got, ref, scale):
@@ -178,15 +171,6 @@ def _conv_chunks(K):
 
 
 # ================================================================== 1. the planes, bit for bit
-def _bf16_split(v):
-    hi = v.to(torch.bfloat16)
-    return hi, (v - hi.float()).to(torch.bfloat16)
-
-
-def _bits_equal(a, b):
-    return torch.equal(a.contiguous().view(torch.int16), b.contiguous().view(torch.int16))
-
-
 # (kind, transpose_io, flip_taps)
 LAYOUTS = {'fwd': (0, 0), 'upf': (2, 0), 'dgrad': (1, 1), 'dgrad_up': (1, 0)}
 
@@ -226,11 +210,11 @@ def test_prep_weights_layouts_bit_exact(shape, kind):
     torch.cuda.synchronize()
     assert _guard_intact(hbuf) and _guard_intact(lbuf) and _guard_intact(sbuf)
     v = w.view(Cout, Cin, 9) * torch.tensor(scale, dtype=torch.float32, device='cuda')
-    ehi, elo = _bf16_split(v)
-    assert _bits_equal(hi, _layout(ehi, kind, Cout, Cin)), 'hi'
-    assert _bits_equal(lo, _layout(elo, kind, Cout, Cin)), 'lo'
+    ehi, elo = bf16_split(v)
+    assert bits_equal(hi, _layout(ehi, kind, Cout, Cin)), 'hi'
+    assert bits_equal(lo, _layout(elo, kind, Cout, Cin)), 'lo'
     ohi, olo, owsq = ops.weight_planes(w, kind, scale)
-    assert _bits_equal(ohi, hi) and _bits_equal(olo, lo)
+    assert bits_equal(ohi, hi) and bits_equal(olo, lo)
     if kind == 'fwd':
         ss = torch.zeros(Cout, Cin, dtype=torch.float32, device='cuda')
         for t in range(9):        # ss = fma(v, v, ss): the product is exact in float64
@@ -267,32 +251,18 @@ def test_split_rows_tails_bit_exact(n):
     _cabi.call('rw_split_rows', _p(a), n, _p(hi), _p(lo), _stream())
     torch.cuda.synchronize()
     assert _guard_intact(hbuf) and _guard_intact(lbuf)
-    ehi, elo = _bf16_split(a)
-    assert _bits_equal(hi, ehi) and _bits_equal(lo, elo)
+    ehi, elo = bf16_split(a)
+    assert bits_equal(hi, ehi) and bits_equal(lo, elo)
     ohi, olo = ops.split_rows(a)
-    assert _bits_equal(ohi, hi) and _bits_equal(olo, lo)
+    assert bits_equal(ohi, hi) and bits_equal(olo, lo)
 
 
 # ================================================================== 2. conv_tc
-def _key64(planes):
-    """(hi, lo) of padded-flat key planes as float64 NCHW."""
-    B, C, H, W = planes.B, planes.C, planes.H, planes.W
-
-    def v(t):
-        return t.view(B, H + 1, W + 1, C)[:, :H, :W].permute(0, 3, 1, 2).double()
-    return v(planes.hi), v(planes.lo)
-
-
 def _pad_rows_zero(planes):
     B, C, H, W = planes.B, planes.C, planes.H, planes.W
     for t in (planes.hi, planes.lo):
         t4 = t.view(B, H + 1, W + 1, C)
         assert t4[:, H].float().abs().max() == 0 and t4[:, :, W].float().abs().max() == 0
-
-
-def _wfwd64(w_hi, w_lo, Cout, Cin):
-    """[Cout][tap][Cin] planes as float64 conv2d weights [Cout, Cin, 3, 3]."""
-    return tuple(t.view(Cout, 3, 3, Cin).permute(0, 3, 1, 2).double() for t in (w_hi, w_lo))
 
 
 def _bn(n):
@@ -319,8 +289,8 @@ def test_modconv_fwd_accumulation(Cin, Cout, kind):
         None, 0, B, Cin, Cout, H, H, _p(out), _stream()))
     assert tiles == {(_bn(Cout), 1)}, tiles
     assert _guard_intact(buf)
-    ref, scale = _three(lambda a, b: F.conv2d(a, b, padding=1), _key64(planes),
-                        _wfwd64(w_hi, w_lo, Cout, Cin))
+    ref, scale = three(lambda a, b: F.conv2d(a, b, padding=1), key64(planes),
+                       wfwd64(w_hi, w_lo, Cout, Cin))
     _check('conv_tc', 'fwd Cin %d Cout %d (%s)' % (Cin, Cout, _conv_chunks(9 * Cin)), kind, out,
            ref, scale, _conv_pred(9 * Cin))
 
@@ -342,8 +312,8 @@ def test_conv3x3_dgrad_accumulation(N, kind):
         None, 0, B, Cout, N, H, H, _p(out), _stream()))
     assert tiles == {(_bn(N), 1)}, tiles
     assert _guard_intact(buf)
-    ref, scale = _three(lambda a, b: F.conv2d(a, b, padding=1), _key64(planes),
-                        _wfwd64(wd_hi, wd_lo, N, Cout))
+    ref, scale = three(lambda a, b: F.conv2d(a, b, padding=1), key64(planes),
+                       wfwd64(wd_hi, wd_lo, N, Cout))
     _check('conv_tc', 'dgrad N %d (%s)' % (N, _conv_chunks(9 * Cout)), kind, out, ref, scale,
            _conv_pred(9 * Cout))
 
@@ -364,8 +334,8 @@ def test_modconv_up_fwd_accumulation(Cout, kind):
         H, H, _p(out), _stream()))
     assert tiles == {(_bn(Cout), 1)}, tiles
     assert _guard_intact(buf)
-    wt = tuple(t.permute(1, 0, 2, 3) for t in _wfwd64(w_hi, w_lo, Cout, Cin))
-    ref, scale = _three(lambda a, b: F.conv_transpose2d(a, b, stride=2), _key64(planes), wt)
+    wt = tuple(t.permute(1, 0, 2, 3) for t in wfwd64(w_hi, w_lo, Cout, Cin))
+    ref, scale = three(lambda a, b: F.conv_transpose2d(a, b, stride=2), key64(planes), wt)
     for a in range(2):
         for b in range(2):
             taps = (2 - a) * (2 - b)
@@ -403,7 +373,7 @@ def test_modconv_up_dgrad_accumulation(N, kind):
                 g[:, :, a::2, b::2] = ph[:, :H + 1 - a, :H + 1 - b, 2 * a + b].permute(0, 3, 1, 2).double()
         return g
     wc = tuple(t.view(N, 3, 3, Cout).permute(0, 3, 1, 2).double() for t in (wd_hi, wd_lo))
-    ref, scale = _three(lambda a, b: F.conv2d(a, b, stride=2), (gt64(gph_hi), gt64(gph_lo)), wc)
+    ref, scale = three(lambda a, b: F.conv2d(a, b, stride=2), (gt64(gph_hi), gt64(gph_lo)), wc)
     _check('conv_tc', 'up_dgrad N %d (%s)' % (N, _conv_chunks(9 * Cout)), kind, out, ref, scale,
            _conv_pred(9 * Cout))
 
@@ -422,8 +392,8 @@ def test_rowgemm_accumulation(K, kind):
                                          K, N, _p(out), _stream()))
     assert tiles == {(128, 1)}, tiles
     assert _guard_intact(buf)
-    ref, scale = _three(lambda x, y: x @ y.t(), (a_hi.double(), a_lo.double()),
-                        (w_hi.double(), w_lo.double()))
+    ref, scale = three(lambda x, y: x @ y.t(), (a_hi.double(), a_lo.double()),
+                       (w_hi.double(), w_lo.double()))
     _check('conv_tc', 'rowgemm K %d (%s)' % (K, _conv_chunks(K)), kind, out, ref, scale,
            _conv_pred(K))
 
@@ -447,8 +417,8 @@ def test_conv3x3_bias_act_accumulation(Cout, kind):
         Cin, Cout, H, H, _p(out), _stream()))
     assert tiles == {(_bn(Cout), 0)}, tiles
     assert _guard_intact(buf)
-    ref, scale = _three(lambda a, b: F.conv2d(a, b, padding=1), _key64(planes),
-                        _wfwd64(w_hi, w_lo, Cout, Cin))
+    ref, scale = three(lambda a, b: F.conv2d(a, b, padding=1), key64(planes),
+                       wfwd64(w_hi, w_lo, Cout, Cin))
     if kind == 'pos':
         assert bool((ref > 0).all())
     ref = F.leaky_relu(ref, 0.2)
@@ -489,8 +459,8 @@ def test_second_moment_accumulation(C, rows, kind):
     assert tiles == {(str(T), str(T))}, tiles
     assert _guard_intact(buf)
     assert torch.equal(mom2, mom2.t())
-    ref, scale = _three(lambda x, y: x.t() @ y, (hi.double(), lo.double()),
-                        (hi.double(), lo.double()))
+    ref, scale = three(lambda x, y: x.t() @ y, (hi.double(), lo.double()),
+                       (hi.double(), lo.double()))
     mt = C // T
     pred = _gram_pred(n, mt * (mt + 1) // 2, 1)
     splits = _gram_splits(mt * (mt + 1) // 2, n, 1)[0]
@@ -550,7 +520,7 @@ def test_wgrad_accumulation(up, kind):
                 s = (u - 1) * Wp + (v - 1)
                 A = (gh.double(), gl.double())
                 Bt = tuple(_shift_rows(p, s) for p in K)
-            ref[:, t], scale[:, t] = _three(lambda x, y: x.t() @ y, A, Bt)
+            ref[:, t], scale[:, t] = three(lambda x, y: x.t() @ y, A, Bt)
     name = '%s rows %d (%d splits)' % (entry[3:], rows, _gram_splits(1, rows, 9)[0])
     _check('gram_tc', name, kind, out, ref, scale, _gram_pred(rows, 1, 9))
 
@@ -576,10 +546,8 @@ def test_modconv_up_fused_y_accumulation(Cin, kind):
         r'upconv_fused_kernel<(\w+),\s*(\w+)>')
     assert found == {('false', 'true')}, found
     assert _guard_intact(buf)
-    # [Cout/16][half][tap][8][Cin] -> conv_transpose2d weights [Cin, Cout, 3, 3]
-    wt = tuple(t.view(Cout // 16, 2, 9, 8, Cin).permute(0, 1, 3, 2, 4).reshape(Cout, 3, 3, Cin)
-               .permute(3, 0, 1, 2).double() for t in (u_hi, u_lo))
-    t, tscale = _three(lambda a, b: F.conv_transpose2d(a, b, stride=2), _key64(planes), wt)
+    wt = wupf64(u_hi, u_lo, Cout, Cin)
+    t, tscale = three(lambda a, b: F.conv_transpose2d(a, b, stride=2), key64(planes), wt)
     k64 = kern.double()
     ref = orc.upfirdn2d(t, k64, pad=(1, 1))
     scale = orc.upfirdn2d(tscale, k64.abs(), pad=(1, 1))
