@@ -23,6 +23,8 @@
  *       utils/stylegan2/models.py:275-281,535-546,622-626                  -> rw_blur_up_act
  *   NoiseInjectionF.forward  utils/stylegan2/models.py:539-546             -> rw_add_noise
  *   ToRGBF.forward           utils/stylegan2/models.py:639-655             -> rw_torgb
+ *   autograd of the ToRGB modulated 1x1 conv (torch.einsum)                -> rw_torgb,
+ *                                                                              rw_torgb_mod_bwd
  *   autograd of the conv (dgrad / wgrad)                                    -> rw_modconv_fwd on
  *                                                                              gradient planes,
  *                                                                              rw_conv_wgrad
@@ -181,6 +183,17 @@ int rw_add_noise(const float* x, const float* noise, long long noise_bstride,
 int rw_torgb(const float* x, const float* style, const float* w, const float* bias,
              const float* skip, int B, int C, int H, int W, float scale, float* out,
              rw_stream_t stream);
+/* Backward of rw_torgb with no bias and no skip (the modulated 1x1 conv to 3 channels,
+ * y[b,o,p] = sum_i scale w[o,i] style[b,i] x[b,i,p]; x [B,C,H,W], w [3,C], gy [B,3,H,W]):
+ *   gx[b,i,p] = scale style[b,i] sum_o w[o,i] gy[b,o,p]     R[b,o,i] = sum_p gy[b,o,p] x[b,i,p]
+ *   gw[o,i]   = scale sum_b style[b,i] R[b,o,i]             gs[b,i]  = scale sum_o w[o,i] R[b,o,i]
+ * Three launches: one pass over x / gy writing gx and per-chunk partial sums of R into
+ * `workspace` (at least rw_torgb_mod_bwd_workspace_bytes bytes; 0 means the shape is refused),
+ * then fixed-order sums.  Any of gx / gs / gw may be NULL, not all three. */
+size_t rw_torgb_mod_bwd_workspace_bytes(int B, int C, int H, int W);
+int rw_torgb_mod_bwd(const float* x, const float* style, const float* w, const float* gy, int B,
+                     int C, int H, int W, float scale, float* gx, float* gs, float* gw,
+                     void* workspace, size_t workspace_bytes, rw_stream_t stream);
 
 /* ---- operator-level ops of the reference ---- */
 int rw_fused_bias_act(const float* x, const float* bias, const float* ref, int act, int grad,

@@ -115,6 +115,9 @@ SIGNATURES = {
                                c_int, c_p, c_p]),
     'rw_add_noise': (c_int, [c_p, c_p, c_ll, c_p, c_int, c_int, c_int, c_p, c_p]),
     'rw_torgb': (c_int, [c_p, c_p, c_p, c_p, c_p, c_int, c_int, c_int, c_int, c_f, c_p, c_p]),
+    'rw_torgb_mod_bwd_workspace_bytes': (c_sz, [c_int, c_int, c_int, c_int]),
+    'rw_torgb_mod_bwd': (c_int, [c_p, c_p, c_p, c_p, c_int, c_int, c_int, c_int, c_f, c_p, c_p, c_p,
+                                 c_p, c_sz, c_p]),
     'rw_fused_bias_act': (c_int, [c_p, c_p, c_p, c_int, c_int, c_f, c_f, c_ll, c_int, c_int,
                                   c_p, c_p]),
     'rw_upfirdn2d': (c_int, [c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
@@ -184,6 +187,7 @@ def check(rc, what):
 LAUNCHES_PER_CALL = {
     'rw_second_moment_accum': 2, 'rw_conv_wgrad': 2, 'rw_conv_up_wgrad': 2,
     'rw_narrow_conv3x3_wgrad': 2, 'rw_torgb1x1_wgrad': 2,
+    'rw_torgb_mod_bwd': 3,
 }
 launch_count = 0
 

@@ -781,6 +781,21 @@ int rw_torgb(const float* x, const float* style, const float* w, const float* bi
   return torgb_launch(x, style, w, bias, skip, B, C, H, W, scale, out, stream);
 }
 
+size_t rw_torgb_mod_bwd_workspace_bytes(int B, int C, int H, int W) {
+  return torgb_mod_bwd_workspace_bytes(B, C, H, W);
+}
+
+int rw_torgb_mod_bwd(const float* x, const float* style, const float* w, const float* gy, int B,
+                     int C, int H, int W, float scale, float* gx, float* gs, float* gw,
+                     void* workspace, size_t workspace_bytes, rw_stream_t stream) {
+  if (!x || !style || !w || !gy || !workspace || (!gx && !gs && !gw)) {
+    set_last_error("rw_torgb_mod_bwd: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  return torgb_mod_bwd_launch(x, style, w, gy, B, C, H, W, scale, gx, gs, gw, workspace,
+                              workspace_bytes, stream);
+}
+
 int rw_fused_bias_act(const float* x, const float* bias, const float* ref, int act, int grad,
                       float alpha, float scale, long long n, int step_b, int size_b, float* y,
                       rw_stream_t stream) {

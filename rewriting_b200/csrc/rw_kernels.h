@@ -170,6 +170,12 @@ int torgb_launch(const float* x, const float* style, const float* w, const float
 int add_noise_launch(const float* x, const float* noise, long long noise_bstride, const float* noise_w,
                      int B, int C, int HW, float* y, cudaStream_t stream);
 
+// backward of the generator's modulated ToRGB (gen_bwd.cu)
+size_t torgb_mod_bwd_workspace_bytes(int B, int C, int H, int W);
+int torgb_mod_bwd_launch(const float* x, const float* style, const float* w, const float* gy, int B,
+                         int C, int H, int W, float scale, float* gx, float* gs, float* gw,
+                         void* workspace, size_t workspace_bytes, cudaStream_t stream);
+
 // StyledConv backward, HBM-bound passes (bwd.cu)
 int act_grad_reduce_launch(const float* gy, const float* y, const float* noise,
                            long long noise_bstride, const float* noise_w, const float* bias,

@@ -863,6 +863,44 @@ class ToRGBFunction(torch.autograd.Function):
         return gx, gW
 
 
+# --------------------------------------------------------------------------- StyleGAN2 ToRGB
+class ModulatedToRGBFunction(torch.autograd.Function):
+    """The ToRGB modulated 1x1 conv, y[b,o] = sum_i (W[o,i] / sqrt(C)) s[b,i] x[b,i], on `rw_torgb`
+    with a zero bias and no skip (ToRGBF adds those in torch); gx, gs and gW on
+    `rw_torgb_mod_bwd`."""
+
+    @staticmethod
+    def forward(ctx, x, style, weight):
+        x = _f32c(x)
+        style = _f32c(style)
+        zero = torch.zeros(3, dtype=torch.float32, device=x.device)
+        out = torgb(x, style, weight.detach(), zero)
+        ctx.save_for_backward(x, style, weight)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gy):
+        x, style, weight = ctx.saved_tensors
+        need_x, need_s, need_w = ctx.needs_input_grad[:3]
+        B, C, H, W = x.shape
+        dev = x.device
+        gx = torch.empty_like(x) if need_x else None
+        gs = torch.empty_like(style) if need_s else None
+        gW = torch.empty(weight.shape, dtype=torch.float32, device=dev) if need_w else None
+        if gx is not None or gs is not None or gW is not None:
+            lib = _cabi.load()
+            ws = _workspace(lib.rw_torgb_mod_bwd_workspace_bytes(B, C, H, W), dev)
+            _cabi.call('rw_torgb_mod_bwd', _p(x), _p(style), _p(_f32c(weight.detach().reshape(3, C))),
+                       _p(_f32c(gy)), B, C, H, W, 1.0 / math.sqrt(C), _p(gx), _p(gs), _p(gW), _p(ws),
+                       ws.numel() * 4, _stream())
+        return gx, gs, gW
+
+
+def modulated_torgb(x, style, weight):
+    return ModulatedToRGBFunction.apply(x, style, weight)
+
+
 # --------------------------------------------------------------------------- key algebra
 def rowgemm(a, w_planes):
     """a [M, K] fp32 (CUDA) times W^T for W [N, K] given as (hi, lo) planes from split_rows:

@@ -399,14 +399,11 @@ class ModulatedConv2d(nn.Module):
                                    blur_kernel=self.blur.kernel if self.upsample else None,
                                    demodulate=self.demodulate, with_noise=False, with_act=False)
         if self.kernel_size == 1 and not self.demodulate and not self.upsample:
-            # generic 1x1 (ToRGBF.forward calls the same kernel with its bias and skip)
-            needs_grad = torch.is_grad_enabled() and (
-                input.requires_grad or s.requires_grad or self.weight.requires_grad)
-            if self.out_channel == 3 and input.is_cuda and not needs_grad:
-                zero = torch.zeros(3, dtype=torch.float32, device=input.device)
-                return ops.torgb(input, s, self.weight.detach(), zero)
-            # differentiable / non-RGB widths: plain torch (off the rewrite path; nothing in the
-            # generator builds such a layer)
+            # ToRGB's 1x1 (ToRGBF.forward's no-grad branch calls the same kernel with its bias and
+            # skip), with or without autograd
+            if self.out_channel == 3 and input.is_cuda and input.dtype == torch.float32:
+                return ops.modulated_torgb(input, s, self.weight)
+            # CPU / non-RGB widths: plain torch (nothing in the generator builds a non-RGB layer)
             w = (self.scale * self.weight[0, :, :, 0, 0])[None] * s[:, None, :]
             return torch.einsum('boi,bihw->bohw', w, input)
         raise NotImplementedError('ModulatedConv2d kernel_size=%d demodulate=%s' % (
