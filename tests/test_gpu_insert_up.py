@@ -25,6 +25,7 @@ import pytest
 import torch
 
 from oracle import sg2_oracle as orc
+from oracle import trajectory_check as tc
 from conftest import GOLD
 
 pytestmark = pytest.mark.gpu
@@ -126,15 +127,23 @@ def _key(gin, premod):
 
 
 def _oracle(gw, layer, gin, gout, d, niter, lr, premod=False, linear=False, **kw):
+    """(W0, the oracle's W, the float64 shadow's record of the same loop)."""
     sd = {k: v.cpu() for k, v in gw.model.state_dict().items()}
-    fn = _target_fn(sd, layer, _key(gin, premod), gin.style)
+    k = _key(gin, premod)
+    fn = _target_fn(sd, layer, k, gin.style)
     W0 = gw.target_weights().detach().clone().cpu()
     if linear:
         W = _linear_insert_loop(W0, gout.fmap.cpu(), d, niter, lr, fn)
     else:
         W = orc.insert_loop(W0, None, None, gout.fmap.cpu(), None, None, d, niter, piter=10, lr=lr,
                             target_fn=fn, **kw)
-    return W0, W
+    p = orc._layer_params(sd, 'layer%d' % layer)
+    B, _, h, w = k.shape
+    rec = tc.shadow('up', W0, k, gin.style, gout.fmap, d, niter, lr, linear=linear,
+                    low_rank_gradient=kw.get('low_rank_gradient', False),
+                    noise=orc.noise_table(B, 4 * h * w), noise_w=p['noise_w'], bias=p['bias'],
+                    blur=sd['layer%d.sconv.mconv.blur.kernel' % layer])
+    return W0, W, rec
 
 
 def _run(gw, gin, gout, d, niter, lr, losses=None):
@@ -270,8 +279,8 @@ def test_tight_crops_at_every_odd_layer_vs_oracle(cuda_model, zds, layer, ys, xs
     d = _direction(1, cin=gin.fmap.shape[1])
     assert gw._fused_up_plan(gin, gout, d.cuda())[0] == UP
     W = _run(gw, gin, gout, d.cuda(), NITER, 0.05)
-    W0, W_orc = _oracle(gw, layer, gin, gout, d, NITER, 0.05)
-    assert (W.cpu() - W_orc).abs().max().item() < 1e-4, layer
+    W0, W_orc, rec = _oracle(gw, layer, gin, gout, d, NITER, 0.05)
+    tc.check_rows(W, W_orc, rec, what='layer %d' % layer)
     assert (W_orc - W0).abs().max().item() > 1e-3, layer
 
 
@@ -291,11 +300,11 @@ def test_tight_crop_layer9_other_blur_kernels_vs_oracle(cuda_model, zds, blur):
         plan = gw._fused_up_plan(gin, gout, d.cuda())
         assert plan[0] == UP and torch.equal(torch.tensor(plan[-1]), orc.blur_case(blur).reshape(16))
         W = _run(gw, gin, gout, d.cuda(), NITER, 0.05)
-        W0, W_orc = _oracle(gw, 9, gin, gout, d, NITER, 0.05)
+        W0, W_orc, rec = _oracle(gw, 9, gin, gout, d, NITER, 0.05)
     finally:
         with torch.no_grad():
             kbuf.copy_(saved)
-    assert (W.cpu() - W_orc).abs().max().item() < 1e-4
+    tc.check_rows(W, W_orc, rec)
     assert (W_orc - W0).abs().max().item() > 1e-3
 
 
@@ -306,8 +315,8 @@ def test_rank2_layer9_vs_oracle(cuda_model, zds, lrg):
     d = _direction(2)
     assert gw._fused_up_plan(gin, gout, d.cuda())[0] == UP
     W = _run(gw, gin, gout, d.cuda(), NITER, 0.05)
-    _, W_orc = _oracle(gw, 9, gin, gout, d, NITER, 0.05, low_rank_gradient=lrg)
-    assert (W.cpu() - W_orc).abs().max().item() < 1e-4
+    _, W_orc, rec = _oracle(gw, 9, gin, gout, d, NITER, 0.05, low_rank_gradient=lrg)
+    tc.check_rows(W, W_orc, rec)
 
 
 def test_batch_of_two_crops_layer9_vs_oracle(cuda_model, zds):
@@ -317,23 +326,24 @@ def test_batch_of_two_crops_layer9_vs_oracle(cuda_model, zds):
     d = _direction(1)
     assert gw._fused_up_plan(gin, gout, d.cuda())[0] == UP
     W = _run(gw, gin, gout, d.cuda(), NITER, 0.01)
-    _, W_orc = _oracle(gw, 9, gin, gout, d, NITER, 0.01)
-    assert (W.cpu() - W_orc).abs().max().item() < 1e-4
+    _, W_orc, rec = _oracle(gw, 9, gin, gout, d, NITER, 0.01)
+    tc.check_rows(W, W_orc, rec)
 
 
 def test_seqpre_odd_target_vs_oracle(cuda_model, zds):
-    """the crop of the layer-9 tight-crop case, on the un-modulated key.  (Image 4's crop
-    [3:9, 20:27] is not used: one of its outputs, channel 145, sits within 1e-5 of the leaky-ReLU
-    kink, so that channel's first Adam step differs between any two fp32 loops, by 9e-4 here, on
-    this target and on SeqStyleGanRewriter's alike; DESIGN.md §4.)"""
+    """the crop of the layer-9 tight-crop case, and image 4's crop [3:9, 20:27], on the
+    un-modulated key.  One output of channel 145 of the latter sits within 1e-5 of the leaky-ReLU
+    kink, so that channel's first Adam step may differ between two fp32 loops (by 9e-4, DESIGN.md
+    §4): the row criterion excuses that row only because the float64 shadow sees the kink."""
     gw = _rewriter(cuda_model, zds, 9, cls='SeqPreStyleGanRewriter')
     assert gw.firstlayer == 'layer9.sconv.mconv.adain'
-    gin, gout = _crop_goal(gw, [0], slice(8, 14), slice(10, 15))
     d = _direction(1)
-    assert gw._fused_up_plan(gin, gout, d.cuda())[0] == UP
-    W = _run(gw, gin, gout, d.cuda(), NITER, 0.05)
-    _, W_orc = _oracle(gw, 9, gin, gout, d, NITER, 0.05, premod=True)
-    assert (W.cpu() - W_orc).abs().max().item() < 1e-4
+    for img, ys, xs in ((0, slice(8, 14), slice(10, 15)), (4, slice(3, 9), slice(20, 27))):
+        gin, gout = _crop_goal(gw, [img], ys, xs)
+        assert gw._fused_up_plan(gin, gout, d.cuda())[0] == UP
+        W = _run(gw, gin, gout, d.cuda(), NITER, 0.05)
+        _, W_orc, rec = _oracle(gw, 9, gin, gout, d, NITER, 0.05, premod=True)
+        tc.check_rows(W, W_orc, rec, what='image %d' % img)
 
 
 def test_whole_layer7_map_vs_oracle(cuda_model, zds):
@@ -342,8 +352,8 @@ def test_whole_layer7_map_vs_oracle(cuda_model, zds):
     d = _direction(1)
     assert gw._fused_up_plan(gin, gout, d.cuda())[0] == UP
     W = _run(gw, gin, gout, d.cuda(), NITER, 0.01)
-    _, W_orc = _oracle(gw, 7, gin, gout, d, NITER, 0.01)
-    assert (W.cpu() - W_orc).abs().max().item() < 1e-4
+    _, W_orc, rec = _oracle(gw, 7, gin, gout, d, NITER, 0.01)
+    tc.check_rows(W, W_orc, rec)
 
 
 def test_linear_insert_layer9_vs_oracle(cuda_model, zds, monkeypatch):
@@ -354,8 +364,8 @@ def test_linear_insert_layer9_vs_oracle(cuda_model, zds, monkeypatch):
     calls = _spy(monkeypatch)
     W = _run(gw, gin, gout, d.cuda(), NITER, 0.05)
     assert LINEAR_UP in calls and UP not in calls
-    _, W_orc = _oracle(gw, 9, gin, gout, d, NITER, 0.05, linear=True)
-    assert (W.cpu() - W_orc).abs().max().item() < 1e-4
+    _, W_orc, rec = _oracle(gw, 9, gin, gout, d, NITER, 0.05, linear=True)
+    tc.check_rows(W, W_orc, rec)
 
 
 @pytest.mark.parametrize('linear', [False, True])

@@ -9,7 +9,9 @@ test_apply_erase_goal_crops_vs_live_reference_golden).  One such flip moves a we
 lr * 2 / (B*h*w) in Adam's normalised step: 1e-4 at lr 0.05 on a 32 x 32 map, and a whole map has
 10-50x more residuals crossing zero than the crops of test_gpu_parity.  The whole-map, batch and
 20 x 20 cases and the ProgGAN ones therefore run at lr 0.01, where a flip stays well inside the
-bound.
+bound.  Every W is held to the oracle's row by row (oracle/trajectory_check.py): a row may part
+by more than 1e-4 only where the float64 shadow of the loop saw one of that row's sign decisions
+within rounding of zero, and only a few rows may part.
 """
 import copy
 import ctypes
@@ -20,6 +22,7 @@ import torch
 
 from oracle import proggan_oracle as ppo
 from oracle import sg2_oracle as orc
+from oracle import trajectory_check as tc
 
 pytestmark = pytest.mark.gpu
 
@@ -47,14 +50,20 @@ def _crop_goal(gw, imgnum, ys, xs):
 
 
 def _oracle(gw, layer, gin, gout, d, niter, piter, premod=False, lr=0.05, **kw):
+    """(W0, the oracle's W, the float64 shadow's record of the same loop)."""
     sd = gw.model.state_dict()
     st = gin.style.cpu()
     k = st[:, :, None, None] * gin.fmap.cpu() if premod else gin.fmap.cpu()
     W0 = gw.target_weights().detach().clone().cpu()
-    W = orc.insert_loop(W0, k, st, gout.fmap.cpu(), sd[layer + '.sconv.noise.weight'].cpu(),
-                        sd[layer + '.sconv.activate.bias'].cpu(), d, niter, piter=piter, lr=lr,
-                        **kw)
-    return W0, W
+    nw, bias = sd[layer + '.sconv.noise.weight'].cpu(), sd[layer + '.sconv.activate.bias'].cpu()
+    W = orc.insert_loop(W0, k, st, gout.fmap.cpu(), nw, bias, d, niter, piter=piter, lr=lr, **kw)
+    act = kw.get('with_noise_act', True)
+    B, _, h, w = k.shape
+    rec = tc.shadow('styled', W0, k, st, gout.fmap, d, niter, lr, piter=piter,
+                    low_rank_gradient=kw.get('low_rank_gradient', False),
+                    noise=orc.noise_table(B, h * w) if act else None, noise_w=nw, bias=bias,
+                    act=act)
+    return W0, W, rec
 
 
 def test_whole_map_goal_layer8_rank1(cuda_model, z40, edit_request):
@@ -73,12 +82,12 @@ def test_whole_map_goal_layer8_rank1(cuda_model, z40, edit_request):
     d = _direction(1)
     assert gw._fused_plan(goal_in, gout, d.cuda())[0] == WIDE
     lo = []
-    W0, W_orc = _oracle(gw, 'layer8', goal_in, gout, d, 30, 10, lr=0.01, record_loss=lo)
+    W0, W_orc, rec = _oracle(gw, 'layer8', goal_in, gout, d, 30, 10, lr=0.01, record_loss=lo)
     losses = []
     gw.insert(goal_in, gout, d.cuda(), niter=30, piter=10, lr=0.01,
               update_callback=lambda it, l: losses.append(float(l)))
     W = gw.target_weights().detach().cpu()
-    assert (W - W_orc).abs().max().item() < 1e-4
+    tc.check_rows(W, W_orc, rec)
     assert (W_orc - W0).abs().max().item() > 5e-3
     np.testing.assert_allclose(np.array(losses), np.array(lo), rtol=2e-4)
     s = torch.linalg.svdvals((W - W0)[0].permute(0, 2, 3, 1).reshape(-1, 512).double())
@@ -94,9 +103,9 @@ def test_wide_crop_layer8_rank2(cuda_model, z40, lrg):
     gin, gout = _crop_goal(gw, 2, slice(10, 22), slice(4, 28))
     d = _direction(2, seed=11)
     assert gw._fused_plan(gin, gout, d.cuda())[0] == WIDE
-    W0, W_orc = _oracle(gw, 'layer8', gin, gout, d, 12, 5, low_rank_gradient=lrg)
+    W0, W_orc, rec = _oracle(gw, 'layer8', gin, gout, d, 12, 5, low_rank_gradient=lrg)
     gw.insert(gin, gout, d.cuda(), niter=12, piter=5, lr=0.05)
-    assert (gw.target_weights().detach().cpu() - W_orc).abs().max().item() < 1e-4
+    tc.check_rows(gw.target_weights(), W_orc, rec)
 
 
 def test_batch_of_two_wide_crops_layer8(cuda_model, z40):
@@ -116,12 +125,12 @@ def test_batch_of_two_wide_crops_layer8(cuda_model, z40):
     d = _direction(1)
     assert gw._fused_plan(gin, gout, d.cuda())[0] == WIDE
     lo = []
-    W0, W_orc = _oracle(gw, 'layer8', gin, gout, d, 12, 5, lr=0.01, record_loss=lo)
+    W0, W_orc, rec = _oracle(gw, 'layer8', gin, gout, d, 12, 5, lr=0.01, record_loss=lo)
     losses = []
     gw.insert(gin, gout, d.cuda(), niter=12, piter=5, lr=0.01,
               update_callback=lambda it, l: losses.append(float(l)))
     W = gw.target_weights().detach().cpu()
-    assert (W - W_orc).abs().max().item() < 1e-4
+    tc.check_rows(W, W_orc, rec)
     assert (W_orc - W0).abs().max().item() > 1e-3
     np.testing.assert_allclose(np.array(losses), np.array(lo), rtol=2e-4)
 
@@ -134,16 +143,16 @@ def test_seqtiny_and_seqpre_targets_on_wide_keys(cuda_model, z40):
     gw = ganrewrite.SeqTinyStyleGanRewriter(cuda_model, zds, 8)
     gin, gout = _crop_goal(gw, 1, slice(3, 13), slice(0, 32))
     assert gw._fused_plan(gin, gout, d.cuda())[0] == WIDE
-    W0, W_orc = _oracle(gw, 'layer8', gin, gout, d, 12, 5, with_noise_act=False)
+    W0, W_orc, rec = _oracle(gw, 'layer8', gin, gout, d, 12, 5, with_noise_act=False)
     gw.insert(gin, gout, d.cuda(), niter=12, piter=5, lr=0.05)
-    assert (gw.target_weights().detach().cpu() - W_orc).abs().max().item() < 1e-4
+    tc.check_rows(gw.target_weights(), W_orc, rec, what='SeqTiny')
     # SeqPre: the key is the un-modulated feature map, the target starts at `adain`
     gp = ganrewrite.SeqPreStyleGanRewriter(cuda_model, zds, 8)
     gin, gout = _crop_goal(gp, 4, slice(6, 26), slice(5, 25))
     assert gp._fused_plan(gin, gout, d.cuda())[0] == WIDE
-    W0, W_orc = _oracle(gp, 'layer8', gin, gout, d, 12, 5, premod=True, lr=0.01)
+    W0, W_orc, rec = _oracle(gp, 'layer8', gin, gout, d, 12, 5, premod=True, lr=0.01)
     gp.insert(gin, gout, d.cuda(), niter=12, piter=5, lr=0.01)
-    assert (gp.target_weights().detach().cpu() - W_orc).abs().max().item() < 1e-4
+    tc.check_rows(gp.target_weights(), W_orc, rec, what='SeqPre')
 
 
 def test_whole_map_layer10(cuda_model, z40):
@@ -160,9 +169,9 @@ def test_whole_map_layer10(cuda_model, z40):
         assert plan is None
         return
     assert plan[0] == WIDE
-    W0, W_orc = _oracle(gw, 'layer10', gin, gout, d, 3, 10)
+    W0, W_orc, rec = _oracle(gw, 'layer10', gin, gout, d, 3, 10)
     gw.insert(gin, gout, d.cuda(), niter=3, piter=10, lr=0.05)
-    assert (gw.target_weights().detach().cpu() - W_orc).abs().max().item() < 1e-4
+    tc.check_rows(gw.target_weights(), W_orc, rec)
 
 
 def test_proggan_plain_conv_on_wide_keys():
@@ -185,9 +194,10 @@ def test_proggan_plain_conv_on_wide_keys():
         assert gw._fused_plan(k, tgt, d.cuda())[0] == WIDE, layer
         W0 = gw.target_weights().detach().clone().cpu()
         W_orc = ppo.insert_loop(W0, k.cpu(), tgt.cpu(), d, 12, piter=5, lr=0.01)
+        rec = tc.shadow('plain', W0, k, None, tgt, d, 12, 0.01, piter=5, act=False)
         gw.insert(k, tgt, d.cuda(), niter=12, piter=5, lr=0.01)
         W = gw.target_weights().detach().cpu()
-        assert (W - W_orc).abs().max().item() < 1e-4, layer
+        tc.check_rows(W, W_orc, rec, what='layer %d' % layer)
         assert (W_orc - W0).abs().max().item() > 1e-3, layer
 
 

@@ -12,6 +12,7 @@ import torch
 import torch.nn.functional as F
 
 from oracle import sg2_oracle as orc
+from oracle import trajectory_check as tc
 
 pytestmark = pytest.mark.gpu
 
@@ -282,9 +283,13 @@ def test_generation_fast_path_equals_layer_path(cuda_model, z40):
     assert (hooked - slow).abs().max().item() < 1e-4
 
 
-def test_fused_layers_equal_leaf_by_leaf_execution(cuda_model, z40):
+KEY8_BOUND = 1.3e-5         # layer-8 key vs float64, per max|key|: 1.6x 8.33e-6 (H100, 700 W)
+
+
+def test_fused_layers_equal_leaf_by_leaf_execution(cuda_model, z40, seeded_sd):
     """The nethook-split execution (context | target | rendering, leaves one by one) must give
-    the same image as the fused whole-layer path."""
+    the same image as the fused whole-layer path.  The layer-8 key, captured with and without a
+    hook, is held to float64 of the oracle's context chain from the same z."""
     from rewriting_b200.utils import nethook
     first, last = 'layer8.sconv.mconv.dconv', 'layer8.sconv.activate'
     ctx = nethook.subsequence(cuda_model, upto_layer=first, share_weights=True)
@@ -302,7 +307,16 @@ def test_fused_layers_equal_leaf_by_leaf_execution(cuda_model, z40):
         key = inst.retained_layer('layer8.sconv.mconv.adain')
     assert key.fmap.shape == (3, 512, 32, 32)
     assert (hooked - whole).abs().max().item() < 2e-4
-    assert torch.allclose(key.fmap, ctx(z).fmap, atol=1e-5)
+    sd64 = {k: v.cuda().double() for k, v in seeded_sd.items()}
+    with torch.no_grad():
+        want = orc.generator_forward(sd64, z.double(), upto_key_layer=8)
+        plain = ctx(z).fmap
+    scale = want.abs().max().item()
+    errs = [((got.double() - want).abs().max().item() / scale) for got in (key.fmap, plain)]
+    print('layer-8 key vs float64 / max|key|: hooked %.3g, no-grad %.3g' % tuple(errs))
+    assert max(errs) < KEY8_BOUND, errs
+    # the two captures, each within KEY8_BOUND of float64, are within twice that of each other
+    assert (key.fmap - plain).abs().max().item() < 2 * KEY8_BOUND * scale
 
 
 def test_rewriter_statistics_direction_and_edit_vs_golden(cuda_model, z40, golden, edit_request,
@@ -434,7 +448,9 @@ def test_insert_variants_rank2_gradient_projection_and_tiny_target(cuda_model, z
         W = gw.target_weights().detach().cpu()
         W_orc = orc.insert_loop(W0, k, st, tgt, nw, bias, d2, 12, piter=5, lr=0.05,
                                 low_rank_gradient=lrg)
-        assert (W - W_orc).abs().max().item() < 1e-4, lrg
+        rec = tc.shadow('styled', W0, k, st, tgt, d2, 12, 0.05, piter=5, low_rank_gradient=lrg,
+                        noise=orc.noise_table(1, k.shape[2] * k.shape[3]), noise_w=nw, bias=bias)
+        tc.check_rows(W, W_orc, rec, what='low_rank_gradient=%s' % lrg)
         s = torch.linalg.svdvals((W - W0)[0].permute(0, 2, 3, 1).reshape(-1, 512).double())
         assert float(s[2] / s[0]) < 1e-5                      # rank <= 2
     # SeqTiny: the target model is the dconv leaf alone (no noise / activation)
@@ -445,7 +461,8 @@ def test_insert_variants_rank2_gradient_projection_and_tiny_target(cuda_model, z
     gw.insert(gin, gout, d2[:1].cuda(), niter=12, piter=5, lr=0.05)
     W_orc = orc.insert_loop(W0, k, st, tgt, nw, bias, d2[:1], 12, piter=5, lr=0.05,
                             with_noise_act=False)
-    assert (gw.target_weights().detach().cpu() - W_orc).abs().max().item() < 1e-4
+    rec = tc.shadow('styled', W0, k, st, tgt, d2[:1], 12, 0.05, piter=5, act=False)
+    tc.check_rows(gw.target_weights(), W_orc, rec, what='SeqTiny')
 
 
 def test_zero_linear_insert_and_erase_run_on_the_kernels(cuda_model, z40, golden, edit_request):
