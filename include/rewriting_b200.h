@@ -475,6 +475,52 @@ int rw_masked_l1(const void* im0, const void* im1, int u8, int B, int H, int W, 
                  int mask_b, double* num, double* den, void* workspace, size_t workspace_bytes,
                  rw_stream_t stream);
 
+/* ---- unified-parsing segmenter (ResNet-50 deep stem + UPerNet): the passes between its convs ----
+ * The convolutions run on rw_conv3x3_bias_act (3x3), rw_rowgemm (1x1 on the planes, giving
+ * channels-last padded rows [B*(H+1)*(W+1)][N]) and rw_narrow_conv3x3 (the 3-channel stem).
+ * rw_seg_input: images as for rw_lpips_input (fp32 NCHW in [-1, 1] or uint8 NHWC) to the
+ *   network's input out [B,3,S,S] fp32: (x + 1) / 2 * 255, channels reversed (RGB -> BGR), minus
+ *   the mean (102.9801, 115.9465, 122.7717); when S < H, W the mean over each (H/S) x (W/S) block
+ *   (AdaptiveAvgPool2d with an integer factor; S must divide H and W).
+ * rw_seg_map: v[b,c,y,x] = a sampled at output (y, x) + bias[c] + res[b,c,y,x], then relu when
+ *   relu = 1.  a is fp32 NCHW [B,C,Hin,Win] (a_cl = 0) or channels-last padded rows
+ *   [B*(Hin+1)*(Win+1)][C] (a_cl = 1, the rw_rowgemm output).  mode 0: a at (y, x) (Ho = Hin,
+ *   Wo = Win); mode 1: a at (2y, 2x) (Ho = ceil(Hin/2), Wo = ceil(Win/2): a stride-2 conv computed
+ *   at stride 1); mode 2: bilinear resize to Ho x Wo (torch's align_corners=False, weights in
+ *   float64).  bias, res may be NULL.  Writes fp32 NCHW out [B,C,Ho,Wo] and / or bf16 hi/lo planes
+ *   [B*(Ho+1)*(Wo+1)][ldc] in channels coff..coff+C-1 (zero pad row / column; ldc, coff multiples
+ *   of 64; 16-byte aligned), so a concatenation's planes are written slice by slice.  C % 64 == 0.
+ * rw_seg_maxpool: MaxPool2d(3, stride 2, padding 1): out [B,C,(H-1)/2+1,(W-1)/2+1]; -inf padding,
+ *   the window scanned in row-major order, a strictly greater value or a NaN wins.
+ * rw_seg_prroi: PrRoI pooling of the whole map (ROI [0, 0, W, H], spatial scale 1) into s x s bins:
+ *   out[b,c,i,j] = the integral of the bilinear surface of x (zero outside the map) over bin
+ *   [jW/s, (j+1)W/s] x [iH/s, (i+1)H/s], divided by the bin's area; float64, fixed order.
+ * rw_seg_classes: the class maps at Ho x Wo from the heads' logits.  logits is a host array of
+ *   3 * nsizes device pointers, per segmentation size (object, part, material head), each the
+ *   head's 1x1 output as padded rows [B*(h_s+1)*(w_s+1)][ld[head]] without its bias; map_hw the
+ *   host array {h_0, w_0, ...}; bias a host array of the three heads' device bias vectors.  groups
+ *   is a host array of ngroups (1..128) records {head, first channel, count, owner}: per group,
+ *   at each size, the logits + bias bilinearly up-sampled to Ho x Wo and a softmax over the
+ *   group's channels; the probabilities summed over the sizes.  probs [B,sum of counts,Ho,Wo]
+ *   (groups in order) is written when not NULL.  labels [B,3,Ho,Wo] int64, when not NULL:
+ *   channel 0 the argmax of group 0 (objects), channel 1 the argmax m of group 1 (materials),
+ *   written as m + mat_offset or 0 for m = 0, channel 2 trans[first channel + argmax] of the
+ *   part group g >= 2 whose owner is the pixel's object, else 0 (trans: device int64, indexed by
+ *   part-head channel).  The argmax is the first maximum.
+ * A null required pointer, a size < 1 or a shape outside these rules returns RW_STATUS_BAD_ARG
+ * before any launch.  No call allocates or synchronises, none uses atomics: two calls give the
+ * same bits, and image b's results do not depend on the other images of the batch. */
+int rw_seg_input(const void* im, int u8, int B, int H, int W, int S, float* out, rw_stream_t stream);
+int rw_seg_map(const float* a, int a_cl, int B, int C, int Hin, int Win, int mode, int Ho, int Wo,
+               const float* bias, const float* res, int relu, void* out_hi, void* out_lo, int ldc,
+               int coff, float* out, rw_stream_t stream);
+int rw_seg_maxpool(const float* x, int B, int C, int H, int W, float* out, rw_stream_t stream);
+int rw_seg_prroi(const float* x, int B, int C, int H, int W, int s, float* out, rw_stream_t stream);
+int rw_seg_classes(int nsizes, const float* const* logits, const int* map_hw, const float* const* bias,
+                   const int* ld, int ngroups, const int* groups, const long long* trans,
+                   long long mat_offset, int B, int Ho, int Wo, float* probs, long long* labels,
+                   rw_stream_t stream);
+
 /* ---- per-phase profiles (tools/prof_upconv.py, tools/prof_conv.py) ---- */
 /* rw_modconv_up_fused instrumented with clock64(): prof_out[grid][8 epilogue warps][16] = cycles in
  * {wait for the MMAs, accumulator exchange, combine + mailbox + barrier, shuffles, edge-lane fix-ups,

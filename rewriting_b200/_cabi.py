@@ -91,6 +91,13 @@ SIGNATURES = {
     'rw_relu_pool': (c_int, [c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p, c_p, c_p]),
     'rw_relu_pool_bwd': (c_int, [c_p, c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p, c_p,
                                  c_p]),
+    'rw_seg_input': (c_int, [c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p]),
+    'rw_seg_map': (c_int, [c_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_p, c_p,
+                           c_int, c_p, c_p, c_int, c_int, c_p, c_p]),
+    'rw_seg_maxpool': (c_int, [c_p, c_int, c_int, c_int, c_int, c_p, c_p]),
+    'rw_seg_prroi': (c_int, [c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p]),
+    'rw_seg_classes': (c_int, [c_int, c_p, c_p, c_p, c_p, c_int, c_p, c_p, c_ll, c_int, c_int,
+                               c_int, c_p, c_p, c_p]),
     'rw_lpips_input': (c_int, [c_p, c_p, c_int, c_int, c_int, c_int, c_p, c_p]),
     'rw_lpips_head': (c_int, [c_p, c_p, c_p, c_int, c_int, c_int, c_int, c_p, c_p]),
     'rw_lpips_combine_workspace_bytes': (c_sz, [c_int, c_int, c_int]),

@@ -1091,6 +1091,33 @@ int rw_linear_insert_loop_up(const rw_linear_insert_args* a, const float blur[16
   return linear_insert_up_launch(p, blur, workspace, workspace_bytes, stream);
 }
 
+int rw_seg_input(const void* im, int u8, int B, int H, int W, int S, float* out, rw_stream_t stream) {
+  return seg_input_launch(im, u8, B, H, W, S, out, stream);
+}
+
+int rw_seg_map(const float* a, int a_cl, int B, int C, int Hin, int Win, int mode, int Ho, int Wo,
+               const float* bias, const float* res, int relu, void* out_hi, void* out_lo, int ldc,
+               int coff, float* out, rw_stream_t stream) {
+  return seg_map_launch(a, a_cl, B, C, Hin, Win, mode, Ho, Wo, bias, res, relu, out_hi, out_lo, ldc,
+                        coff, out, stream);
+}
+
+int rw_seg_maxpool(const float* x, int B, int C, int H, int W, float* out, rw_stream_t stream) {
+  return seg_maxpool_launch(x, B, C, H, W, out, stream);
+}
+
+int rw_seg_prroi(const float* x, int B, int C, int H, int W, int s, float* out, rw_stream_t stream) {
+  return seg_prroi_launch(x, B, C, H, W, s, out, stream);
+}
+
+int rw_seg_classes(int nsizes, const float* const* logits, const int* map_hw, const float* const* bias,
+                   const int* ld, int ngroups, const int* groups, const long long* trans,
+                   long long mat_offset, int B, int Ho, int Wo, float* probs, long long* labels,
+                   rw_stream_t stream) {
+  return seg_classes_launch(nsizes, logits, map_hw, bias, ld, ngroups, groups, trans, mat_offset, B,
+                            Ho, Wo, probs, labels, stream);
+}
+
 int rw_rowgemm(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo, int rows, int K,
                int N, float* out, rw_stream_t stream) {
   if (!a_hi || !a_lo || !w_hi || !w_lo || !out || rows < 1 || K % 64 != 0 || N % 64 != 0) {

@@ -288,4 +288,18 @@ int masked_l1_launch(const void* im0, const void* im1, int u8, int B, int H, int
                      int mask_b, double* num, double* den, void* workspace, size_t workspace_bytes,
                      cudaStream_t stream);
 
+// ---------------------------------------------------------------------------
+// unified-parsing segmenter passes (seg.cu)
+// ---------------------------------------------------------------------------
+int seg_input_launch(const void* im, int u8, int B, int H, int W, int S, float* out, cudaStream_t stream);
+int seg_map_launch(const float* a, int a_cl, int B, int C, int Hin, int Win, int mode, int Ho, int Wo,
+                   const float* bias, const float* res, int relu, void* hi, void* lo, int ldc,
+                   int coff, float* out, cudaStream_t stream);
+int seg_maxpool_launch(const float* x, int B, int C, int H, int W, float* out, cudaStream_t stream);
+int seg_prroi_launch(const float* x, int B, int C, int H, int W, int s, float* out, cudaStream_t stream);
+int seg_classes_launch(int nsizes, const float* const* logits, const int* map_hw, const float* const* bias,
+                       const int* ld, int ngroups, const int* groups, const long long* trans,
+                       long long mat_offset, int B, int Ho, int Wo, float* probs, long long* labels,
+                       cudaStream_t stream);
+
 }  // namespace rw
