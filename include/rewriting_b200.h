@@ -521,6 +521,31 @@ int rw_seg_classes(int nsizes, const float* const* logits, const int* map_hw, co
                    long long mat_offset, int B, int Ho, int Wo, float* probs, long long* labels,
                    rw_stream_t stream);
 
+/* ---- dissection: unit / label intersection counts (GAN dissection, utils/quickdissect) ----
+ * Both calls up-sample a layer's activations act [B,U,h,w] fp32 to H x W as torch's grid_sample
+ * with align_corners=True and padding_mode='zeros' does over an axis-affine grid: output (y, x)
+ * reads the source at (y * sy + oy, x * sx + ox) in pixel units (0 the first pixel's centre);
+ * the two taps per axis are weighted linearly and taps outside the map read 0, so the border
+ * fades toward 0.  The value is computed in float64 and rounded once to float.
+ * rw_upsample_bilinear: rows [B*H*W][U] fp32, row (b*H + y)*W + x.
+ * rw_dissect_counts: with the same up-sampled values v (the same bits as the rows above), the
+ *   per-unit levels level [U] fp32 and the label maps labels [B,K,H,W] int64 (0 = no label,
+ *   values in 0..C-1), ADDS to the caller's int64 counters: isect [C,U] the pixels that carry
+ *   label c in at least one of their K channels and have v[u] > level[u]; unit_total [U] the
+ *   pixels with v[u] > level[u]; label_total [C] the pixels carrying label c; count [1] B*H*W.
+ *   Label 0 is never counted; labels outside 1..C-1 are skipped (callers check the range: the
+ *   call cannot report it).  Integer atomics: the counts are exact and independent of launch
+ *   order and of how a sample set is split into batches.
+ * Sizes 1..1024, U <= 65535, K 1..8, C 2..32768, the grid's source coordinates within 2^20;
+ * a null pointer or a shape outside these returns RW_STATUS_BAD_ARG before any launch.  No call
+ * allocates or synchronises. */
+int rw_upsample_bilinear(const float* act, int B, int U, int h, int w, int H, int W, double sy,
+                         double oy, double sx, double ox, float* rows, rw_stream_t stream);
+int rw_dissect_counts(const float* act, const float* level, const long long* labels, int B, int U,
+                      int h, int w, int H, int W, int K, int C, double sy, double oy, double sx,
+                      double ox, long long* isect, long long* unit_total, long long* label_total,
+                      long long* count, rw_stream_t stream);
+
 /* ---- per-phase profiles (tools/prof_upconv.py, tools/prof_conv.py) ---- */
 /* rw_modconv_up_fused instrumented with clock64(): prof_out[grid][8 epilogue warps][16] = cycles in
  * {wait for the MMAs, accumulator exchange, combine + mailbox + barrier, shuffles, edge-lane fix-ups,

@@ -24,15 +24,15 @@ def install_aliases(reference_root=None):
     rewriteapp` gives this package's rewriter and the reference's device-independent UI."""
     import os
     from . import utils as _utils, rewrite as _rewrite
-    from .utils import (imgviz, nethook, pbar, renormalize, runningstats, segmenter, tally, zdataset,
-                        stylegan2)
+    from .utils import (imgviz, nethook, pbar, quickdissect, renormalize, runningstats, segmenter,
+                        tally, upsample, zdataset, stylegan2)
     from .rewrite import ganrewrite
     sys.modules.setdefault('utils', _utils)
     sys.modules.setdefault('rewrite', _rewrite)
     for name, mod in [('imgviz', imgviz), ('nethook', nethook), ('pbar', pbar),
-                      ('renormalize', renormalize),
+                      ('quickdissect', quickdissect), ('renormalize', renormalize),
                       ('runningstats', runningstats), ('segmenter', segmenter), ('tally', tally),
-                      ('zdataset', zdataset),
+                      ('upsample', upsample), ('zdataset', zdataset),
                       ('stylegan2', stylegan2)]:
         sys.modules.setdefault('utils.' + name, mod)
     sys.modules.setdefault('rewrite.ganrewrite', ganrewrite)

@@ -15,6 +15,7 @@ c_ll = ctypes.c_longlong
 c_f = ctypes.c_float
 c_p = ctypes.c_void_p
 c_sz = ctypes.c_size_t
+c_d = ctypes.c_double
 
 
 class RwError(RuntimeError):
@@ -98,6 +99,10 @@ SIGNATURES = {
     'rw_seg_prroi': (c_int, [c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p]),
     'rw_seg_classes': (c_int, [c_int, c_p, c_p, c_p, c_p, c_int, c_p, c_p, c_ll, c_int, c_int,
                                c_int, c_p, c_p, c_p]),
+    'rw_upsample_bilinear': (c_int, [c_p, c_int, c_int, c_int, c_int, c_int, c_int, c_d, c_d, c_d,
+                                     c_d, c_p, c_p]),
+    'rw_dissect_counts': (c_int, [c_p, c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                                  c_int, c_d, c_d, c_d, c_d, c_p, c_p, c_p, c_p, c_p]),
     'rw_lpips_input': (c_int, [c_p, c_p, c_int, c_int, c_int, c_int, c_p, c_p]),
     'rw_lpips_head': (c_int, [c_p, c_p, c_p, c_int, c_int, c_int, c_int, c_p, c_p]),
     'rw_lpips_combine_workspace_bytes': (c_sz, [c_int, c_int, c_int]),

@@ -1118,6 +1118,19 @@ int rw_seg_classes(int nsizes, const float* const* logits, const int* map_hw, co
                             Ho, Wo, probs, labels, stream);
 }
 
+int rw_upsample_bilinear(const float* act, int B, int U, int h, int w, int H, int W, double sy,
+                         double oy, double sx, double ox, float* rows, rw_stream_t stream) {
+  return upsample_bilinear_launch(act, B, U, h, w, H, W, sy, oy, sx, ox, rows, stream);
+}
+
+int rw_dissect_counts(const float* act, const float* level, const long long* labels, int B, int U,
+                      int h, int w, int H, int W, int K, int C, double sy, double oy, double sx,
+                      double ox, long long* isect, long long* unit_total, long long* label_total,
+                      long long* count, rw_stream_t stream) {
+  return dissect_counts_launch(act, level, labels, B, U, h, w, H, W, K, C, sy, oy, sx, ox, isect,
+                               unit_total, label_total, count, stream);
+}
+
 int rw_rowgemm(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo, int rows, int K,
                int N, float* out, rw_stream_t stream) {
   if (!a_hi || !a_lo || !w_hi || !w_lo || !out || rows < 1 || K % 64 != 0 || N % 64 != 0) {

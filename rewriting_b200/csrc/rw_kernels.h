@@ -302,4 +302,14 @@ int seg_classes_launch(int nsizes, const float* const* logits, const int* map_hw
                        long long mat_offset, int B, int Ho, int Wo, float* probs, long long* labels,
                        cudaStream_t stream);
 
+// ---------------------------------------------------------------------------
+// dissection statistics (dissect.cu)
+// ---------------------------------------------------------------------------
+int upsample_bilinear_launch(const float* act, int B, int U, int h, int w, int H, int W, double sy,
+                             double oy, double sx, double ox, float* rows, cudaStream_t stream);
+int dissect_counts_launch(const float* act, const float* level, const long long* labels, int B, int U,
+                          int h, int w, int H, int W, int K, int C, double sy, double oy, double sx,
+                          double ox, long long* isect, long long* unit_total, long long* label_total,
+                          long long* count, cudaStream_t stream);
+
 }  // namespace rw

@@ -913,3 +913,60 @@ def rowgemm(a, w_planes):
     out = torch.empty((M, N), dtype=torch.float32, device=a.device)
     _cabi.call('rw_rowgemm', _p(a_hi), _p(a_lo), _p(w_hi), _p(w_lo), M, K, N, _p(out), _stream())
     return out
+
+
+# --------------------------------------------------------------------------- dissection
+class DissectBatch(object):
+    """One batch for the fused unit / label count (rw_dissect_counts): activations [B,U,h,w],
+    per-unit levels [U], label maps [B,K,H,W] int64 with labels in 0..num_labels-1, and the
+    up-sampler's per-axis affine (sy, oy, sx, ox) onto the H x W label grid."""
+    __slots__ = ('act', 'level', 'labels', 'num_labels', 'affine')
+
+    def __init__(self, act, level, labels, num_labels, affine):
+        self.act, self.level, self.labels = act, level, labels
+        self.num_labels, self.affine = int(num_labels), tuple(float(v) for v in affine)
+
+
+def upsample_rows(act, size, affine):
+    """act [B,U,h,w] -> rows [B*H*W, U]: grid_sample(align_corners=True, zeros) over the affine
+    grid, row (b*H + y)*W + x (rw_upsample_bilinear)."""
+    act = _f32c(act)
+    if act.dim() != 4:
+        raise _cabi.RwError('upsample_rows: activations must be [B,U,h,w], got %s' % (tuple(act.shape),))
+    B, U, h, w = act.shape
+    H, W = size
+    rows = torch.empty(B * H * W, U, dtype=torch.float32, device=act.device)
+    _cabi.call('rw_upsample_bilinear', _p(act), B, U, h, w, H, W, *affine, _p(rows), _stream())
+    return rows
+
+
+def dissect_counts(batch, isect, unit_total, label_total, count):
+    """Adds one DissectBatch's counts to the int64 counters isect [C,U], unit_total [U],
+    label_total [C], count [1] (rw_dissect_counts).  Labels outside 0..C-1 are refused here,
+    before the launch, since the kernel cannot report them."""
+    act = _f32c(batch.act)
+    level = _f32c(batch.level)
+    labels = batch.labels
+    C = batch.num_labels
+    if act.dim() != 4 or labels.dim() != 4:
+        raise _cabi.RwError('dissect_counts: activations [B,U,h,w] and labels [B,K,H,W] expected, '
+                            'got %s and %s' % (tuple(act.shape), tuple(labels.shape)))
+    B, U, h, w = act.shape
+    _, K, H, W = labels.shape
+    if not labels.is_cuda or labels.dtype != torch.int64 or labels.shape[0] != B:
+        raise _cabi.RwError('dissect_counts: labels must be CUDA int64 [%d,K,H,W], got %s %s %s'
+                            % (B, labels.device, labels.dtype, tuple(labels.shape)))
+    if level.shape != (U,):
+        raise _cabi.RwError('dissect_counts: levels must be [%d], got %s' % (U, tuple(level.shape)))
+    for name, t, shape in (('isect', isect, (C, U)), ('unit_total', unit_total, (U,)),
+                           ('label_total', label_total, (C,)), ('count', count, (1,))):
+        if not t.is_cuda or t.dtype != torch.int64 or tuple(t.shape) != shape or not t.is_contiguous():
+            raise _cabi.RwError('dissect_counts: %s must be a contiguous CUDA int64 %s, got %s %s %s'
+                                % (name, shape, t.device, t.dtype, tuple(t.shape)))
+    labels = labels.contiguous()
+    lo, hi = torch.aminmax(labels)
+    lo, hi = int(lo), int(hi)
+    if lo < 0 or hi >= C:
+        raise _cabi.RwError('dissect_counts: labels must lie in 0..%d, got %d..%d' % (C - 1, lo, hi))
+    _cabi.call('rw_dissect_counts', _p(act), _p(level), _p(labels), B, U, h, w, H, W, K, C,
+               *batch.affine, _p(isect), _p(unit_total), _p(label_total), _p(count), _stream())

@@ -20,8 +20,14 @@ read-out, so quantiles are exact and deterministic; the reference's estimates ag
 to within its sketch resolution, and exactly while the sample fits the sketch (count <= 2r).
 State files interchange: a reference sketch (several levels with weights 2^level) loads and
 reads out with the reference's own interpolation rule, and the state written here is a
-one-level sketch the reference can load.  IoU / conditional statistics of the dissection tools
-stay out of scope (SURVEY.md §2.1 row 6).
+one-level sketch the reference can load.
+
+`RunningAllIntersectionAndUnion` holds GAN dissection's unit x label counts (reference:
+runningstats.py:1286-1344) as exact int64 on the device.  `add_dissection` adds one
+`ops.DissectBatch` (activations, levels, label maps, the up-sampler's affine) through the fused
+kernel `rw_dissect_counts`; the generic `add(S, G)` on bool tensors stays on torch (a float64
+matrix product, exact for these counts).  The conditional quantile sketch
+(`RunningConditionalQuantile`) and the other conditional statistics are not provided.
 """
 import math
 
@@ -403,6 +409,18 @@ class RunningQuantile(object):
     def minmax(self):
         return self.extremes.clone()
 
+    def unit_range(self, lo, hi):
+        """A RunningQuantile over units lo..hi-1 only, sharing this one's samples: its read-out
+        equals rows lo..hi-1 of this one's, with a fraction of the read-out's working memory."""
+        sub = RunningQuantile.__new__(RunningQuantile)
+        sub.__dict__.update(self.__dict__)
+        sub.depth = hi - lo
+        sub.extremes = self.extremes[lo:hi]
+        sub._chunks = [c[lo:hi] for c in self._chunks]
+        sub._upper = [None if u is None else u[lo:hi] for u in self._upper]
+        sub._summary = None
+        return sub
+
     def median(self):
         return self.quantiles([0.5])[:, 0]
 
@@ -457,6 +475,86 @@ class RunningQuantile(object):
         self.device = self.extremes.device
         self._summary = None
         self._level0_count = self._chunks[0].shape[1] if self._chunks else 0
+
+
+class RunningAllIntersectionAndUnion(object):
+    """Counts of two streams of binary vectors: intersection [a, b] (pairs set in both),
+    total_a [a], total_b [b] and the sample count (reference: runningstats.py:1286-1344).  The
+    counts are int64; `iou()` is intersection / union as the reference computes it.  State files
+    interchange with the reference's: the arrays are written as int64, and a reference state
+    (float32 counts) loads as int64."""
+
+    def __init__(self, state=None):
+        if state is not None:
+            self.set_state_dict(resolve_state_dict(state))
+            return
+        self.count = 0
+        self.intersection = None
+        self.total_a = None
+        self.total_b = None
+
+    def _init(self, a, b, device):
+        if self.intersection is None:
+            # stored [b, a] so that the fused kernel's [label, unit] counter is contiguous
+            self.intersection = torch.zeros(b, a, dtype=torch.int64, device=device).t()
+            self.total_a = torch.zeros(a, dtype=torch.int64, device=device)
+            self.total_b = torch.zeros(b, dtype=torch.int64, device=device)
+
+    def add(self, S, G):
+        """S [N, a], G [N, b] bool: intersection += S^T G, totals += column sums (torch)."""
+        assert S.dim() == 2 and G.dim() == 2 and S.dtype == torch.bool and G.dtype == torch.bool
+        assert len(S) == len(G), '%d vs %d' % (len(S), len(G))
+        self._init(S.shape[1], G.shape[1], S.device)
+        Sd, Gd = S.double(), G.double()
+        self.intersection += torch.mm(Sd.t(), Gd).round().long()
+        self.total_a += S.sum(0)
+        self.total_b += G.sum(0)
+        self.count += len(S)
+
+    def add_dissection(self, batch):
+        """One ops.DissectBatch: a = units above their level, b = labels (fused kernel)."""
+        U, C = batch.act.shape[1], batch.num_labels
+        self._init(U, C, batch.act.device)
+        if tuple(self.intersection.shape) != (U, C):
+            raise RuntimeError('RunningAllIntersectionAndUnion: %s counts, batch of %d units x %d '
+                               'labels' % (tuple(self.intersection.shape), U, C))
+        isect = self.intersection.t()
+        if not isect.is_contiguous() or not isect.is_cuda:
+            isect = isect.contiguous().to(batch.act.device)
+            self.intersection = isect.t()
+            self.total_a = self.total_a.to(isect.device)
+            self.total_b = self.total_b.to(isect.device)
+        n = torch.zeros(1, dtype=torch.int64, device=isect.device)
+        with nvtx.range('rw:dissect_counts'):
+            ops.dissect_counts(batch, isect, self.total_a, self.total_b, n)
+        self.count += batch.labels.shape[0] * batch.labels.shape[2] * batch.labels.shape[3]
+
+    def size(self):
+        return self.count
+
+    def iou(self):
+        union = self.total_a[:, None] + self.total_b[None, :] - self.intersection
+        return self.intersection / (union + 1e-20)
+
+    def to_(self, device):
+        self.total_a = self.total_a.to(device)
+        self.total_b = self.total_b.to(device)
+        self.intersection = self.intersection.to(device)
+
+    def state_dict(self):
+        return dict(constructor=self.__module__ + '.' + self.__class__.__name__ + '()',
+                    count=self.count,
+                    total_a=self.total_a.cpu().numpy(),
+                    total_b=self.total_b.cpu().numpy(),
+                    intersection=numpy.ascontiguousarray(self.intersection.cpu().numpy()))
+
+    def set_state_dict(self, dic):
+        def counts(v):
+            return torch.from_numpy(numpy.rint(numpy.asarray(v)).astype(numpy.int64))
+        self.count = int(numpy.asarray(dic['count']).item())
+        self.total_a = counts(dic['total_a'])
+        self.total_b = counts(dic['total_b'])
+        self.intersection = counts(dic['intersection'])
 
 
 def resolve_state_dict(s):

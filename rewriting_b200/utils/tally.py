@@ -1,6 +1,7 @@
 """Batched statistic drivers with .npz caching (API of the reference's `utils/tally.py`,
 hot-path subset): `tally_second_moment`, `tally_mean`, `tally_topk`, `tally_quantile`,
-`tally_topk_and_quantile`, `make_loader`, `load_cached_state`, `save_cached_state`.
+`tally_topk_and_quantile`, `tally_all_intersection_and_union`, `make_loader`, `load_cached_state`,
+`save_cached_state`.
 
 `tally_second_moment(compute, dataset, sample_size=None, batch_size=10, cachefile=None)`
 (reference: tally.py:424-443) iterates a DataLoader over the z dataset, calls
@@ -10,7 +11,9 @@ are `numpy.savez(cachefile, **state_dict, **args)` and are validated against `ar
 
 Extension (not in the reference): `compute` may return `ops.KeyPlanes` instead of a tensor,
 in which case the planes feed the tensor-core accumulator directly with no fp32 round trip
-(used by the rewriter's fused key capture).
+(used by the rewriter's fused key capture).  Likewise `tally_all_intersection_and_union` takes
+`ops.DissectBatch` (activations, levels, label maps, the up-sampler's affine) and feeds it to the
+fused dissection count, which never builds the indicator tensors.
 """
 import os
 
@@ -198,3 +201,25 @@ def tally_topk_and_quantile(compute, dataset, sample_size=None, batch_size=10, k
     rq.to_('cpu')
     save_cached_state(cachefile, _Combined(rtk=rtk, rq=rq), args)
     return rtk, rq
+
+
+def tally_all_intersection_and_union(compute, dataset, sample_size=None, batch_size=10,
+                                     cachefile=None, **kwargs):
+    """All-pairs intersection and union counts of two streams of binary vectors (reference:
+    tally.py:446-466): `compute` returns (S [N, a], G [N, b]) bool batches, or an
+    `ops.DissectBatch` for the fused unit x label count."""
+    args = dict(sample_size=sample_size)
+    cached = load_cached_state(cachefile, args)
+    if cached is not None:
+        return runningstats.RunningAllIntersectionAndUnion(state=cached)
+    riu = runningstats.RunningAllIntersectionAndUnion()
+    loader = batches(dataset, sample_size, batch_size, **kwargs)
+    for batch in pbar(loader):
+        sample = call_compute(compute, batch)
+        if isinstance(sample, ops.DissectBatch):
+            riu.add_dissection(sample)
+        else:
+            riu.add(*sample)
+    riu.to_('cpu')
+    save_cached_state(cachefile, riu, args)
+    return riu
