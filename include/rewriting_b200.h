@@ -108,7 +108,11 @@ int rw_modconv_up_fwd(const void* kp_hi, const void* kp_lo, const void* wt_hi, c
  *                                   with rgb_w[B,3,Cout]
  * `out` (fp32 NCHW) becomes optional.  rw_modconv_up_fwd_cl writes the conv_transpose output
  * channels-last per phase, t_cl[4][rows][Cout]; rw_blur_up_fused turns it into the next layer's
- * planes (and/or fp32 NCHW); rw_rgb_combine = sum of partials + bias + 2x-upsampled skip. */
+ * planes, split_bf16(next_scale[b,c] * leaky_relu(blur(t) + noise_w[0]*noise + bias)*sqrt(2));
+ * rw_rgb_combine = sum of partials + bias + 2x-upsampled skip.
+ * rw_blur_up_fused requires every pointer, C % 64 == 0, bias and next_scale 16-byte aligned,
+ * and fewer than 2^31 rows in t_cl and 8x16-output tiles x 64-channel blocks; otherwise it returns
+ * RW_STATUS_BAD_ARG before anything is launched. */
 int rw_modconv_fwd_fused(const void* kp_hi, const void* kp_lo, const void* wt_hi,
                          const void* wt_lo, const float* scale_bo, const float* noise,
                          long long noise_bstride, const float* noise_w, const float* bias, int act,
@@ -120,8 +124,8 @@ int rw_modconv_up_fwd_cl(const void* kp_hi, const void* kp_lo, const void* wt_hi
                          int W, float* t_cl, rw_stream_t stream);
 int rw_blur_up_fused(const float* t_cl, int B, int C, int Hin, int Win, const float* kernel4x4,
                      const float* noise, long long noise_bstride, const float* noise_w,
-                     const float* bias, int act, const float* next_scale, void* next_hi,
-                     void* next_lo, float* y_out, rw_stream_t stream);
+                     const float* bias, const float* next_scale, void* next_hi, void* next_lo,
+                     rw_stream_t stream);
 /* The whole upsampling StyledConv of the fast path in ONE kernel (csrc/upconv_tc.cu):
  * conv_transpose2d(stride 2) -> 4x4 blur (pad 1,1) -> * demod -> + noise_w*noise + bias ->
  * leaky-ReLU*sqrt(2) -> * next_scale -> the next layer's bf16 hi/lo planes (pad row/column zeroed).

@@ -116,7 +116,7 @@ SIGNATURES = {
                                       c_int, c_int, c_int, c_int, c_int, c_p, c_p, c_p, c_p,
                                       c_p, c_p, c_p, c_p]),
     'rw_blur_up_fused': (c_int, [c_p, c_int, c_int, c_int, c_int, c_p, c_p, c_ll, c_p, c_p,
-                                 c_int, c_p, c_p, c_p, c_p, c_p]),
+                                 c_p, c_p, c_p, c_p]),
     'rw_styles': (c_int, [c_p, c_int, c_int, c_int, c_f, c_int, c_p, c_p, c_p, c_p, c_p, c_p]),
     'rw_equal_linear': (c_int, [c_p, c_int, c_int, c_p, c_p, c_int, c_f, c_f, c_int, c_p, c_p]),
     'rw_pixel_norm': (c_int, [c_p, c_int, c_int, c_p, c_p]),

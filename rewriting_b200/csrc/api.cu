@@ -683,15 +683,14 @@ int rw_debug_upconv_profile(const void* kp_hi, const void* kp_lo, const void* wt
 
 int rw_blur_up_fused(const float* t_cl, int B, int C, int Hin, int Win, const float* kernel4x4,
                      const float* noise, long long noise_bstride, const float* noise_w,
-                     const float* bias, int act, const float* next_scale, void* next_hi,
-                     void* next_lo, float* y_out, rw_stream_t stream) {
-  if (!t_cl || !kernel4x4 || (noise && !noise_w) || ((next_hi != nullptr) != (next_lo != nullptr)) ||
-      (!next_hi && !y_out)) {
-    set_last_error("rw_blur_up_fused: bad argument");
+                     const float* bias, const float* next_scale, void* next_hi, void* next_lo,
+                     rw_stream_t stream) {
+  if (!t_cl || !kernel4x4 || !noise || !noise_w || !bias || !next_scale || !next_hi || !next_lo) {
+    set_last_error("rw_blur_up_fused: bad argument (every pointer is required)");
     return RW_ERR_BAD_ARG;
   }
   return blur_up_fused_launch(t_cl, B, C, Hin, Win, kernel4x4, noise, noise_bstride, noise_w, bias,
-                              act, next_scale, next_hi, next_lo, y_out, stream);
+                              next_scale, next_hi, next_lo, stream);
 }
 
 int rw_styles(const float* latent, int B, int n_latent, int K, float scale, int n,

@@ -137,8 +137,8 @@ int blur_up_act_launch(const float* t, int B, int C, int Hin, int Win, const flo
                        const float* bias, int act, float* y, cudaStream_t stream);
 int blur_up_fused_launch(const float* t_cl, int B, int C, int Hin, int Win, const float* k4,
                          const float* noise, long long noise_bstride, const float* noise_w,
-                         const float* bias, int act, const float* next_scale, void* next_hi,
-                         void* next_lo, float* y_out, cudaStream_t stream);
+                         const float* bias, const float* next_scale, void* next_hi, void* next_lo,
+                         cudaStream_t stream);
 int rgb_combine_launch(const float* part, int nparts, int B, int H, int W, const float* bias,
                        const float* prev, const float* k4, float* out, unsigned char* out_u8,
                        cudaStream_t stream);

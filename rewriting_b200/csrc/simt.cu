@@ -368,143 +368,31 @@ __global__ void add_noise_kernel(const float* __restrict__ x, const float* __res
 }
 
 // ---------------------------------------------------------------------------
-// blur_up_fused: generation fast path for an upsampling StyledConv.
+// blur_up_fused: the blur half of the generation fast path's round-1 upsampling pair.
 //   t_cl  [4 phases][rows_in][C] fp32 channels-last (conv_tc out_mode 1; phase = (ty&1)*2+(tx&1),
 //         row = (b*(H+1) + ty/2)*(W+1) + tx/2) — the conv_transpose output, demodulated
-//   v = act( FIR4x4(pad(t,1,1)) + noise_w*noise + bias )                       (as blur_up_act)
+//   v = lrelu( FIR4x4(pad(t,1,1)) + noise_w*noise + bias ) * sqrt(2)            (as blur_up_act)
 //   -> next layer's key planes  split_bf16(next_scale[b,c] * v)  over the padded-flat grid of
-//      the OUTPUT resolution (pad row / column written as zeros), optional fp32 NCHW copy.
-// block: 64 channels x (8 x 16) outputs; thread = (pixel group, channel quad); float4 smem reads.
-// ---------------------------------------------------------------------------
-constexpr int BF_TY = 8, BF_TX = 16, BF_C = 64;
-constexpr int BF_PW = BF_TX + 3, BF_PH = BF_TY + 3;
-
-__global__ void __launch_bounds__(256, 4)
-blur_up_fused_kernel(const float* __restrict__ t_cl, int B, int C, int H, int W,
-                     const float* __restrict__ k4, const float* __restrict__ noise,
-                     long long noise_bstride, const float* __restrict__ noise_w,
-                     const float* __restrict__ bias, int act,
-                     const float* __restrict__ next_scale, __nv_bfloat16* __restrict__ next_hi,
-                     __nv_bfloat16* __restrict__ next_lo, float* __restrict__ y_out) {
-  extern __shared__ float4 tile4[];      // [BF_PH*BF_PW][16 quads]
-  __shared__ float kf[16];
-  const int Ho = 2 * H, Wo = 2 * W;
-  const int Hp_in = H + 1, Wp_in = W + 1;
-  const long long rows_in = static_cast<long long>(B) * Hp_in * Wp_in;
-  const int cblocks = C / BF_C;
-  const int b = blockIdx.z / cblocks;
-  const int c0 = (blockIdx.z - b * cblocks) * BF_C;
-  const int ox0 = blockIdx.x * BF_TX, oy0 = blockIdx.y * BF_TY;
-  const int tid = threadIdx.x;
-  if (tid < 16) kf[tid] = __ldg(k4 + 15 - tid);   // flipped kernel (upfirdn2d correlates)
-  for (int i = tid; i < BF_PH * BF_PW * 16; i += 256) {
-    const int qd = i & 15;
-    const int pos = i >> 4;
-    const int ly = pos / BF_PW, lx = pos - ly * BF_PW;
-    const int ty = oy0 + ly - 1, tx = ox0 + lx - 1;
-    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (ty >= 0 && ty <= Ho && tx >= 0 && tx <= Wo) {
-      const int ph = (ty & 1) * 2 + (tx & 1);
-      const long long row = (static_cast<long long>(b) * Hp_in + (ty >> 1)) * Wp_in + (tx >> 1);
-      v = __ldg(reinterpret_cast<const float4*>(t_cl + (ph * rows_in + row) * C + c0) + qd);
-    }
-    tile4[i] = v;
-  }
-  __syncthreads();
-  const int qd = tid & 15;
-  const int grp = tid >> 4;                 // 16 groups of 8 pixels
-  const int ly = grp >> 1;
-  const int lx0 = (grp & 1) * 8;
-  const int oy = oy0 + ly;
-  if (oy > Ho) return;
-  const int c = c0 + qd * 4;
-  const float nw = noise ? __ldg(noise_w) : 0.f;
-  float4 bs = make_float4(0.f, 0.f, 0.f, 0.f);
-  if (bias) bs = __ldg(reinterpret_cast<const float4*>(bias + c));
-  float4 sc = make_float4(1.f, 1.f, 1.f, 1.f);
-  if (next_scale) sc = __ldg(reinterpret_cast<const float4*>(next_scale + static_cast<size_t>(b) * C + c));
-  const size_t out_row0 = (static_cast<size_t>(b) * (Ho + 1) + oy) * (Wo + 1);
-
-  // 8 consecutive outputs of one row: slide over 11 input columns per filter row, so every
-  // smem value is read once (44 LDS.128 instead of 128) — the kernel is smem-bound otherwise.
-  float4 a[8];
-#pragma unroll
-  for (int px = 0; px < 8; ++px) a[px] = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-  for (int fy = 0; fy < 4; ++fy) {
-    float4 tv[11];
-#pragma unroll
-    for (int i = 0; i < 11; ++i) tv[i] = tile4[((ly + fy) * BF_PW + lx0 + i) * 16 + qd];
-#pragma unroll
-    for (int fx = 0; fx < 4; ++fx) {
-      const float kk = kf[fy * 4 + fx];
-#pragma unroll
-      for (int px = 0; px < 8; ++px) {
-        a[px].x = fmaf(tv[px + fx].x, kk, a[px].x);
-        a[px].y = fmaf(tv[px + fx].y, kk, a[px].y);
-        a[px].z = fmaf(tv[px + fx].z, kk, a[px].z);
-        a[px].w = fmaf(tv[px + fx].w, kk, a[px].w);
-      }
-    }
-  }
-#pragma unroll
-  for (int px = 0; px < 8; ++px) {
-    const int ox = ox0 + lx0 + px;
-    if (ox > Wo) break;
-    float4 v = a[px];
-    const bool real = (oy < Ho) && (ox < Wo);
-    if (real) {
-      if (noise) {
-        const float nz = nw * __ldg(noise + static_cast<size_t>(b) * noise_bstride +
-                                    static_cast<size_t>(oy) * Wo + ox);
-        v.x += nz; v.y += nz; v.z += nz; v.w += nz;
-      }
-      v.x += bs.x; v.y += bs.y; v.z += bs.z; v.w += bs.w;
-      if (act) {
-        v.x = (v.x > 0.f ? v.x : 0.2f * v.x) * 1.4142135623730951f;
-        v.y = (v.y > 0.f ? v.y : 0.2f * v.y) * 1.4142135623730951f;
-        v.z = (v.z > 0.f ? v.z : 0.2f * v.z) * 1.4142135623730951f;
-        v.w = (v.w > 0.f ? v.w : 0.2f * v.w) * 1.4142135623730951f;
-      }
-      if (y_out) {
-        const size_t hw = static_cast<size_t>(Ho) * Wo;
-        float* yp = y_out + (static_cast<size_t>(b) * C + c) * hw + static_cast<size_t>(oy) * Wo + ox;
-        yp[0] = v.x; yp[hw] = v.y; yp[2 * hw] = v.z; yp[3 * hw] = v.w;
-      }
-    }
-    if (next_hi) {
-      const float k0 = real ? sc.x * v.x : 0.f, k1 = real ? sc.y * v.y : 0.f;
-      const float k2 = real ? sc.z * v.z : 0.f, k3 = real ? sc.w * v.w : 0.f;
-      const __nv_bfloat162 h01 = __floats2bfloat162_rn(k0, k1), h23 = __floats2bfloat162_rn(k2, k3);
-      const float2 f01 = __bfloat1622float2(h01), f23 = __bfloat1622float2(h23);
-      const __nv_bfloat162 l01 = __floats2bfloat162_rn(k0 - f01.x, k1 - f01.y);
-      const __nv_bfloat162 l23 = __floats2bfloat162_rn(k2 - f23.x, k3 - f23.y);
-      const size_t off = (out_row0 + ox) * C + c;
-      *reinterpret_cast<uint2*>(next_hi + off) =
-          make_uint2(*reinterpret_cast<const uint32_t*>(&h01), *reinterpret_cast<const uint32_t*>(&h23));
-      *reinterpret_cast<uint2*>(next_lo + off) =
-          make_uint2(*reinterpret_cast<const uint32_t*>(&l01), *reinterpret_cast<const uint32_t*>(&l23));
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------
-// blur_up_pipe: blur_up_fused for the generation fast path's configuration (noise + bias +
-// leaky-ReLU, output = the next layer's key planes only), rebuilt after an ncu capture of the
-// one-tile-per-CTA kernel on layer 13 (profiles/: 0.84 ms, DRAM 31 %, issue slots 58 % busy, ALU
-// the top pipe — 607 M warp instructions, of which the 16-tap FIR was only a third):
+//      the OUTPUT resolution (pad row / column written as zeros).
+// tile: 64 channels x (8 x 16) outputs; thread = (pixel group, channel quad); float4 smem reads.
+// The design follows an ncu capture of an earlier one-tile-per-CTA version on layer 13 (profiles/:
+// 0.84 ms, DRAM 31 %, issue slots 58 % busy, ALU the top pipe — 607 M warp instructions, of which
+// the 16-tap FIR was only a third):
 //  * persistent CTAs (2 per SM) walk the tile list with a static stride; tile i+1 is prefetched
 //    with cp.async (16 B, zero-fill outside the image) into the second buffer while tile i is
 //    filtered;
 //  * index arithmetic hoisted: the (ly, lx) of a thread's 14 staging slots come from a small
 //    shared table, the tile coordinate advances as a mixed-radix counter (no division in the
 //    loop), channel-block fastest so that both 256-byte halves of a row move together;
-//  * no per-pixel null-pointer branches (the generic kernel keeps those), leaky-ReLU as
-//    max(v, 0.2 v);
+//  * every operand is required (the host refuses a NULL), so no per-pixel null-pointer branches;
+//    leaky-ReLU as max(v, 0.2 v);
 //  * a rank-one 4x4 FIR (the model's [1,3,3,1] x [1,3,3,1]) is applied separably: 176 + 128
 //    instead of 512 FMAs per thread.  Detected on the device (exact rank-one test), other
 //    kernels take the 16-tap loop.
 // ---------------------------------------------------------------------------
+constexpr int BF_TY = 8, BF_TX = 16, BF_C = 64;
+constexpr int BF_PW = BF_TX + 3, BF_PH = BF_TY + 3;
+
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(dst), "l"(src) : "memory");
 }
@@ -1338,59 +1226,42 @@ int add_noise_launch(const float* x, const float* noise, long long noise_bstride
 
 int blur_up_fused_launch(const float* t_cl, int B, int C, int Hin, int Win, const float* k4,
                          const float* noise, long long noise_bstride, const float* noise_w,
-                         const float* bias, int act, const float* next_scale, void* next_hi,
-                         void* next_lo, float* y_out, cudaStream_t stream) {
+                         const float* bias, const float* next_scale, void* next_hi, void* next_lo,
+                         cudaStream_t stream) {
   if (C % BF_C != 0) {
     set_last_error("blur_up_fused: C=%d must be a multiple of 64", C);
     return RW_ERR_BAD_ARG;
   }
+  if ((reinterpret_cast<uintptr_t>(bias) | reinterpret_cast<uintptr_t>(next_scale)) & 15u) {
+    set_last_error("blur_up_fused: bias and next_scale must be 16-byte aligned");
+    return RW_ERR_BAD_ARG;
+  }
   const int Ho = 2 * Hin, Wo = 2 * Win;
+  const int tiles_x = (Wo + 1 + BF_TX - 1) / BF_TX, tiles_y = (Ho + 1 + BF_TY - 1) / BF_TY;
+  const long long ntiles = static_cast<long long>(tiles_x) * tiles_y * B * (C / BF_C);
+  const long long rows_in4 = 4LL * B * (Hin + 1) * (Win + 1);
+  if (ntiles >= 0x7fffffffLL || rows_in4 >= 0x7fffffffLL) {
+    set_last_error("blur_up_fused: %lld tiles, %lld input rows: both must stay below 2^31", ntiles,
+                   rows_in4);
+    return RW_ERR_BAD_ARG;
+  }
   const size_t smem = static_cast<size_t>(BF_PH) * BF_PW * 16 * sizeof(float4);
   static bool attr = false;
   if (!attr) {
-    int rc = check_cuda(cudaFuncSetAttribute(blur_up_fused_kernel,
+    int rc = check_cuda(cudaFuncSetAttribute(blur_up_pipe_kernel,
                                              cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             static_cast<int>(smem)),
-                        "blur_up_fused smem attr");
+                                             static_cast<int>(2 * smem)),
+                        "blur_up_pipe smem attr");
     if (rc) return rc;
     attr = true;
   }
-  const long long gz = static_cast<long long>(B) * (C / BF_C);
-  if (gz > 65535) {
-    set_last_error("blur_up_fused: grid.z %lld too large", gz);
-    return RW_ERR_BAD_ARG;
-  }
-  const int tiles_x = (Wo + 1 + BF_TX - 1) / BF_TX, tiles_y = (Ho + 1 + BF_TY - 1) / BF_TY;
-  const long long ntiles = static_cast<long long>(tiles_x) * tiles_y * gz;
-  const long long rows_in4 = 4LL * B * (Hin + 1) * (Win + 1);
-  // the generation fast path's configuration runs the pipelined kernel; anything else (no noise,
-  // no activation, fp32 NCHW output, huge index ranges) the generic one-tile-per-CTA kernel
-  const bool fast = noise && noise_w && bias && act && next_scale && next_hi && next_lo && !y_out &&
-                    ntiles < 0x7fffffffLL && rows_in4 < 0x7fffffffLL &&
-                    ((reinterpret_cast<uintptr_t>(bias) | reinterpret_cast<uintptr_t>(next_scale)) & 15u) == 0;
-  if (fast) {
-    static bool attr2 = false;
-    if (!attr2) {
-      int rc = check_cuda(cudaFuncSetAttribute(blur_up_pipe_kernel,
-                                               cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                               static_cast<int>(2 * smem)),
-                          "blur_up_pipe smem attr");
-      if (rc) return rc;
-      attr2 = true;
-    }
-    long long g = 2LL * device_sm_count();
-    if (g > ntiles) g = ntiles;
-    blur_up_pipe_kernel<<<static_cast<unsigned>(g), 256, 2 * smem, stream>>>(
-        t_cl, B, C, Hin, Win, k4, noise, noise_bstride, noise_w, bias, next_scale,
-        static_cast<__nv_bfloat16*>(next_hi), static_cast<__nv_bfloat16*>(next_lo), tiles_x, tiles_y,
-        static_cast<unsigned>(ntiles));
-    return check_cuda(cudaGetLastError(), "blur_up_pipe launch");
-  }
-  dim3 grid(tiles_x, tiles_y, static_cast<unsigned>(gz));
-  blur_up_fused_kernel<<<grid, 256, smem, stream>>>(
-      t_cl, B, C, Hin, Win, k4, noise, noise_bstride, noise_w, bias, act, next_scale,
-      static_cast<__nv_bfloat16*>(next_hi), static_cast<__nv_bfloat16*>(next_lo), y_out);
-  return check_cuda(cudaGetLastError(), "blur_up_fused launch");
+  long long g = 2LL * device_sm_count();
+  if (g > ntiles) g = ntiles;
+  blur_up_pipe_kernel<<<static_cast<unsigned>(g), 256, 2 * smem, stream>>>(
+      t_cl, B, C, Hin, Win, k4, noise, noise_bstride, noise_w, bias, next_scale,
+      static_cast<__nv_bfloat16*>(next_hi), static_cast<__nv_bfloat16*>(next_lo), tiles_x, tiles_y,
+      static_cast<unsigned>(ntiles));
+  return check_cuda(cudaGetLastError(), "blur_up_pipe launch");
 }
 
 int rgb_combine_launch(const float* part, int nparts, int B, int H, int W, const float* bias,

@@ -6,7 +6,9 @@ extra passes over every activation.  When the WHOLE generator runs unhooked and 
 autograd, nothing observes those tensors, so this module chains the kernels directly:
 
     planes(L) --conv_tc--> epilogue { lrelu(..)·√2 ; x next style -> planes(L+1) ; ToRGB partial }
+    planes(L) --modconv_up_fused--> planes(L+1)      (upsampling layers, one kernel)
     planes(L) --conv_tc(4 phases)--> t (channels-last) --blur_up_fused--> planes(L+1)
+                                     (upsampling layers that `ops.up_fused_eligible` declines)
     rgb partials --rgb_combine--> running image (+ bias + 2x-upsampled skip)
 
 The arithmetic per element is the same as the layer path (same kernels, same fp32 epilogue
@@ -81,19 +83,6 @@ def eligible(model, z):
     if sg2._is_hooked(model):
         return False
     return _layer_list(model) is not None
-
-
-import os as _os
-
-# RW_UP_FUSED=0 keeps the round-1 pair (conv_transpose phases -> channels-last t -> blur kernel);
-# RW_UP_FUSED_MINW = smallest input width that takes the fused kernel
-_UP_FUSED = _os.environ.get('RW_UP_FUSED', '1') != '0'
-_UP_FUSED_MINW = int(_os.environ.get('RW_UP_FUSED_MINW', '4'))
-
-
-def _use_fused_up(mc, Cin, Cout, H, W):
-    return (_UP_FUSED and H == W and _UP_FUSED_MINW <= W <= 128 and (W & (W - 1)) == 0 and
-            Cin % 64 == 0 and Cout % 16 == 0 and ops.blur_is_separable(mc.blur.kernel))
 
 
 def _mapping(model, z, stream):
@@ -214,7 +203,7 @@ def _forward(model, z, upto_key_layer, noise_period, out_u8):
         next_scale = styles[nxt[0]] if nxt is not None else None
         nw = sconv.noise.weight.detach()
         bias = sconv.activate.bias.detach()
-        if mc.upsample and _use_fused_up(mc, Cin, Cout, H, W):
+        if mc.upsample and ops.up_fused_eligible(Cin, Cout, H, W, mc.blur.kernel):
             # conv_transpose + blur + noise + bias + act + next style in ONE tensor-core kernel
             u_hi, u_lo, _ = ops.weight_planes(dconv.weight, 'upf')
             Ho, Wo = 2 * H, 2 * W
@@ -238,8 +227,7 @@ def _forward(model, z, upto_key_layer, noise_period, out_u8):
             nh = torch.empty((rows_o, Cout), dtype=torch.bfloat16, device=dev)
             nl = torch.empty_like(nh)
             _cabi.call('rw_blur_up_fused', _p(t_cl), B, Cout, H, W, _p(mc.blur.kernel), _p(noise),
-                       noise.stride(0), _p(nw), _p(bias), 1, _p(next_scale), _p(nh), _p(nl), None,
-                       stream)
+                       noise.stride(0), _p(nw), _p(bias), _p(next_scale), _p(nh), _p(nl), stream)
             H, W = Ho, Wo
             planes = ops.KeyPlanes(nh, nl, B, Cout, H, W)
         else:

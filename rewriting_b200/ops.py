@@ -175,11 +175,10 @@ _SEPARABLE = {}
 
 def up_fused_eligible(Cin, Cout, H, W, blur_kernel):
     """Shapes the fused upsampling kernel takes (csrc/upconv_tc.cu): square power-of-two input of
-    width 4..128, Cin % 64 == 0, Cout % 16 == 0, rank-one 4x4 FIR; RW_UP_FUSED=0 turns it off."""
-    import os
-    return (os.environ.get('RW_UP_FUSED', '1') != '0' and H == W and 4 <= W <= 128 and
-            (W & (W - 1)) == 0 and Cin % 64 == 0 and Cout % 16 == 0 and
-            tuple(blur_kernel.shape) == (4, 4) and blur_is_separable(blur_kernel))
+    width 4..128, Cin % 64 == 0, Cout % 16 == 0, rank-one 4x4 FIR.  The one rule by which both the
+    layer path and the generation fast path choose it over the conv_transpose + blur pair."""
+    return (H == W and 4 <= W <= 128 and (W & (W - 1)) == 0 and Cin % 64 == 0 and
+            Cout % 16 == 0 and tuple(blur_kernel.shape) == (4, 4) and blur_is_separable(blur_kernel))
 
 
 def blur_is_separable(kernel):
@@ -345,6 +344,28 @@ def conv_wgrad_planes(g_planes, k_planes):
     return out
 
 
+def convT3x3_dgrad_planes(gph_hi, gph_lo, w_hi, w_lo, B, Cin, Cout, H, W):
+    """data gradient of convT3x3_planes from the four gradient phase planes [rows, 4*Cout] and the
+    'dgrad_up' weight planes -> [B,Cin,H,W] fp32."""
+    out = torch.empty((B, Cin, H, W), dtype=torch.float32, device=gph_hi.device)
+    _cabi.call('rw_modconv_up_dgrad', _p(gph_hi), _p(gph_lo), _p(w_hi), _p(w_lo), None, B, Cin,
+               Cout, H, W, _p(out), _stream())
+    return out
+
+
+def conv_up_wgrad_planes(gph_hi, gph_lo, k_planes, Cout):
+    """weight gradient of convT3x3_planes from the four gradient phase planes and the key planes
+    -> [Cout, 9, Cin] fp32."""
+    rows, Cin = k_planes.rows, k_planes.C
+    dev = gph_hi.device
+    lib = _cabi.load()
+    ws = _workspace(lib.rw_gram_workspace_bytes(Cout, Cin, rows, 9), dev)
+    out = torch.empty((Cout, 9, Cin), dtype=torch.float32, device=dev)
+    _cabi.call('rw_conv_up_wgrad', _p(gph_hi), _p(gph_lo), _p(k_planes.hi), _p(k_planes.lo), rows,
+               Cout, Cin, k_planes.W + 1, _p(out), _p(ws), ws.numel() * 4, _stream())
+    return out
+
+
 # --------------------------------------------------------------------------- rank projection
 def project_rank(weight, direction, base=None, sign=1.0):
     """base + sign * projected_conv(weight, direction)   (ganrewrite.py:806-813)."""
@@ -466,16 +487,9 @@ class StyledConvFunction(torch.autograd.Function):
                        Cout, H, W, _p(gph_hi), _p(gph_lo), _stream())
             if need_dk:
                 wd_hi, wd_lo, _ = ctx.wholder.planes('dgrad_up')
-                dk = torch.empty((B, Cin, H, W), dtype=torch.float32, device=dev)
-                _cabi.call('rw_modconv_up_dgrad', _p(gph_hi), _p(gph_lo), _p(wd_hi), _p(wd_lo),
-                           None, B, Cin, Cout, H, W, _p(dk), _stream())
+                dk = convT3x3_dgrad_planes(gph_hi, gph_lo, wd_hi, wd_lo, B, Cin, Cout, H, W)
             if need_w:
-                lib = _cabi.load()
-                ws = _workspace(lib.rw_gram_workspace_bytes(Cout, Cin, rows, 9), dev)
-                dwt = torch.empty((Cout, 9, Cin), dtype=torch.float32, device=dev)
-                _cabi.call('rw_conv_up_wgrad', _p(gph_hi), _p(gph_lo), _p(k_planes.hi),
-                           _p(k_planes.lo), rows, Cout, Cin, W + 1, _p(dwt), _p(ws),
-                           ws.numel() * 4, _stream())
+                dwt = conv_up_wgrad_planes(gph_hi, gph_lo, k_planes, Cout)
         else:
             g_planes, _ = prep_keys(g_pre, dm)          # planes of g_t = g_pre * demod
             if need_dk:
@@ -564,16 +578,9 @@ class ConvTransposeLeafFunction(torch.autograd.Function):
         gk = g_style = gW = None
         if need_k:
             wd_hi, wd_lo, _ = ctx.wholder.planes('dgrad_up')
-            gk = torch.empty((B, Cin, H, W), dtype=torch.float32, device=dev)
-            _cabi.call('rw_modconv_up_dgrad', _p(gph_hi), _p(gph_lo), _p(wd_hi), _p(wd_lo), None, B,
-                       Cin, Cout, H, W, _p(gk), _stream())
+            gk = convT3x3_dgrad_planes(gph_hi, gph_lo, wd_hi, wd_lo, B, Cin, Cout, H, W)
         if need_w:
-            lib = _cabi.load()
-            ws = _workspace(lib.rw_gram_workspace_bytes(Cout, Cin, rows, 9), dev)
-            dwt = torch.empty((Cout, 9, Cin), dtype=torch.float32, device=dev)
-            _cabi.call('rw_conv_up_wgrad', _p(gph_hi), _p(gph_lo), _p(ctx.planes.hi),
-                       _p(ctx.planes.lo), rows, Cout, Cin, W + 1, _p(dwt), _p(ws), ws.numel() * 4,
-                       _stream())
+            dwt = conv_up_wgrad_planes(gph_hi, gph_lo, ctx.planes, Cout)
             gW = torch.empty(weight.shape, dtype=torch.float32, device=dev)
             _cabi.call('rw_wgrad_finish', _p(dwt), _p(_f32c(weight.detach())), _p(s_dot), _p(dm),
                        _p(style), B, Cout, Cin, 1.0 / math.sqrt(Cin * 9), _p(gW), _stream())

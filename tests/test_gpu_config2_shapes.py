@@ -220,19 +220,19 @@ def test_styled_conv_fwd_bwd_batch32_vs_fp64(seeded_sd, shape, monkeypatch):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize('shape', UP_SHAPES, ids=[s[0] for s in UP_SHAPES])
-def test_round1_upsampling_pair_batch32_vs_fp64(seeded_sd, shape, monkeypatch):
-    """RW_UP_FUSED=0 (or a shape the fused kernel does not take): rw_modconv_up_fwd, conv_tc over
-    the four conv_transpose phases with decode_tile's phase-rotating schedule, then
-    rw_blur_up_act.  From layer 9 on, conv_tc's units outnumber its clusters, so clusters take
-    further units."""
-    from rewriting_b200 import _cabi
+def test_round1_pair_where_fused_declined_batch32_vs_fp64(seeded_sd, shape, monkeypatch):
+    """The pair that shapes the fused kernel does not take run (forced here by patching
+    `ops.up_fused_eligible`): rw_modconv_up_fwd, conv_tc over the four conv_transpose phases with
+    decode_tile's phase-rotating schedule, then rw_blur_up_act.  From layer 9 on, conv_tc's units
+    outnumber its clusters, so clusters take further units."""
+    from rewriting_b200 import _cabi, ops
     name, cin, cout, h, up = shape
     if h >= 32:
         m_tiles = -(-B * (h + 1) * (h + 1) // 128)
         units = -(-m_tiles // 2) * (cout // 128) * 4          # (m-tile pair, n-tile, phase)
         assert units > _cabi.load().rw_device_sm_count() // 2, (name, units)
     inp = _inputs(seeded_sd, shape, seed=300 + int(name[5:]))
-    monkeypatch.setenv('RW_UP_FUSED', '0')
+    monkeypatch.setattr(ops, 'up_fused_eligible', lambda *a: False)
     calls = _spy(monkeypatch)
     got = _run(inp, backward=False)['y']
     torch.cuda.synchronize()

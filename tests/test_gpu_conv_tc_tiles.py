@@ -477,7 +477,8 @@ def _byte_offset(t, nbytes):
 @pytest.mark.parametrize('Cout', [64, 128])
 def test_misaligned_epilogue_pointers_are_refused(Cout):
     """Pointers the epilogue would access misaligned return RW_STATUS_BAD_ARG, with the pointer
-    named in rw_last_error(), and nothing is launched: the outputs keep their NaN fill."""
+    named in rw_last_error(), and nothing is launched: the outputs keep their NaN fill.  So do a
+    NULL noise and a misaligned bias given to rw_blur_up_fused, which reads this conv's t_cl."""
     from rewriting_b200 import ops
     c = Conv3x3(2, 64, Cout, 6, seed=900 + Cout)
     st = ops._stream()
@@ -517,8 +518,23 @@ def test_misaligned_epilogue_pointers_are_refused(Cout):
     rc, msg = _status('rw_modconv_fwd', *base, _p(c.scale_bo), None, 0, None,
                       _byte_offset(c.bias, 2), 1, c.B, c.Cin, Cout, c.H, c.W, _p(out), st)
     assert rc == BAD_ARG and 'bias' in msg, (rc, msg)
+    # the pipelined blur over this conv's channels-last phases: every operand is required, and
+    # bias / next_scale are read as float4
+    kern = torch.ones(4, 4, device='cuda')
+    bnoise = ops.noise_table(c.B, 4 * c.H * c.W, 'cuda')
+    rows_o = c.B * (2 * c.H + 1) * (2 * c.W + 1)
+    bhi_buf, bhi = _guarded((rows_o, Cout), torch.bfloat16)
+    blo_buf, blo = _guarded((rows_o, Cout), torch.bfloat16)
+
+    def blur(noise_p, bias_p):
+        return _status('rw_blur_up_fused', _p(t_cl), c.B, Cout, c.H, c.W, _p(kern), noise_p,
+                       bnoise.stride(0), _p(c.nw), bias_p, _p(c.nscale), _p(bhi), _p(blo), st)
+    rc, msg = blur(None, _p(c.bias))
+    assert rc == BAD_ARG and 'rw_blur_up_fused' in msg, (rc, msg)
+    rc, msg = blur(_p(bnoise), _p(_offset_view(c.bias)))
+    assert rc == BAD_ARG and 'bias' in msg and '16-byte' in msg, (rc, msg)
     torch.cuda.synchronize()
-    for b, v in ((hi_buf, hi), (lo_buf, lo), (obuf, out)):
+    for b, v in ((hi_buf, hi), (lo_buf, lo), (obuf, out), (bhi_buf, bhi), (blo_buf, blo)):
         assert torch.isnan(v.float()).all() and _guard_intact(b)
 
     # the same buffers, aligned, are accepted

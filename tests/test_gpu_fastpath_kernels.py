@@ -98,10 +98,9 @@ def test_rgb_combine_vs_oracle_upsample(B, H, W, nparts, has_prev):
 @pytest.mark.parametrize('separable', [True, False])
 @pytest.mark.parametrize('B,C,H,W', [(2, 64, 4, 4), (1, 128, 5, 7), (3, 64, 16, 16), (2, 128, 33, 9),
                                      (2, 192, 20, 40)])
-def test_blur_up_fused_vs_layer_kernels(B, C, H, W, separable):
-    """both blur kernels — the generic one (fp32 NCHW output + planes) and the pipelined
-    persistent one the generation fast path launches (planes only; separable and 16-tap FIR) —
-    == blur_up_act on the NCHW conv_transpose output -> prep_keys"""
+def test_blur_up_pipelined_vs_layer_kernels(B, C, H, W, separable):
+    """the pipelined persistent blur the generation fast path launches (planes only; separable
+    and 16-tap FIR) == blur_up_act on the NCHW conv_transpose output -> prep_keys"""
     from rewriting_b200 import _cabi, ops
     torch.manual_seed(3)
     dev = 'cuda'
@@ -127,21 +126,17 @@ def test_blur_up_fused_vs_layer_kernels(B, C, H, W, separable):
     want = ops.blur_up_act(t, kern, noise, nw, bias, True)
     planes, _ = ops.prep_keys(want, nscale)
     ref = planes.hi.float() + planes.lo.float()
-    for with_y in (True, False):                          # generic kernel / pipelined kernel
-        nh = torch.full((rows_o, C), float('nan'), dtype=torch.bfloat16, device=dev)
-        nl = torch.full_like(nh, float('nan'))
-        y = torch.empty(B, C, Ho, Wo, device=dev) if with_y else None
-        _cabi.call('rw_blur_up_fused', ops._p(t_cl), B, C, H, W, ops._p(kern), ops._p(noise),
-                   noise.stride(0), ops._p(nw), ops._p(bias), 1, ops._p(nscale), ops._p(nh),
-                   ops._p(nl), ops._p(y), ops._stream())
-        if with_y:
-            assert (y - want).abs().max().item() < 1e-5 * max(1.0, want.abs().max().item())
-        got = nh.float() + nl.float()
-        assert torch.isfinite(got).all()                  # every row written, pads included
-        # hi + lo reconstructs each side to 2^-17 relative; the two sides may round differently
-        assert (got - ref).abs().max().item() < 3e-5 * max(1.0, ref.abs().max().item()), with_y
-        v = got.view(B, Ho + 1, Wo + 1, C)
-        assert v[:, Ho].abs().max() == 0 and v[:, :, Wo].abs().max() == 0   # pad row / column
+    nh = torch.full((rows_o, C), float('nan'), dtype=torch.bfloat16, device=dev)
+    nl = torch.full_like(nh, float('nan'))
+    _cabi.call('rw_blur_up_fused', ops._p(t_cl), B, C, H, W, ops._p(kern), ops._p(noise),
+               noise.stride(0), ops._p(nw), ops._p(bias), ops._p(nscale), ops._p(nh), ops._p(nl),
+               ops._stream())
+    got = nh.float() + nl.float()
+    assert torch.isfinite(got).all()                      # every row written, pads included
+    # hi + lo reconstructs each side to 2^-17 relative; the two sides may round differently
+    assert (got - ref).abs().max().item() < 3e-5 * max(1.0, ref.abs().max().item())
+    v = got.view(B, Ho + 1, Wo + 1, C)
+    assert v[:, Ho].abs().max() == 0 and v[:, :, Wo].abs().max() == 0   # pad row / column
 
 
 def _sym_then(cases, extra):

@@ -363,8 +363,7 @@ def _resolve(T, calls, i):
         name2, b = calls[i + 1]
         assert name2 == 'rw_blur_up_fused' and _ptr(b[0]) == _ptr(a[10]) and b[1:5] == (B, Cout, H, W)
         L.blur, L.noise, L.nw, L.bias = T(b[5], 4, 4), T(b[6]), T(b[8]), T(b[9], Cout)
-        assert b[10] == 1 and b[14] is None
-        L.ns_a, L.nh_a, L.nl_a = b[11], b[12], b[13]
+        L.ns_a, L.nh_a, L.nl_a = b[10], b[11], b[12]
         L.rgb_w = L.rgb_part = None
         L.Ho, L.Wo = 2 * H, 2 * W
     else:
@@ -604,7 +603,7 @@ def test_key_pass_b250_layer8(monkeypatch, cuda_model):
     meter.finish()
 
 
-def test_car512_b8(monkeypatch, car_model):
+def test_car512_b8_layer15_on_round1_pair(monkeypatch, car_model):
     """The 512² car model at B = 8: layer 15 on the round-1 pair (rw_modconv_up_fwd_cl ->
     pipelined rw_blur_up_fused), layer 16 on 64-column tiles, 23 style jobs."""
     import copy

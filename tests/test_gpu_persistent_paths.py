@@ -15,7 +15,7 @@ covering less:
   * the insert loops (`rw_insert_loop`, `_wide`, `_up` and their `rw_linear_*` twins) with
     Cout = 4 SMs + 6, so two CTAs take a second channel group and the last group has two channels;
     rank 32 and a batch of four; guard rows past Cout;
-  * the pipelined blur (`rw_blur_up_fused`, planes only) with every CTA taking two tiles or more
+  * the pipelined blur (`rw_blur_up_fused`) with every CTA taking two tiles or more
     and a ragged last round, separable and non-separable FIR;
   * the column GEMM's split-K with trailing splits that own no row block (`rw_conv_wgrad`,
     `rw_conv_up_wgrad`, `rw_second_moment_accum`).
@@ -419,8 +419,8 @@ def test_insert_wide_batch_of_four_vs_oracle():
 @pytest.mark.parametrize('separable,blur', [pytest.param(True, 'sym', id='True'),
                                             pytest.param(False, 'sym', id='False'),
                                             pytest.param(True, 't', id='True-t')])
-def test_blur_up_pipelined_every_cta_two_tiles_ragged_vs_fp64(separable, blur):
-    """rw_blur_up_fused with planes only takes the persistent, double-buffered kernel.  At B = 8,
+def test_blur_up_fused_every_cta_two_tiles_ragged_vs_fp64(separable, blur):
+    """rw_blur_up_fused runs the persistent, double-buffered kernel.  At B = 8,
     C = 128 and a 32x32 input there are 720 tiles of 8x16 outputs x 64 channels: every CTA runs at
     least two (so it prefetches into its second buffer) and the last round is ragged.  'sym' and
     't' take the separable branch; 't' changes under flips and transposition, so it also catches
@@ -457,8 +457,8 @@ def test_blur_up_pipelined_every_cta_two_tiles_ragged_vs_fp64(separable, blur):
     nh.fill_(float('nan'))
     nl.fill_(float('nan'))
     _cabi.call('rw_blur_up_fused', ops._p(t_cl), B, C, H, W, ops._p(kern_d), ops._p(noise),
-               noise.stride(0), ops._p(nw_d), ops._p(bias_d), 1, ops._p(ns_d), ops._p(nh),
-               ops._p(nl), None, ops._stream())
+               noise.stride(0), ops._p(nw_d), ops._p(bias_d), ops._p(ns_d), ops._p(nh),
+               ops._p(nl), ops._stream())
     torch.cuda.synchronize()
     assert _guard_intact(nh_buf, rows) and _guard_intact(nl_buf, rows)
     got = (nh.float() + nl.float()).view(B, Ho + 1, Wo + 1, C)

@@ -292,10 +292,10 @@ def test_seeded_vgg16_is_deterministic_and_leaves_the_rng_alone():
     assert not torch.equal(seeded_vgg16(seed=1).features[0].weight, a.features[0].weight)
 
 
-def test_up_fused_eligibility_matches_the_kernel_limits(monkeypatch):
+def test_up_fused_eligibility_is_the_one_routing_rule():
     """Shapes the one-kernel upsampling StyledConv takes (csrc/upconv_tc.cu: power-of-two square
-    inputs of width 4..128, Cin % 64 == 0, Cout % 16 == 0, rank-one 4x4 FIR); everything else —
-    and RW_UP_FUSED=0 — keeps the conv_transpose + blur pair."""
+    inputs of width 4..128, Cin % 64 == 0, Cout % 16 == 0, rank-one 4x4 FIR); everything else
+    keeps the conv_transpose + blur pair."""
     from rewriting_b200 import ops
     k1 = torch.tensor([1., 3., 3., 1.])
     sep = k1[:, None] * k1[None, :] / 16
@@ -309,5 +309,3 @@ def test_up_fused_eligibility_matches_the_kernel_limits(monkeypatch):
     nonsep = sep.clone()
     nonsep[1, 2] += 0.01
     assert not ops.up_fused_eligible(128, 32, 32, 32, nonsep)       # FIR not rank one
-    monkeypatch.setenv('RW_UP_FUSED', '0')
-    assert not ops.up_fused_eligible(512, 512, 4, 4, sep)
