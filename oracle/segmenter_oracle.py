@@ -195,6 +195,16 @@ SYNTH_LABELS = {
 }
 
 
+def wide_labels():
+    """A label set of the unified-parsing model's widths: 336 objects, 26 materials and 40 objects
+    with 6 parts each (the object head N = 384 rows padded, the part head 240 channels, N = 256)."""
+    objects = ['-', 'sky', 'building', 'person'] + ['obj%d' % i for i in range(332)]
+    owners = ['sky', 'building', 'person'] + ['obj%d' % i for i in range(37)]
+    return {'object': objects, 'material': ['-'] + ['mat%d' % i for i in range(25)],
+            'scene': ['-', 'a'], 'part': [],
+            'object_part': {o: ['%s-p%d' % (o, k) for k in range(6)] for o in owners}}
+
+
 def seeded_state_dicts(labeldata=SYNTH_LABELS, seed=2024, head_scale=6.0):
     """(encoder, decoder) state dicts of the deep-stem ResNet-50 / UPerNet (fpn_dim 512) with
     seeded weights: He-normal convs, batch norms near identity with the residual branch's last

@@ -35,7 +35,6 @@ from rewriting_b200 import ops                                      # noqa: E402
 from rewriting_b200.utils import (nethook, proggan, quickdissect, runningstats, segmenter,  # noqa: E402
                                   upsample, zdataset)
 from tools.bench_insert_wide import smi                              # noqa: E402
-from tools.bench_segmenter import wide_labels                        # noqa: E402
 
 KITCHEN_SIZES = [512, 512, 512, 512, 512, 256, 128, 64]
 
@@ -96,7 +95,7 @@ def main():
     gen = ppo.seeded_state_dict(lambda: proggan.ProgressiveGenerator(sizes=KITCHEN_SIZES))
     model = nethook.InstrumentedModel(gen).cuda().eval()
     model.retain_layer('layer4')
-    labels = wide_labels()
+    labels = so.wide_labels()
     enc, dec = so.seeded_state_dicts(labels)
     seg = segmenter.UnifiedParsingSegmenter(enc, dec, labels, segsizes=[256], segdiv='quad',
                                             all_parts=True)

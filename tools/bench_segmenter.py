@@ -34,14 +34,6 @@ from rewriting_b200.metrics import segmenter_net as snet   # noqa: E402
 from rewriting_b200.utils import segmenter as useg         # noqa: E402
 
 
-def wide_labels():
-    objects = ['-', 'sky', 'building', 'person'] + ['obj%d' % i for i in range(332)]
-    owners = ['sky', 'building', 'person'] + ['obj%d' % i for i in range(37)]
-    return {'object': objects, 'material': ['-'] + ['mat%d' % i for i in range(25)],
-            'scene': ['-', 'a'], 'part': [],
-            'object_part': {o: ['%s-p%d' % (o, k) for k in range(6)] for o in owners}}
-
-
 def torch_segment(sd, seg, img, size):
     """segment_batch's three channels from the network composed from torch ops (float32)."""
     x = (img + 1) / 2 * 255
@@ -122,7 +114,7 @@ def main():
         raise SystemExit('bench_segmenter: needs a CUDA device')
     gpu = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'],
                          capture_output=True, text=True).stdout.strip()
-    labels = wide_labels()
+    labels = so.wide_labels()
     enc, dec = so.seeded_state_dicts(labels)
     seg = useg.UnifiedParsingSegmenter(enc, dec, labels, segsizes=[256])
     sd = {k: v.detach().float().cuda() for k, v in list(enc.items()) + list(dec.items())}
