@@ -525,6 +525,44 @@ int rw_seg_classes(int nsizes, const float* const* logits, const int* map_hw, co
                    long long mat_offset, int B, int Ho, int Wo, float* probs, long long* labels,
                    rw_stream_t stream);
 
+/* ---- semantic (colour) segmenter (dilated ResNet-18 + PPMDeepsup): its passes between convs ----
+ * The same rules as the unified-parsing passes above (status, no allocation, no atomics, refusal
+ * before launch); the convolutions run on the same kernels.
+ * rw_seg_input_norm: as rw_seg_input, with the labels' image format: out[b,c] = the block mean of
+ *   ((x + 1) / 2 - mean[c]) / stdev[c], x image channel 2 - c when bgr = 1, else c.  mean, stdev:
+ *   host arrays of 3 floats, finite, stdev != 0.
+ * rw_seg_map_phase: rw_seg_map with phase-split source and destination.  Split by d (1..8), an
+ *   H x W map of B images is stored as d*d*B sub-images of ceil(H/d) x ceil(W/d): map pixel (y, x)
+ *   of image b is pixel (y / d, x / d) of sub-image ((y % d) * d + x % d) * B + b, in the layout
+ *   of the plain map (fp32 NCHW, padded rows or planes).  a is split by src_phase and res, out and
+ *   the planes by dst_phase; sub-image positions past the map are written as 0, which is the zero
+ *   padding of a dilation-d 3x3 conv run as the plain 3x3 conv over the d*d*B sub-images.  With
+ *   both phases 1 it is rw_seg_map, bit for bit.  dst_phase^2 * B <= 65535.
+ * rw_seg_avgpool: AdaptiveAvgPool2d(s) of x [B,C,H,W]: bin (i, j) covers rows floor(iH/s) ..
+ *   ceil((i+1)H/s) - 1 and likewise columns, summed in float row-major, divided by its height
+ *   then its width; out [B,C,s,s].
+ * rw_semseg_classes: the semantic head's class maps at Ho x Wo.  logits is a host array of nsizes
+ *   device pointers, each the class conv's padded rows [B*(h_s+1)*(w_s+1)][ld] without its bias
+ *   (device, [ncls]); map_hw the host array {h_0, w_0, ...}.  Per size, the logits + bias
+ *   bilinearly up-sampled (align_corners=False), p = softmax over the ncls (1..256) classes, then
+ *   per category q = softmax of p over the category's channels; q summed over the sizes.  The
+ *   categories (1..16) are host arrays: category k holds channels cat_chan[cat_start[k] ..
+ *   cat_start[k+1]) (every class exactly once), cat_label the label of each entry, cat_mask
+ *   {mask category or -1, index in it} per category.  probs [B,ncls,Ho,Wo] when not NULL.  labels
+ *   int64 [B,lchan,Ho,Wo] when not NULL: channel lcoff + k = offset + cat_label of category k's
+ *   argmax (the first maximum), or offset + 0 where category k has a mask and the argmax of the
+ *   mask category is not the mask index. */
+int rw_seg_input_norm(const void* im, int u8, int B, int H, int W, int S, const float* mean,
+                      const float* stdev, int bgr, float* out, rw_stream_t stream);
+int rw_seg_map_phase(const float* a, int a_cl, int src_phase, int B, int C, int Hin, int Win, int mode,
+                     int Ho, int Wo, const float* bias, const float* res, int relu, int dst_phase,
+                     void* out_hi, void* out_lo, int ldc, int coff, float* out, rw_stream_t stream);
+int rw_seg_avgpool(const float* x, int B, int C, int H, int W, int s, float* out, rw_stream_t stream);
+int rw_semseg_classes(int nsizes, const float* const* logits, const int* map_hw, const float* bias,
+                      int ld, int ncls, int ncat, const int* cat_start, const int* cat_chan,
+                      const int* cat_label, const int* cat_mask, int B, int Ho, int Wo, float* probs,
+                      long long* labels, int lchan, int lcoff, long long offset, rw_stream_t stream);
+
 /* ---- dissection: unit / label intersection counts (GAN dissection, utils/quickdissect) ----
  * Both calls up-sample a layer's activations act [B,U,h,w] fp32 to H x W as torch's grid_sample
  * with align_corners=True and padding_mode='zeros' does over an axis-affine grid: output (y, x)

@@ -99,6 +99,12 @@ SIGNATURES = {
     'rw_seg_prroi': (c_int, [c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p]),
     'rw_seg_classes': (c_int, [c_int, c_p, c_p, c_p, c_p, c_int, c_p, c_p, c_ll, c_int, c_int,
                                c_int, c_p, c_p, c_p]),
+    'rw_seg_input_norm': (c_int, [c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p, c_int, c_p, c_p]),
+    'rw_seg_map_phase': (c_int, [c_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                                 c_p, c_p, c_int, c_int, c_p, c_p, c_int, c_int, c_p, c_p]),
+    'rw_seg_avgpool': (c_int, [c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p]),
+    'rw_semseg_classes': (c_int, [c_int, c_p, c_p, c_p, c_int, c_int, c_int, c_p, c_p, c_p, c_p, c_int,
+                                  c_int, c_int, c_p, c_p, c_int, c_int, c_ll, c_p]),
     'rw_upsample_bilinear': (c_int, [c_p, c_int, c_int, c_int, c_int, c_int, c_int, c_d, c_d, c_d,
                                      c_d, c_p, c_p]),
     'rw_dissect_counts': (c_int, [c_p, c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int,

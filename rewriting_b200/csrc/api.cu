@@ -1117,6 +1117,31 @@ int rw_seg_classes(int nsizes, const float* const* logits, const int* map_hw, co
                             Ho, Wo, probs, labels, stream);
 }
 
+int rw_seg_input_norm(const void* im, int u8, int B, int H, int W, int S, const float* mean,
+                      const float* stdev, int bgr, float* out, rw_stream_t stream) {
+  return seg_input_norm_launch(im, u8, B, H, W, S, mean, stdev, bgr, out, stream);
+}
+
+int rw_seg_map_phase(const float* a, int a_cl, int src_phase, int B, int C, int Hin, int Win, int mode,
+                     int Ho, int Wo, const float* bias, const float* res, int relu, int dst_phase,
+                     void* out_hi, void* out_lo, int ldc, int coff, float* out, rw_stream_t stream) {
+  return seg_map_phase_launch(a, a_cl, src_phase, B, C, Hin, Win, mode, Ho, Wo, bias, res, relu,
+                              dst_phase, out_hi, out_lo, ldc, coff, out, stream);
+}
+
+int rw_seg_avgpool(const float* x, int B, int C, int H, int W, int s, float* out, rw_stream_t stream) {
+  return seg_avgpool_launch(x, B, C, H, W, s, out, stream);
+}
+
+int rw_semseg_classes(int nsizes, const float* const* logits, const int* map_hw, const float* bias,
+                      int ld, int ncls, int ncat, const int* cat_start, const int* cat_chan,
+                      const int* cat_label, const int* cat_mask, int B, int Ho, int Wo, float* probs,
+                      long long* labels, int lchan, int lcoff, long long offset, rw_stream_t stream) {
+  return semseg_classes_launch(nsizes, logits, map_hw, bias, ld, ncls, ncat, cat_start, cat_chan,
+                               cat_label, cat_mask, B, Ho, Wo, probs, labels, lchan, lcoff, offset,
+                               stream);
+}
+
 int rw_upsample_bilinear(const float* act, int B, int U, int h, int w, int H, int W, double sy,
                          double oy, double sx, double ox, float* rows, rw_stream_t stream) {
   return upsample_bilinear_launch(act, B, U, h, w, H, W, sy, oy, sx, ox, rows, stream);

@@ -295,12 +295,23 @@ int seg_input_launch(const void* im, int u8, int B, int H, int W, int S, float* 
 int seg_map_launch(const float* a, int a_cl, int B, int C, int Hin, int Win, int mode, int Ho, int Wo,
                    const float* bias, const float* res, int relu, void* hi, void* lo, int ldc,
                    int coff, float* out, cudaStream_t stream);
+int seg_input_norm_launch(const void* im, int u8, int B, int H, int W, int S, const float* mean,
+                          const float* stdev, int bgr, float* out, cudaStream_t stream);
+int seg_map_phase_launch(const float* a, int a_cl, int sd, int B, int C, int Hin, int Win, int mode,
+                         int Ho, int Wo, const float* bias, const float* res, int relu, int dd,
+                         void* hi, void* lo, int ldc, int coff, float* out, cudaStream_t stream);
 int seg_maxpool_launch(const float* x, int B, int C, int H, int W, float* out, cudaStream_t stream);
+int seg_avgpool_launch(const float* x, int B, int C, int H, int W, int s, float* out, cudaStream_t stream);
 int seg_prroi_launch(const float* x, int B, int C, int H, int W, int s, float* out, cudaStream_t stream);
 int seg_classes_launch(int nsizes, const float* const* logits, const int* map_hw, const float* const* bias,
                        const int* ld, int ngroups, const int* groups, const long long* trans,
                        long long mat_offset, int B, int Ho, int Wo, float* probs, long long* labels,
                        cudaStream_t stream);
+int semseg_classes_launch(int nsizes, const float* const* logits, const int* map_hw, const float* bias,
+                          int ld, int ncls, int ncat, const int* cat_start, const int* cat_chan,
+                          const int* cat_label, const int* cat_mask, int B, int Ho, int Wo,
+                          float* probs, long long* labels, int lchan, int lcoff, long long offset,
+                          cudaStream_t stream);
 
 // ---------------------------------------------------------------------------
 // dissection statistics (dissect.cu)

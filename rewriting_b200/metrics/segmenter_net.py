@@ -1,5 +1,7 @@
-"""The unified-parsing segmenter's network (reference utils/upsegmodel/: the deep-stem ResNet-50
-encoder and the UPerNet decoder) as a forward-only launch sequence on the package's kernels.
+"""The segmenters' networks as forward-only launch sequences on the package's kernels: the
+unified-parsing one (reference utils/upsegmodel/: the deep-stem ResNet-50 encoder and the UPerNet
+decoder) and the semantic colour one (utils/segmodel/: the deep-stem ResNet-18 dilated to 1/8 and
+the PPMDeepsup decoder).  Both share the stem, the folded convs and their launch helpers.
 
 Every batch norm is an affine map at inference; it is folded into its conv's weight and a bias once
 per state dict, and the weight planes are formed then too.  Per layer:
@@ -15,6 +17,14 @@ per state dict, and the weight planes are formed then too.  Per layer:
     `rw_seg_maxpool`, PrRoI pooling in `rw_seg_prroi` and the class maps in `rw_seg_classes`
     (csrc/seg.cu).
 The scene head is not run: segment_batch never reads it.
+
+The semantic network's dilated 3x3 convs (dilation 2 in layer3, 4 in layer4) run on conv_tc as
+plain 3x3 convs over phase-split maps: a dilation-d conv on an H x W map is the plain conv on each
+of the d*d sub-grids {y = i, x = j mod d}, each padded to ceil(H/d) x ceil(W/d) with zeros, which are
+the conv's own zero padding.  `rw_seg_map_phase` writes the planes in that order and reads them back,
+so only the map passes where d changes reshuffle, and conv_tc is unchanged.  Its PPM average-pools
+with `rw_seg_avgpool` and its class maps come from `rw_semseg_classes`.  The deep-supervision branch
+is not run at inference.
 """
 import ctypes
 
@@ -28,6 +38,12 @@ PLANES = (64, 128, 256, 512)
 POOL_SCALES = (1, 2, 3, 6)
 FPN_DIM = 512
 HEADS = ('object', 'part', 'material')
+# the semantic network: ResNet-18's two BasicBlocks per layer, and with dilate_scale 8 the
+# (conv1, conv2) dilation of each block (the reference's _nostride_dilate: a conv that had stride 2
+# gets half the layer's dilation)
+SEM_PLANES = (64, 128, 256, 512)
+SEM_DILATIONS = (((1, 1), (1, 1)), ((1, 1), (1, 1)), ((1, 2), (2, 2)), ((2, 4), (4, 4)))
+SEM_FC_DIM = 512
 
 
 def _fail(msg):
@@ -90,44 +106,124 @@ class _Conv(object):
                        ops._p(self.lo), ops._stream())
 
 
-def _planes(B, C, H, W, device):
-    hi = torch.empty((B * (H + 1) * (W + 1), C), dtype=torch.bfloat16, device=device)
+def _planes(B, C, H, W, device, d=1):
+    """Planes of B images of H x W, or phase-split by d: d*d*B sub-images of ceil(H/d) x ceil(W/d)."""
+    hi = torch.empty((d * d * B * (-(-H // d) + 1) * (-(-W // d) + 1), C), dtype=torch.bfloat16,
+                     device=device)
     return hi, torch.empty_like(hi)
 
 
 def seg_map(a, a_cl, B, C, Hin, Win, mode=0, Ho=None, Wo=None, bias=None, res=None, relu=False,
-            planes=None, ldc=None, coff=0, fp32=False):
-    """rw_seg_map: returns the fp32 NCHW output when `fp32`, else None; `planes` (hi, lo) are
+            planes=None, ldc=None, coff=0, fp32=False, src_phase=1, dst_phase=1):
+    """rw_seg_map, or rw_seg_map_phase when a phase is not 1: returns the fp32 NCHW output when
+    `fp32` ([d*d*B, C, ceil(Ho/d), ceil(Wo/d)] for dst_phase d), else None; `planes` (hi, lo) are
     written in place (channel slice coff..coff+C-1 of row length ldc)."""
     if mode == 0:
         Ho, Wo = Hin, Win
     elif mode == 1:
         Ho, Wo = (Hin + 1) // 2, (Win + 1) // 2
-    out = torch.empty((B, C, Ho, Wo), dtype=torch.float32, device=a.device) if fp32 else None
+    d = dst_phase
+    out = (torch.empty((d * d * B, C, -(-Ho // d), -(-Wo // d)), dtype=torch.float32, device=a.device)
+           if fp32 else None)
     hi, lo = planes if planes is not None else (None, None)
-    _cabi.call('rw_seg_map', ops._p(a), 1 if a_cl else 0, B, C, Hin, Win, mode, Ho, Wo, ops._p(bias),
-               ops._p(res), 1 if relu else 0, ops._p(hi), ops._p(lo), ldc or C, coff, ops._p(out),
-               ops._stream())
+    if src_phase == d == 1:
+        _cabi.call('rw_seg_map', ops._p(a), 1 if a_cl else 0, B, C, Hin, Win, mode, Ho, Wo,
+                   ops._p(bias), ops._p(res), 1 if relu else 0, ops._p(hi), ops._p(lo), ldc or C, coff,
+                   ops._p(out), ops._stream())
+    else:
+        _cabi.call('rw_seg_map_phase', ops._p(a), 1 if a_cl else 0, src_phase, B, C, Hin, Win, mode,
+                   Ho, Wo, ops._p(bias), ops._p(res), 1 if relu else 0, d, ops._p(hi), ops._p(lo),
+                   ldc or C, coff, ops._p(out), ops._stream())
     return out
 
 
-class SegmenterNet(object):
+def unphase(x, B, H, W, d):
+    """The plain [B,C,H,W] map of a phase-split fp32 map [d*d*B, C, ceil(H/d), ceil(W/d)]."""
+    if d == 1:
+        return x
+    C, hs, ws = x.shape[1:]
+    v = x.reshape(d, d, B, C, hs, ws).permute(2, 3, 4, 0, 5, 1).reshape(B, C, hs * d, ws * d)
+    return v[:, :, :H, :W]
+
+
+class _FoldedNet(object):
+    """What both segmenter networks share: the device, BN folding into `_Conv`s, the deep stem
+    and the conv launch helpers."""
+
+    def __init__(self, device):
+        self.device = torch.device(device)
+        if self.device.type == 'cuda' and self.device.index is None:
+            self.device = torch.device('cuda', torch.cuda.current_device())
+
+    def conv_bn(self, sd, wkey, bnkey, kind):
+        return _Conv(kind, *fold_bn(_get(sd, wkey), _bn(sd, bnkey)), device=self.device)
+
+    def _fold_stem(self, enc):
+        self.stem = [self.conv_bn(enc, 'conv1.weight', 'bn1.', 'stem'),
+                     self.conv_bn(enc, 'conv2.weight', 'bn2.', '3x3'),
+                     self.conv_bn(enc, 'conv3.weight', 'bn3.', '3x3')]
+
+    def _stem_ok(self):
+        c = self.stem
+        return c[0].cin == 3 and c[0].cout == 64 and c[1].cin == 64 and c[2].cout == 128
+
+    def _conv3x3(self, cv, planes, B, H, W):
+        a = torch.empty((B, cv.cout, H, W), dtype=torch.float32, device=planes[0].device)
+        _cabi.call('rw_conv3x3_bias_act', ops._p(planes[0]), ops._p(planes[1]), ops._p(cv.hi),
+                   ops._p(cv.lo), ops._p(cv.bias), 0, 1.0, B, cv.cin, cv.cout, H, W, ops._p(a),
+                   ops._stream())
+        return a
+
+    def _conv1x1(self, cv, planes, B, H, W):
+        """Channels-last padded rows [B*(H+1)*(W+1)][N] (no bias)."""
+        rows = B * (H + 1) * (W + 1)
+        out = torch.empty((rows, cv.w.shape[0]), dtype=torch.float32, device=planes[0].device)
+        _cabi.call('rw_rowgemm', ops._p(planes[0]), ops._p(planes[1]), ops._p(cv.hi), ops._p(cv.lo),
+                   rows, cv.cin, cv.w.shape[0], ops._p(out), ops._stream())
+        return out
+
+    def _relu_planes(self, a, B, C, H, W, fp32=False):
+        planes = _planes(B, C, H, W, a.device)
+        out = torch.empty_like(a) if fp32 else None
+        _cabi.call('rw_relu_pool', ops._p(a), None, B, C, H, W, 0, ops._p(planes[0]),
+                   ops._p(planes[1]), ops._p(out), ops._stream())
+        return planes, out
+
+    def stem_forward(self, x):
+        """(planes, fp32 NCHW, H, W) of the deep stem and max pool on x [B,3,H,W]."""
+        B, _, H, W = x.shape
+        d = x.device
+        c1, c2, c3 = self.stem
+        a = torch.empty((B, 64, H, W), dtype=torch.float32, device=d)
+        _cabi.call('rw_narrow_conv3x3', ops._p(x), ops._p(c1.w), None, 1.0, B, 3, 64, H, W,
+                   ops._p(a), ops._stream())
+        H0, W0 = H, W
+        H, W = (H + 1) // 2, (W + 1) // 2
+        P = _planes(B, 64, H, W, d)
+        seg_map(a, False, B, 64, H0, W0, mode=1, bias=c1.bias, relu=True, planes=P)
+        P = self._relu_planes(self._conv3x3(c2, P, B, H, W), B, 64, H, W)[0]
+        _, r = self._relu_planes(self._conv3x3(c3, P, B, H, W), B, 128, H, W, fp32=True)
+        Ho, Wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1
+        xf = torch.empty((B, 128, Ho, Wo), dtype=torch.float32, device=d)
+        _cabi.call('rw_seg_maxpool', ops._p(r), B, 128, H, W, ops._p(xf), ops._stream())
+        del r
+        H, W = Ho, Wo
+        X = _planes(B, 128, H, W, d)
+        seg_map(xf, False, B, 128, H, W, planes=X)
+        return X, xf, H, W
+
+
+class SegmenterNet(_FoldedNet):
     """The folded network of one (encoder, decoder) state-dict pair on one device.  `n_part` is
     the part head's width (the sum of the part-group sizes)."""
 
     def __init__(self, encoder_sd, decoder_sd, n_object, n_part, n_material, device):
+        super().__init__(device)
         enc, dec = _strip(encoder_sd), _strip(decoder_sd)
-        self.device = torch.device(device)
-        if self.device.type == 'cuda' and self.device.index is None:
-            self.device = torch.device('cuda', torch.cuda.current_device())
         self.n = {'object': n_object, 'part': n_part, 'material': n_material}
         d = self.device
-
-        def conv_bn(sd, wkey, bnkey, kind):
-            return _Conv(kind, *fold_bn(_get(sd, wkey), _bn(sd, bnkey)), device=d)
-        self.stem = [conv_bn(enc, 'conv1.weight', 'bn1.', 'stem'),
-                     conv_bn(enc, 'conv2.weight', 'bn2.', '3x3'),
-                     conv_bn(enc, 'conv3.weight', 'bn3.', '3x3')]
+        conv_bn = self.conv_bn
+        self._fold_stem(enc)
         self.layers = []
         for li, (nb, p) in enumerate(zip(LAYERS, PLANES)):
             blocks = []
@@ -163,8 +259,7 @@ class SegmenterNet(object):
         self.check_shapes()
 
     def check_shapes(self):
-        c = self.stem
-        if c[0].cin != 3 or c[0].cout != 64 or c[1].cin != 64 or c[2].cout != 128:
+        if not self._stem_ok():
             _fail('segmenter: the encoder is not the deep-stem ResNet-50')
         cin = 128
         for blocks, p in zip(self.layers, PLANES):
@@ -178,28 +273,6 @@ class SegmenterNet(object):
             _fail('segmenter: the decoder is not UPerNet with fpn_dim 512')
 
     # ------------------------------------------------------------------ layers
-    def _conv3x3(self, cv, planes, B, H, W):
-        a = torch.empty((B, cv.cout, H, W), dtype=torch.float32, device=planes[0].device)
-        _cabi.call('rw_conv3x3_bias_act', ops._p(planes[0]), ops._p(planes[1]), ops._p(cv.hi),
-                   ops._p(cv.lo), ops._p(cv.bias), 0, 1.0, B, cv.cin, cv.cout, H, W, ops._p(a),
-                   ops._stream())
-        return a
-
-    def _conv1x1(self, cv, planes, B, H, W):
-        """Channels-last padded rows [B*(H+1)*(W+1)][N] (no bias)."""
-        rows = B * (H + 1) * (W + 1)
-        out = torch.empty((rows, cv.w.shape[0]), dtype=torch.float32, device=planes[0].device)
-        _cabi.call('rw_rowgemm', ops._p(planes[0]), ops._p(planes[1]), ops._p(cv.hi), ops._p(cv.lo),
-                   rows, cv.cin, cv.w.shape[0], ops._p(out), ops._stream())
-        return out
-
-    def _relu_planes(self, a, B, C, H, W, fp32=False):
-        planes = _planes(B, C, H, W, a.device)
-        out = torch.empty_like(a) if fp32 else None
-        _cabi.call('rw_relu_pool', ops._p(a), None, B, C, H, W, 0, ops._p(planes[0]),
-                   ops._p(planes[1]), ops._p(out), ops._stream())
-        return planes, out
-
     def _bottleneck(self, blk, X, xf, B, H, W):
         """(planes, fp32) of the block output and its size, from the input planes X / fp32 xf."""
         c1, c2, c3, ds = blk['c1'], blk['c2'], blk['c3'], blk['ds']
@@ -233,25 +306,8 @@ class SegmenterNet(object):
     def encoder(self, x):
         """The four layer outputs [(planes, fp32 NCHW, H, W)] of x [B,3,H,W] (the input pass's
         output)."""
-        B, _, H, W = x.shape
-        d = x.device
-        c1, c2, c3 = self.stem
-        a = torch.empty((B, 64, H, W), dtype=torch.float32, device=d)
-        _cabi.call('rw_narrow_conv3x3', ops._p(x), ops._p(c1.w), None, 1.0, B, 3, 64, H, W,
-                   ops._p(a), ops._stream())
-        H0, W0 = H, W
-        H, W = (H + 1) // 2, (W + 1) // 2
-        P = _planes(B, 64, H, W, d)
-        seg_map(a, False, B, 64, H0, W0, mode=1, bias=c1.bias, relu=True, planes=P)
-        P = self._relu_planes(self._conv3x3(c2, P, B, H, W), B, 64, H, W)[0]
-        _, r = self._relu_planes(self._conv3x3(c3, P, B, H, W), B, 128, H, W, fp32=True)
-        Ho, Wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1
-        xf = torch.empty((B, 128, Ho, Wo), dtype=torch.float32, device=d)
-        _cabi.call('rw_seg_maxpool', ops._p(r), B, 128, H, W, ops._p(xf), ops._stream())
-        del r
-        H, W = Ho, Wo
-        X = _planes(B, 128, H, W, d)
-        seg_map(xf, False, B, 128, H, W, planes=X)
+        B = x.shape[0]
+        X, xf, H, W = self.stem_forward(x)
         taps = []
         for blocks in self.layers:
             for blk in blocks:
@@ -335,6 +391,167 @@ class SegmenterNet(object):
                    ops._p(trans), int(mat_offset), B, Ho, Wo, ops._p(probs), ops._p(labels),
                    ops._stream())
         return probs, labels
+
+
+class SemanticNet(_FoldedNet):
+    """The folded semantic segmenter network (reference utils/segmodel/: ResnetDilated over the
+    deep-stem ResNet-18 with dilate_scale 8, PPMDeepsup with fc_dim 512) of one (encoder, decoder)
+    state-dict pair with `n_class` classes, on one device."""
+
+    def __init__(self, encoder_sd, decoder_sd, n_class, device):
+        super().__init__(device)
+        enc, dec = _strip(encoder_sd), _strip(decoder_sd)
+        conv_bn = self.conv_bn
+        self._fold_stem(enc)
+        self.layers = []
+        for li, (p, dil) in enumerate(zip(SEM_PLANES, SEM_DILATIONS)):
+            blocks = []
+            for bi, dl in enumerate(dil):
+                pre = 'layer%d.%d.' % (li + 1, bi)
+                ds = None
+                if pre + 'downsample.0.weight' in enc:
+                    ds = conv_bn(enc, pre + 'downsample.0.weight', pre + 'downsample.1.', '1x1')
+                blocks.append({'stride': 2 if (li == 1 and bi == 0) else 1, 'dil': dl,
+                               'c1': conv_bn(enc, pre + 'conv1.weight', pre + 'bn1.', '3x3'),
+                               'c2': conv_bn(enc, pre + 'conv2.weight', pre + 'bn2.', '3x3'),
+                               'ds': ds})
+            self.layers.append(blocks)
+        self.ppm = [conv_bn(dec, 'ppm.%d.1.weight' % i, 'ppm.%d.2.' % i, '1x1')
+                    for i in range(len(POOL_SCALES))]
+        self.last = conv_bn(dec, 'conv_last.0.weight', 'conv_last.1.', '3x3')
+        w = torch.as_tensor(_get(dec, 'conv_last.4.weight')).detach().float()
+        if w.shape[0] != n_class:
+            _fail('segmenter: conv_last has %d classes, the labels give %d' % (w.shape[0], n_class))
+        self.n_class = n_class
+        self.cls = _Conv('1x1', w, torch.as_tensor(_get(dec, 'conv_last.4.bias')).detach().float(),
+                         self.device, npad=(n_class + 63) // 64 * 64)
+        self.check_shapes()
+
+    def check_shapes(self):
+        ok = self._stem_ok()
+        cin = 128
+        for blocks, p in zip(self.layers, SEM_PLANES):
+            for bi, blk in enumerate(blocks):
+                need_ds = cin != p or blk['stride'] == 2
+                ds = blk['ds']
+                ok = ok and (blk['c1'].cin == cin and blk['c1'].cout == p and blk['c2'].cin == p and
+                             blk['c2'].cout == p and (ds is not None) == need_ds and
+                             (ds is None or (ds.cin == cin and ds.cout == p)))
+                cin = p
+        ok = ok and all(cv.cin == SEM_FC_DIM and cv.cout == 512 for cv in self.ppm)
+        ok = ok and self.last.cin == SEM_FC_DIM + 512 * len(POOL_SCALES) and self.last.cout == 512
+        ok = ok and self.cls.cin == 512
+        if not ok:
+            _fail('segmenter: the colour network is not the deep-stem ResNet-18 dilated / PPMDeepsup '
+                  'with fc_dim 512')
+
+    def _basic(self, blk, X, xf, din, B, H, W):
+        """(planes, fp32, phase, H, W) of a BasicBlock's output from its input planes X / fp32 xf,
+        both phase-split by din (which is the block's conv1 dilation)."""
+        c1, c2, ds = blk['c1'], blk['c2'], blk['ds']
+        d1, d2 = blk['dil']
+        s = blk['stride']
+        dev = xf.device
+        a = self._conv3x3(c1, X, d1 * d1 * B, -(-H // d1), -(-W // d1))
+        Ho, Wo = ((H + 1) // 2, (W + 1) // 2) if s == 2 else (H, W)
+        P1 = _planes(B, c1.cout, Ho, Wo, dev, d2)
+        seg_map(a, False, B, c1.cout, H, W, mode=1 if s == 2 else 0, relu=True, planes=P1,
+                src_phase=d1, dst_phase=d2)
+        del a
+        a = self._conv3x3(c2, P1, d2 * d2 * B, -(-Ho // d2), -(-Wo // d2))
+        if ds is not None:
+            Xs, Hs, Ws = X, -(-H // din), -(-W // din)
+            if s == 2:
+                Xs, Hs, Ws = _planes(B, ds.cin, Ho, Wo, dev), Ho, Wo
+                seg_map(xf, False, B, ds.cin, H, W, mode=1, planes=Xs)
+            r = seg_map(self._conv1x1(ds, Xs, din * din * B, Hs, Ws), True, B, ds.cout, Ho, Wo,
+                        bias=ds.bias, fp32=True, src_phase=din if s == 1 else 1, dst_phase=d2)
+        else:
+            r = xf
+        Y = _planes(B, c2.cout, Ho, Wo, dev, d2)
+        y = seg_map(a, False, B, c2.cout, Ho, Wo, res=r, relu=True, planes=Y, fp32=True,
+                    src_phase=d2, dst_phase=d2)
+        return Y, y, d2, Ho, Wo
+
+    def encoder(self, x):
+        """The four layer outputs [(planes, fp32, phase, H, W)] of x [B,3,H,W] (the input pass's
+        output); layer3 is phase-split by 2 and layer4 by 4 (`unphase` gives the plain maps)."""
+        B = x.shape[0]
+        X, xf, H, W = self.stem_forward(x)
+        d = 1
+        taps = []
+        for blocks in self.layers:
+            for blk in blocks:
+                X, xf, d, H, W = self._basic(blk, X, xf, d, B, H, W)
+            taps.append((X, xf, d, H, W))
+        return taps
+
+    def decoder(self, taps, keep=False):
+        """(class logits as padded rows [B*(h+1)*(w+1)][n_class padded to 64] without their bias,
+        (h, w)); with `keep` also {'conv5': fp32, 'concat': planes, 'last': fp32} of the PPM."""
+        X4, c5, d4, h, w = taps[3]
+        B = c5.shape[0] // (d4 * d4)
+        dev = c5.device
+        nppm = SEM_FC_DIM + 512 * len(POOL_SCALES)
+        Pc = _planes(B, nppm, h, w, dev)
+        conv5 = seg_map(c5, False, B, SEM_FC_DIM, h, w, planes=Pc, ldc=nppm, coff=0, fp32=True,
+                        src_phase=d4)
+        for i, (s, cv) in enumerate(zip(POOL_SCALES, self.ppm)):
+            pooled = torch.empty((B, SEM_FC_DIM, s, s), dtype=torch.float32, device=dev)
+            _cabi.call('rw_seg_avgpool', ops._p(conv5), B, SEM_FC_DIM, h, w, s, ops._p(pooled),
+                       ops._stream())
+            Pp = _planes(B, SEM_FC_DIM, s, s, dev)
+            seg_map(pooled, False, B, SEM_FC_DIM, s, s, planes=Pp)
+            # the reference's conv, BN and ReLU act on the s x s pooled map, then it is resized
+            t = seg_map(self._conv1x1(cv, Pp, B, s, s), True, B, 512, s, s, bias=cv.bias, relu=True,
+                        fp32=True)
+            seg_map(t, False, B, 512, s, s, mode=2, Ho=h, Wo=w, planes=Pc, ldc=nppm,
+                    coff=SEM_FC_DIM + 512 * i)
+        Pl, last = self._relu_planes(self._conv3x3(self.last, Pc, B, h, w), B, 512, h, w, fp32=keep)
+        logits = self._conv1x1(self.cls, Pl, B, h, w)
+        if keep:
+            return logits, (h, w), {'conv5': conv5, 'concat': Pc, 'last': last}
+        return logits, (h, w)
+
+    def classes(self, logits_per_size, B, Ho, Wo, cats, want_probs, labels=None, lcoff=0, offset=0):
+        """rw_semseg_classes over the sizes' logits ([(rows, (h, w))]).  cats: [(channels, labels,
+        mask category or -1, mask index)] per category.  Labels go to channels lcoff.. of `labels`
+        (int64 [B, L, Ho, Wo]) with `offset` added; returns the probabilities [B,n_class,Ho,Wo] or
+        None."""
+        ns = len(logits_per_size)
+        ptrs = (ctypes.c_void_p * ns)(*[lg.data_ptr() for lg, _ in logits_per_size])
+        hw = (ctypes.c_int * (2 * ns))(*[v for _, s in logits_per_size for v in s])
+        start, chan, lab, mask = [0], [], [], []
+        for ch, lb, mc, mi in cats:
+            chan += ch
+            lab += lb
+            start.append(len(chan))
+            mask += [mc, mi]
+        arr = [(ctypes.c_int * len(v))(*v) for v in (start, chan, lab, mask)]
+        probs = (torch.empty((B, self.n_class, Ho, Wo), dtype=torch.float32, device=self.device)
+                 if want_probs else None)
+        _cabi.call('rw_semseg_classes', ns, ctypes.cast(ptrs, ctypes.c_void_p),
+                   ctypes.cast(hw, ctypes.c_void_p), ops._p(self.cls.bias), self.cls.w.shape[0],
+                   self.n_class, len(cats), *[ctypes.cast(a, ctypes.c_void_p) for a in arr], B, Ho, Wo,
+                   ops._p(probs), ops._p(labels), 0 if labels is None else labels.shape[1], lcoff,
+                   int(offset), ops._stream())
+        return probs
+
+
+def input_pass_norm(images, u8, size, mean, stdev, bgr):
+    """rw_seg_input_norm: ((x + 1) / 2 - mean) / stdev per channel (reversed when `bgr`),
+    [B,3,size,size], from fp32 NCHW or uint8 NHWC images."""
+    if u8:
+        B, H, W, _ = images.shape
+    else:
+        B, _, H, W = images.shape
+    out = torch.empty((B, 3, size, size), dtype=torch.float32, device=images.device)
+    m = (ctypes.c_float * 3)(*mean)
+    sd = (ctypes.c_float * 3)(*stdev)
+    _cabi.call('rw_seg_input_norm', ops._p(images), int(u8), B, H, W, size,
+               ctypes.cast(m, ctypes.c_void_p), ctypes.cast(sd, ctypes.c_void_p), 1 if bgr else 0,
+               ops._p(out), ops._stream())
+    return out
 
 
 def input_pass(images, u8, size):

@@ -3,7 +3,8 @@ units of a layer fire on which segmentation labels, by IoU, as the paper's refle
 reads them (`DissectVis(model='kitchen').top_units('layer4', 'window', 20)`).
 
     python -m rewriting_b200.utils.quickdissect --model kitchen --layer layer4 \\
-        --model_path kitchen.pth --segmodel_dir <dir with labels.json, encoder/decoder .pth>
+        --model_path kitchen.pth --segmodel_dir <dir with labels.json, encoder/decoder .pth> \\
+        [--colordir <the colour segmenter's dir: labels.json, encoder/decoder_epoch_<N>.pth>]
 
 writes <outdir>/<model>/<layer>/<seg>/<sample_size>/ with the reference's files: rq.npz (the
 layer's quantiles over the up-sampled activations), iou.npy ([units, labels seen + 1]),
@@ -135,12 +136,17 @@ def main(argv=None):
                         help='the ProgGAN generator (.pth state dict)')
     parser.add_argument('--segmodel_dir', type=str, required=True,
                         help='labels.json, encoder_epoch_40.pth and decoder_epoch_40.pth')
+    parser.add_argument('--colordir', type=str, default=None,
+                        help="the colour segmenter's labels.json and encoder_epoch_<N>.pth / "
+                             "decoder_epoch_<N>.pth, merged after the unified labels when --seg "
+                             "has a 'c'")
     parser.add_argument('--batch_size', type=int, default=32)
     args = parser.parse_args(argv)
     dirname = os.path.join(args.outdir, args.model, args.layer, args.seg, str(args.sample_size))
     model = nethook.InstrumentedModel(proggan.from_pth_file(args.model_path)).cuda().eval()
     zds = zdataset.z_dataset_for_model(model, size=args.sample_size, seed=1)
-    segmodel, seglabels = segmenter.load_segmenter(args.seg, modeldir=args.segmodel_dir)
+    segmodel, seglabels = segmenter.load_segmenter(args.seg, modeldir=args.segmodel_dir,
+                                                   colordir=args.colordir)
     dissect(model, args.layer, zds, segmodel, seglabels, dirname, batch_size=args.batch_size)
 
 

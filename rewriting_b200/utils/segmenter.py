@@ -1,12 +1,16 @@
-"""The unified-parsing segmenter of the reference (utils/segmenter.py:16-41, 150-389) on the
-package's kernels: a ResNet-50 / UPerNet network (metrics/segmenter_net.py, csrc/seg.cu) with the
-reference's label numbering, part translation and 'quad' subdivision.
+"""The segmenters of the reference (utils/segmenter.py) on the package's kernels: the
+unified-parsing ResNet-50 / UPerNet (segmenter.py:150-389) with the reference's label numbering,
+part translation and 'quad' subdivision; the semantic colour segmenter, a dilated ResNet-18 /
+PPMDeepsup (segmenter.py:392-574); and MergedSegmenter (segmenter.py:82-113), which appends the
+colour labels after the unified-parsing ones, as load_segmenter('netpqc') does.  The networks are in
+metrics/segmenter_net.py and their passes in csrc/seg.cu.
 
 The weights and the label data are arguments (nothing is downloaded); `load_segmenter` reads them
-from the reference's directory layout.  Only the unified-parsing part of a name is built: the colour
-and texture segmenters ('c', 'x') are not provided, and a name that asks for them says so.  The
-network runs forward only, on CUDA tensors; there is no CPU path.
+from the reference's directory layout.  The colour segmenter ('c') is built when its directory is
+given; the texture segmenter ('x') is not provided, and a name that asks for it says so.  The
+networks run forward only, on CUDA tensors; there is no CPU path.
 """
+import glob
 import json
 import os
 import warnings
@@ -24,14 +28,21 @@ def _fail(msg):
     raise _cabi.RwError(msg)
 
 
-def load_segmenter(segmenter_name='netpqc', modeldir=None):
+def load_segmenter(segmenter_name='netpqc', modeldir=None, colordir=None):
     """(segmenter, labels) as the reference's load_segmenter returns them, from `modeldir` holding
-    labels.json, encoder_epoch_40.pth and decoder_epoch_40.pth."""
+    labels.json, encoder_epoch_40.pth and decoder_epoch_40.pth.  With 'c' in the name and
+    `colordir` (labels.json and encoder_epoch_<N>.pth / decoder_epoch_<N>.pth, the highest N taken)
+    the colour segmenter is merged after the unified-parsing one; without `colordir` only the
+    unified-parsing segmenter is built, with a warning."""
     all_parts = 'p' in segmenter_name
     quad_seg = 'q' in segmenter_name
-    if 'x' in segmenter_name or 'c' in segmenter_name:
+    colors = 'c' in segmenter_name and colordir is not None
+    if ('x' in segmenter_name or 'c' in segmenter_name) and not colors:
         warnings.warn('load_segmenter(%r): the colour / texture segmenters are not provided; '
                       'only the unified-parsing segmenter is built' % (segmenter_name,))
+    elif 'x' in segmenter_name:
+        warnings.warn('load_segmenter(%r): the texture segmenter is not provided; the unified-parsing '
+                      'and colour segmenters are built' % (segmenter_name,))
     if modeldir is None:
         _fail('load_segmenter: pass modeldir=, the directory with labels.json, encoder_epoch_40.pth '
               'and decoder_epoch_40.pth')
@@ -46,8 +57,31 @@ def load_segmenter(segmenter_name='netpqc', modeldir=None):
     dec = torch.load(files[2], map_location='cpu')
     segmodel = UnifiedParsingSegmenter(enc, dec, labeldata, segsizes=[256], all_parts=all_parts,
                                        segdiv=('quad' if quad_seg else None))
+    if colors:
+        segmodel = MergedSegmenter([segmodel, SemanticSegmenter(*load_semantic_model(colordir))])
     seglabels = [l for l, c in segmodel.get_label_and_category_names()[0]]
     return segmodel, seglabels
+
+
+def load_semantic_model(modeldir):
+    """(encoder state dict, decoder state dict, label data) of a semantic segmenter directory:
+    labels.json and encoder_epoch_<N>.pth / decoder_epoch_<N>.pth with N the highest epoch of the
+    encoder files, as the reference's load_segmentation_model picks it."""
+    lj = os.path.join(modeldir, 'labels.json')
+    epochs = [os.path.basename(n)[14:-4] for n in
+              glob.glob(os.path.join(modeldir, 'encoder_epoch_*.pth'))]
+    epochs = [int(e) for e in epochs if e.isdigit()]
+    if not os.path.isfile(lj) or not epochs:
+        _fail('load_segmenter: %s needs labels.json and encoder_epoch_<N>.pth / decoder_epoch_<N>.pth'
+              % modeldir)
+    files = [os.path.join(modeldir, '%s_epoch_%d.pth' % (k, max(epochs))) for k in ('encoder', 'decoder')]
+    missing = [f for f in files if not os.path.isfile(f)]
+    if missing:
+        _fail('load_segmenter: missing %s' % ', '.join(missing))
+    with open(lj) as f:
+        labeldata = json.load(f)
+    return (torch.load(files[0], map_location='cpu'), torch.load(files[1], map_location='cpu'),
+            labeldata)
 
 
 class LabelMap(object):
@@ -204,6 +238,10 @@ class UnifiedParsingSegmenter(LabelMap):
                         [('part', self.head_groups[i][0], len(idx), self.objects_with_parts[i])
                          for i, idx in enumerate(self.part_index)])
 
+    @property
+    def label_channels(self):
+        return 5 if self.segdiv == 'quad' else 3
+
     def _run(self, images, downsample, want_probs, want_labels):
         u8, B, H, W = _images(images)
         if images.device != self.net.device:
@@ -271,3 +309,173 @@ class UnifiedParsingSegmenter(LabelMap):
         if result is None:
             _fail('segmenter: unrecognized class %d' % classnum)
         return result, mask
+
+
+class SemanticSegmenter(object):
+    """The reference's SemanticSegmenter (segmenter.py:392-574) for the colour model's architecture
+    (resnet18dilated, ppm_deepsup) with the weights passed in: `encoder_sd` / `decoder_sd` the state
+    dicts, `labeldata` the labels.json dict (`labels[]` with name / category / internal,
+    `categories[]` with name / mask, `imageformat` with byteorder / mean / stdev, optional
+    `segsizes`).  Forward only, CUDA only; segdiv is not offered."""
+
+    def __init__(self, encoder_sd, decoder_sd, labeldata, segsizes=None, device='cuda'):
+        if segsizes is None:
+            segsizes = labeldata.get('segsizes', [256])
+        self.segsizes = list(segsizes)
+        if not 1 <= len(self.segsizes) <= 4:
+            _fail('segmenter: 1 to 4 segsizes (got %d)' % len(self.segsizes))
+        self.labeldata = labeldata
+        meta = labeldata['labels']
+        catnames = [c['name'] for c in labeldata['categories']]
+        fmt = labeldata['imageformat']
+        self.bgr = fmt['byteorder'] == 'BGR'
+        self.imagemean = [float(v) for v in fmt['mean']]
+        self.imagestd = [float(v) for v in fmt['stdev']]
+        self.labelmap = {'-': 0}
+        self.channelmap = {'-': []}
+        self.labels = [('-', '-')]
+        self.num_underlying_classes = len(meta)
+        for i, label in enumerate(meta):
+            if label['category'] not in catnames:
+                _fail('segmenter: label %d (%s) is in category %r, which labels.json does not list'
+                      % (i, label['name'], label['category']))
+            self.channelmap.setdefault(label['name'], []).append(i)
+            if label.get('internal') or label['name'] in self.labelmap:
+                continue
+            self.labelmap[label['name']] = len(self.labels)
+            self.labels.append((label['name'], label['category']))
+        self.category_indexes = {c: [i for i, l in enumerate(meta) if l['category'] == c]
+                                 for c in catnames}
+        self.catindexmap = {}
+        for c, idx in self.category_indexes.items():
+            if not idx:
+                _fail('segmenter: category %r has no labels' % c)
+            for k, i in enumerate(idx):
+                self.catindexmap[meta[i]['name']] = (c, k)
+        self.category_map = {c: torch.tensor([self.labelmap.get(meta[i]['name'], 0) for i in idx])
+                             for c, idx in self.category_indexes.items()}
+        self.categories = catnames
+        self.channellist = [self.channelmap[name] for name, _ in self.labels]
+        self._cats = []
+        for cat in labeldata['categories']:
+            mc, mi = -1, 0
+            if cat.get('mask') is not None:
+                if cat['mask'] not in self.catindexmap:
+                    _fail('segmenter: category %r masks on %r, which is no label' % (cat['name'], cat['mask']))
+                mcat, mi = self.catindexmap[cat['mask']]
+                mc = catnames.index(mcat)
+            self._cats.append((self.category_indexes[cat['name']],
+                               self.category_map[cat['name']].tolist(), mc, mi))
+        self.net = net.SemanticNet(encoder_sd, decoder_sd, len(meta), device)
+
+    def get_label_and_category_names(self, dataset=None):
+        return self.labels, self.categories
+
+    @property
+    def label_channels(self):
+        return len(self.categories)
+
+    def _run(self, images, downsample, want_probs, labels=None, lcoff=0, offset=0):
+        u8, B, H, W = _images(images)
+        if images.device != self.net.device:
+            _fail('segmenter: images on %s, the segmenter on %s' % (images.device, self.net.device))
+        if images.requires_grad:
+            _fail('segmenter: the segmenter is forward-only; pass images that do not require grad')
+        Ho, Wo = H // downsample, W // downsample
+        if labels is not None and (labels.dtype != torch.int64 or labels.device != self.net.device or
+                                   not labels.is_contiguous() or labels.dim() != 4 or
+                                   tuple(labels.shape) != (B, labels.shape[1], Ho, Wo)):
+            _fail('segmenter: labels must be contiguous int64 [%d, L, %d, %d] on %s'
+                  % (B, Ho, Wo, self.net.device))
+        images = images.contiguous()
+        per_size = []
+        with torch.no_grad():
+            for s in self.segsizes:
+                if (s, s) != (H, W) and (H % s or W % s):
+                    _fail('segmenter: segsize %d must divide the image size %dx%d' % (s, H, W))
+                x = net.input_pass_norm(images, u8, s, self.imagemean, self.imagestd, self.bgr)
+                logits, hw = self.net.decoder(self.net.encoder(x))
+                per_size.append((logits, hw))
+            return self.net.classes(per_size, B, Ho, Wo, self._cats, want_probs, labels, lcoff,
+                                    offset)
+
+    def raw_seg_prediction(self, tensor_images, downsample=1):
+        """[B, classes, H // downsample, W // downsample]: the per-category softmaxes of the
+        network's class probabilities, summed over segsizes."""
+        return self._run(tensor_images, downsample, True)
+
+    def raw_segment_batch(self, tensor_images, downsample=1):
+        """(segment_batch's labels, raw_seg_prediction's probabilities) from one pass."""
+        segs = self._new_labels(tensor_images, downsample, len(self.categories))
+        pred = self._run(tensor_images, downsample, True, segs)
+        return segs, pred
+
+    def segment_batch(self, tensor_images, downsample=1):
+        """int64 [B, categories, H // downsample, W // downsample]: per category the label of its
+        most probable channel, 0 where the category's mask label does not win its own category."""
+        return self.segment_into(tensor_images, None, 0, 0, downsample)
+
+    def segment_into(self, tensor_images, labels, lcoff, offset, downsample=1):
+        """segment_batch + offset written into channels lcoff.. of `labels` (a new tensor when
+        None), which is returned."""
+        if labels is None:
+            labels = self._new_labels(tensor_images, downsample, len(self.categories))
+        self._run(tensor_images, downsample, False, labels, lcoff, offset)
+        return labels
+
+    def _new_labels(self, images, downsample, n):
+        _, B, H, W = _images(images)
+        return torch.empty((B, n, H // downsample, W // downsample), dtype=torch.int64,
+                           device=images.device)
+
+    def predict_single_class(self, tensor_images, classnum, downsample=1):
+        """(score, mask) for one label number, as the reference's (segmenter.py:547-574)."""
+        seg, pred = self.raw_segment_batch(tensor_images, downsample=downsample)
+        result = pred[:, self.channellist[classnum]].sum(dim=1)
+        mask = (seg == classnum).max(1)[0]
+        return result, mask
+
+
+class MergedSegmenter(object):
+    """The reference's MergedSegmenter (segmenter.py:82-113): the components' labels numbered one
+    after the other.  segment_batch writes every component's channels into one tensor (a semantic
+    component writes its slice with its offset added); predict_single_class passes `downsample`
+    on, where the reference's raises a NameError."""
+
+    def __init__(self, component_segmenters):
+        self.component_segmenters = component_segmenters
+        self.labels = []
+        self.cats = []
+        self.offsets = []
+        for sgm in self.component_segmenters:
+            self.offsets.append(len(self.labels))
+            slabels, scats = sgm.get_label_and_category_names()
+            self.labels.extend(slabels)
+            for cat in scats:
+                if cat not in self.cats:
+                    self.cats.append(cat)
+
+    def get_label_and_category_names(self):
+        return (self.labels, self.cats)
+
+    def segment_batch(self, tensor_images, downsample=1):
+        _, B, H, W = _images(tensor_images)
+        chans = [sgm.label_channels for sgm in self.component_segmenters]
+        out = torch.empty((B, sum(chans), H // downsample, W // downsample), dtype=torch.int64,
+                          device=tensor_images.device)
+        c = 0
+        for sgm, off, n in zip(self.component_segmenters, self.offsets, chans):
+            if isinstance(sgm, SemanticSegmenter):
+                sgm.segment_into(tensor_images, out, c, off, downsample)
+            else:
+                seg = sgm.segment_batch(tensor_images, downsample=downsample)
+                out[:, c:c + n] = seg + off if off else seg
+            c += n
+        return out
+
+    def predict_single_class(self, tensor_images, classnum, downsample=1):
+        for i, sgm in enumerate(self.component_segmenters):
+            if i + 1 == len(self.offsets) or classnum < self.offsets[i + 1]:
+                classnum -= self.offsets[i]
+                break
+        return sgm.predict_single_class(tensor_images, classnum, downsample=downsample)
