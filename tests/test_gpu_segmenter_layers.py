@@ -3,7 +3,8 @@ launch against float64, at the label widths of the unified-parsing label set
 (`segmenter_oracle.wide_labels`: 336 objects, 26 materials, 40 part groups of 6, so the object head
 is N = 384, the part head N = 256 and `rw_seg_classes` runs 42 groups).
 
-The run is observed, not changed.  `torch.empty` / `torch.empty_like` and `_cabi.call` are
+The run is observed, not changed (the recorder, the fold and the shared launch checks are in
+`oracle/launch_record.py`).  `torch.empty` / `torch.empty_like` and `_cabi.call` are
 wrapped, so every tensor the run allocates and every launch (entry point and arguments, in order)
 is recorded; every recorded tensor stays referenced until the checks end, so no allocation is
 freed and reused during the run.  A `rw_seg_map` that writes a channel slice of a wider plane set
@@ -49,14 +50,11 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from oracle import launch_record as lr
 from oracle import segmenter_oracle as so
-from oracle.exact_operands import bf16_split, bits_equal, three
 
 pytestmark = pytest.mark.gpu
 
-U = 2.0 ** -24
-SPLIT = 2.0 ** -17
-BN_EPS = 1e-5
 LAYERS = (3, 4, 6, 3)
 POOL_SCALES = (1, 2, 3, 6)
 HEADS = ('object', 'part', 'material')
@@ -79,67 +77,6 @@ BOUNDS = {
 
 
 # ------------------------------------------------------------------ observation
-class _Run(object):
-    def __init__(self):
-        self.calls, self.tensors, self.slices = [], [], {}
-
-
-def _ptr(a):
-    if a is None:
-        return None
-    return a.value if isinstance(a, ctypes.c_void_p) else int(a)
-
-
-def _observe(monkeypatch, fn):
-    """(record, fn()) with every allocation and launch of fn recorded; each slice write of
-    rw_seg_map is followed by a comparison of the planes' other channels with their state
-    before it."""
-    from rewriting_b200 import _cabi
-    run = _Run()
-    real_empty, real_empty_like, real_call = torch.empty, torch.empty_like, _cabi.call
-
-    def empty(*a, **k):
-        t = real_empty(*a, **k)
-        run.tensors.append(t)
-        return t
-
-    def empty_like(*a, **k):
-        t = real_empty_like(*a, **k)
-        run.tensors.append(t)
-        return t
-
-    def find(p):
-        for t in reversed(run.tensors):
-            if t.data_ptr() == p:
-                return t
-        raise AssertionError('no recorded tensor at %#x' % p)
-
-    def call(name, *args):
-        i = len(run.calls)
-        run.calls.append((name, args))
-        if name != 'rw_seg_map' or args[12] is None or args[14] == args[3]:
-            return real_call(name, *args)
-        C, ldc, coff = args[3], args[14], args[15]
-        planes = [find(_ptr(args[12])), find(_ptr(args[13]))]
-        before = [t.view(-1, ldc).clone() for t in planes]
-        rc = real_call(name, *args)
-        kept = True
-        for t, b in zip(planes, before):
-            t = t.view(-1, ldc)
-            kept = kept and bits_equal(t[:, :coff], b[:, :coff]) and bits_equal(t[:, coff + C:],
-                                                                                b[:, coff + C:])
-        run.slices[i] = kept
-        return rc
-
-    with monkeypatch.context() as m:
-        m.setattr(torch, 'empty', empty)
-        m.setattr(torch, 'empty_like', empty_like)
-        m.setattr(_cabi, 'call', call)
-        out = fn()
-    torch.cuda.synchronize()
-    return run, out
-
-
 def _convs(net):
     """{conv key: _Conv} of the network; a key is (state dict, weight key, batch-norm prefix or
     None for the class heads' unfolded 1x1)."""
@@ -166,121 +103,18 @@ def _convs(net):
     return out
 
 
-class _Tensors(object):
+def _Tensors(run, seg, extra):
     """data_ptr -> tensor over everything the run could have handed a kernel."""
-
-    def __init__(self, run, seg, extra):
-        self.map = {}
-        for t in list(extra) + run.tensors:
-            self._add(t)
-        for c in _convs(seg.net).values():
-            for t in (c.w, c.bias, c.hi, c.lo):
-                self._add(t)
-        self._add(seg._trans)
-
-    def _add(self, t):
-        if t is not None and t.numel():
-            self.map.setdefault(t.data_ptr(), t)
-
-    def __call__(self, a, *shape):
-        t = self.map[_ptr(a)]
-        return t.reshape(shape) if shape else t
-
-
-# ------------------------------------------------------------------ the fold, from the state dict
-def _fold(sds, key):
-    """fp32 (weight, bias) of one conv: the float64 batch-norm fold of its state-dict entries,
-    rounded once; the class heads' 1x1 convs are their weight and bias as stored."""
-    sd = sds[key[0]]
-    w = torch.as_tensor(sd[key[1]]).detach().double()
-    if key[2] is None:
-        b = torch.as_tensor(sd[key[1][:-len('weight')] + 'bias']).detach().double()
-        return w.float(), b.float()
-    p = key[2]
-    g, beta = sd[p + 'weight'].double(), sd[p + 'bias'].double()
-    mean, var = sd[p + 'running_mean'].double(), sd[p + 'running_var'].double()
-    k = g / torch.sqrt(var + BN_EPS)
-    return (w * k[:, None, None, None]).float(), (beta - mean * k).float()
-
-
-class _Folds(object):
-    """The folds of one (encoder, decoder) pair, computed once per key, on the device."""
-
-    def __init__(self, enc, dec):
-        self.sds = {'enc': enc, 'dec': dec}
-        self.cache = {}
-
-    def __call__(self, key):
-        if key not in self.cache:
-            w, b = _fold(self.sds, key)
-            self.cache[key] = (w.cuda(), b.cuda())
-        return self.cache[key]
-
-
-def _fp32_bits(a, b):
-    return a.dtype == b.dtype == torch.float32 and a.shape == b.shape and torch.equal(
-        a.contiguous().view(torch.int32), b.contiguous().view(torch.int32))
-
-
-def _padded(t, n):
-    """t [c, ...] with zero rows appended up to n"""
-    if t.shape[0] == n:
-        return t
-    return torch.cat([t, t.new_zeros((n - t.shape[0],) + tuple(t.shape[1:]))])
-
-
-def _w1x1(folds, key, n):
-    w, b = folds(key)
-    return _padded(w.reshape(w.shape[0], -1), n), _padded(b, n)
-
-
-def _w3x3_planes(w):
-    """the `fwd` planes ([Cout][tap][Cin], flat) of an fp32 [Cout, Cin, 3, 3] weight"""
-    hi, lo = bf16_split(w)
-    return tuple(t.permute(0, 2, 3, 1).contiguous().flatten() for t in (hi, lo))
-
-
-def _net_operands_exact(net, folds):
-    """every _Conv's fp32 weight, bias and planes against the fold, bit for bit"""
-    bad = []
-    for key, c in _convs(net).items():
-        w, b = folds(key)
-        if c.kind == '1x1':
-            n = c.w.shape[0]
-            w, b = _w1x1(folds, key, n)
-            ok = _fp32_bits(c.w, w) and _fp32_bits(c.bias, b)
-            hi, lo = bf16_split(w)
-            ok = ok and bits_equal(c.hi, hi) and bits_equal(c.lo, lo)
-            if key[2] is None:            # a class head: pad rows zero in every operand
-                m = c.cout
-                ok = ok and all(bool((t[m:].float() == 0).all()) for t in (c.w, c.hi, c.lo))
-                ok = ok and bool((c.bias[m:] == 0).all()) and n % 64 == 0 and n - m < 64
-        else:
-            ok = _fp32_bits(c.w, w) and _fp32_bits(c.bias, b)
-            if c.kind == '3x3':
-                hi, lo = _w3x3_planes(w)
-                ok = ok and bits_equal(c.hi, hi) and bits_equal(c.lo, lo)
-        if not ok:
-            bad.append(key)
-    return bad
+    return lr.Tensors(run, extra, lr.conv_tensors(_convs(seg.net)) + [seg._trans])
 
 
 # ------------------------------------------------------------------ the plan of launches
-class _Step(object):
-    """One expected launch: entry point, place in the network, the conv whose operands it reads
-    (or None), the step whose output it reads as its input and as its residual."""
-    __slots__ = ('name', 'where', 'conv', 'src', 'res')
-
-    def __init__(self, name, where, conv=None, src=None, res=None):
-        self.name, self.where, self.conv, self.src, self.res = name, where, conv, src, res
-
-
 def _plan():
     """The launches of one forward at one segmentation size, in order."""
     P = []
 
     def add(*a, **k):
-        P.append(_Step(*a, **k))
+        P.append(lr.Step(*a, **k))
         return P[-1].where
 
     def enc(p, n):
@@ -350,134 +184,6 @@ def _plan():
     return P
 
 
-def _outputs(name, a):
-    """the pointers a launch writes"""
-    idx = {'rw_seg_input': [6], 'rw_narrow_conv3x3': [9], 'rw_seg_map': [12, 16],
-           'rw_conv3x3_bias_act': [12], 'rw_relu_pool': [7, 9], 'rw_seg_maxpool': [5],
-           'rw_rowgemm': [7], 'rw_seg_prroi': [6], 'rw_seg_classes': [12, 13]}[name]
-    return {_ptr(a[i]) for i in idx if a[i] is not None}
-
-
-def _resolve(plan, calls):
-    """the launch sequence and the wiring: each launch reads the output of its planned source"""
-    names = [c[0] for c in calls]
-    assert names == [s.name for s in plan], [(i, n, s.name) for i, (n, s) in
-                                             enumerate(zip(names, plan)) if n != s.name][:5]
-    outs = {}
-    for step, (name, a) in zip(plan, calls):
-        if step.src is not None:
-            assert _ptr(a[0]) in outs[step.src], step.where
-        if step.res is not None:
-            assert _ptr(a[10]) in outs[step.res], step.where + ' (residual)'
-        outs[step.where] = _outputs(name, a)
-
-
-# ------------------------------------------------------------------ operand checks
-def _operands_ok(step, a, T, folds):
-    """the launch's weight / bias operands are those of the fold of step.conv, bit for bit"""
-    key, name = step.conv, step.name
-    if name == 'rw_narrow_conv3x3':
-        w, _ = folds(key)
-        return a[2] is None and float(a[3]) == 1.0 and _fp32_bits(T(a[1], *w.shape), w)
-    if name == 'rw_conv3x3_bias_act':
-        w, b = folds(key)
-        Cout = a[9]
-        hi, lo = _w3x3_planes(w)
-        return (a[5] == 0 and bits_equal(T(a[2]).flatten(), hi) and
-                bits_equal(T(a[3]).flatten(), lo) and _fp32_bits(T(a[4], Cout), b))
-    if name == 'rw_rowgemm':
-        w, _ = _w1x1(folds, key, a[6])
-        hi, lo = bf16_split(w)
-        return bits_equal(T(a[2], *w.shape), hi) and bits_equal(T(a[3], *w.shape), lo)
-    if name == 'rw_seg_map':
-        _, b = folds(key)
-        return a[9] is not None and _fp32_bits(T(a[9], a[3]), b)
-    raise AssertionError(name)
-
-
-def _check_operands(plan, calls, T, folds):
-    """{place: bool} over every launch that reads a conv's weight or bias (the class heads' bias
-    is checked with rw_seg_classes)"""
-    return {s.where: _operands_ok(s, a, T, folds) for s, (_, a) in zip(plan, calls)
-            if s.conv is not None}
-
-
-# ------------------------------------------------------------------ the record of errors
-class _Meter(object):
-    def __init__(self, case):
-        self.case = case
-        self.worst = {}
-        self.notes = []
-
-    def add(self, family, value, where):
-        if family not in self.worst or value > self.worst[family][0]:
-            self.worst[family] = (value, where)
-
-    def note(self, text):
-        self.notes.append(text)
-
-    def finish(self):
-        for fam, (v, where) in sorted(self.worst.items()):
-            print('\n[segmenter-layers] %-10s %-8s %.3e  (%s; bound %.3g)'
-                  % (self.case, fam, v, where, BOUNDS[fam]), end='')
-        for n in self.notes:
-            print('\n[segmenter-layers] %-10s %s' % (self.case, n), end='')
-        print()
-        bad = {f: (v, w, BOUNDS[f]) for f, (v, w) in self.worst.items() if not v < BOUNDS[f]}
-        assert not bad, bad
-
-
-def _err_u(got, ref, S):
-    """max |got - ref| / (u·S) over outputs with S > 0; outputs with S = 0 must be exact"""
-    d = (got.double() - ref).abs()
-    zero = S == 0
-    assert bool((d[zero] == 0).all())
-    return (d[~zero] / (U * S[~zero])).max().item() if bool((~zero).any()) else 0.0
-
-
-def _planes_err_u(got, v, S):
-    """planes: max (|got - v| - 2^-17·|v|) / (u·S), the split residual taken off first"""
-    d = (got - v).abs() - SPLIT * v.abs()
-    return max(0.0, (d / (U * S)).max().item())
-
-
-def _relu(v):
-    return torch.where(v > 0, v, torch.zeros_like(v))
-
-
-def _rows(t, B, H, W, C):
-    """padded-flat rows [B·(H+1)·(W+1)][C] as [B, H+1, W+1, C]"""
-    return t.reshape(B, H + 1, W + 1, C)
-
-
-def _nchw(t, B, H, W, C, c0=0, n=None):
-    n = C - c0 if n is None else n
-    return _rows(t, B, H, W, C)[:, :H, :W, c0:c0 + n].permute(0, 3, 1, 2)
-
-
-def _up64(x, H, W):
-    return F.interpolate(x, size=(H, W), mode='bilinear', align_corners=False)
-
-
-def _planes_exact(hi, lo, v, B, H, W, ldc, coff):
-    """planes hi / lo [rows][ldc] at channels coff.. hold the bf16 split of v [B,C,H,W], their pad
-    rows and columns zero"""
-    C = v.shape[1]
-    ehi, elo = bf16_split(v)
-    for got, e in ((hi, ehi), (lo, elo)):
-        g = _rows(got, B, H, W, ldc)[..., coff:coff + C]
-        assert bits_equal(g[:, :H, :W].permute(0, 3, 1, 2), e)
-        assert bool((g[:, H].contiguous().view(torch.int16) == 0).all())
-        assert bool((g[:, :, W].contiguous().view(torch.int16) == 0).all())
-
-
-def _planes_pads_zero(hi, lo, B, H, W, ldc, coff, C):
-    for t in (hi, lo):
-        g = _rows(t, B, H, W, ldc)[..., coff:coff + C]
-        assert bool((g[:, H].contiguous().view(torch.int16) == 0).all())
-        assert bool((g[:, :, W].contiguous().view(torch.int16) == 0).all())
-
-
 # ------------------------------------------------------------------ launch checks
 def _check_input(m, T, a, images):
     im, u8, B, H, W, S = a[0], a[1], a[2], a[3], a[4], a[5]
@@ -486,127 +192,24 @@ def _check_input(m, T, a, images):
     ref = so.net_input(x, S)
     mean = torch.tensor(so.MEAN_BGR, dtype=torch.float64)[None, :, None, None]
     Sx = F.adaptive_avg_pool2d((so.net_input(x, H) + mean).abs() + mean, (S, S))
-    m.add('input', _err_u(T(a[6], B, 3, S, S).cpu(), ref, Sx), 'rw_seg_input %d -> %d' % (H, S))
-
-
-def _check_stem(m, T, a, sel):
-    x, B, Cin, Cout, H, W = a[0], a[4], a[5], a[6], a[7], a[8]
-    x = T(x, B, Cin, H, W)[sel].double()
-    w = T(a[1], Cout, Cin, 3, 3).double()
-    ref = F.conv2d(x, w, padding=1)
-    S = F.conv2d(x.abs(), w.abs(), padding=1)
-    m.add('stem', _err_u(T(a[9], B, Cout, H, W)[sel], ref, S), 'stem conv1')
-
-
-def _check_conv3x3(m, T, a, sel, where):
-    B, Cin, Cout, H, W = a[7:12]
-    wh, wl = (T(p, Cout, 3, 3, Cin).permute(0, 3, 1, 2).double() for p in (a[2], a[3]))
-    b = T(a[4], Cout).double()[None, :, None, None]
-    out = T(a[12], B, Cout, H, W)
-    for i in sel:
-        xh, xl = (_nchw(T(p), B, H, W, Cin)[i:i + 1].double() for p in (a[0], a[1]))
-        ref, S = three(lambda x, w: F.conv2d(x, w, padding=1), (xh, xl), (wh, wl))
-        m.add('conv3x3', _err_u(out[i:i + 1], ref + b, S + b.abs()), '%s (K %d)' % (where, 9 * Cin))
-
-
-def _check_rowgemm(m, T, a, B, sel, where):
-    rows, K, N = a[4], a[5], a[6]
-    per = rows // B
-    assert per * B == rows
-    idx = torch.cat([torch.arange(i * per, (i + 1) * per) for i in sel]) if rows > 4096 \
-        else torch.arange(rows)
-    idx = idx.cuda()
-    xh, xl = (T(p, rows, K)[idx].double() for p in (a[0], a[1]))
-    wh, wl = (T(p, N, K).double() for p in (a[2], a[3]))
-    ref, S = three(lambda x, w: x @ w.t(), (xh, xl), (wh, wl))
-    m.add('rowgemm', _err_u(T(a[7], rows, N)[idx], ref, S), '%s (K %d, N %d)' % (where, K, N))
-
-
-def _map_source(T, a):
-    src, a_cl, B, C, Hin, Win = a[0], a[1], a[2], a[3], a[4], a[5]
-    if a_cl:
-        return _nchw(T(src), B, Hin, Win, C)
-    return T(src, B, C, Hin, Win)
-
-
-def _check_map(m, T, a, sel, where, kept):
-    """rw_seg_map: modes 0 / 1 bit for bit, mode 2 against float64"""
-    B, C, Hin, Win, mode, Ho, Wo = a[2:9]
-    relu, hi, lo, ldc, coff, outp = a[11], a[12], a[13], a[14], a[15], a[16]
-    x = _map_source(T, a)
-    bias = T(a[9], C)[None, :, None, None] if a[9] is not None else None
-    res = T(a[10], B, C, Ho, Wo) if a[10] is not None else None
-    out = T(outp, B, C, Ho, Wo) if outp is not None else None
-    if hi is not None:
-        hi, lo = T(hi), T(lo)
-        if ldc != C:
-            assert kept, where + ': a channel slice outside the launch changed'
-    if mode in (0, 1):
-        v = x if mode == 0 else x[:, :, ::2, ::2]
-        if bias is not None:
-            v = v + bias
-        if res is not None:
-            v = v + res
-        if relu:
-            v = _relu(v)
-        if out is not None:
-            assert _fp32_bits(out, v.contiguous()), where
-        if hi is not None:
-            _planes_exact(hi, lo, v, B, Ho, Wo, ldc, coff)
-        return
-    # mode 2: float64 resize, + bias, + residual, ReLU
-    if out is not None and hi is not None:
-        _planes_exact(hi, lo, out, B, Ho, Wo, ldc, coff)
-    elif hi is not None:
-        _planes_pads_zero(hi, lo, B, Ho, Wo, ldc, coff, C)
-    for i in sel:
-        x64 = x[i:i + 1].double()
-        ref, S = _up64(x64, Ho, Wo), _up64(x64.abs(), Ho, Wo)
-        if bias is not None:
-            ref, S = ref + bias.double(), S + bias.double().abs()
-        if res is not None:
-            r = res[i:i + 1].double()
-            ref, S = ref + r, S + r.abs()
-        if relu:
-            ref = _relu(ref)
-        if out is not None:
-            m.add('resize', _err_u(out[i:i + 1], ref, S), where)
-        elif hi is not None:
-            g = (_nchw(hi, B, Ho, Wo, ldc, coff, C)[i:i + 1].double() +
-                 _nchw(lo, B, Ho, Wo, ldc, coff, C)[i:i + 1].double())
-            m.add('resize', _planes_err_u(g, ref, S), where + ' (planes)')
-
-
-def _check_relu_pool(T, a, where):
-    assert a[1] is None and a[6] == 0, where
-    B, C, H, W = a[2:6]
-    v = _relu(T(a[0], B, C, H, W))
-    if a[9] is not None:
-        assert _fp32_bits(T(a[9], B, C, H, W), v), where
-    _planes_exact(T(a[7]), T(a[8]), v, B, H, W, C, 0)
-
-
-def _check_maxpool(T, a):
-    B, C, H, W = a[1:5]
-    want = F.max_pool2d(T(a[0], B, C, H, W), 3, 2, 1)
-    assert _fp32_bits(T(a[5], *want.shape), want.contiguous())
+    m.add('input', lr.err_u(T(a[6], B, 3, S, S).cpu(), ref, Sx), 'rw_seg_input %d -> %d' % (H, S))
 
 
 def _check_prroi(m, T, a, where):
     B, C, H, W, s = a[1:6]
     x = T(a[0], B, C, H, W).double()
     ref, S = so.prroi_whole(x, s), so.prroi_whole(x.abs(), s)
-    m.add('prroi', _err_u(T(a[6], B, C, s, s), ref, S), where)
+    m.add('prroi', lr.err_u(T(a[6], B, C, s, s), ref, S), where)
 
 
 def _classes_args(a):
     """the recorded rw_seg_classes arguments decoded from their ctypes arrays"""
     ns, ng = a[0], a[5]
-    ptrs = (ctypes.c_void_p * (3 * ns)).from_address(_ptr(a[1]))
-    hw = (ctypes.c_int * (2 * ns)).from_address(_ptr(a[2]))
-    bias = (ctypes.c_void_p * 3).from_address(_ptr(a[3]))
-    ld = (ctypes.c_int * 3).from_address(_ptr(a[4]))
-    gr = (ctypes.c_int * (4 * ng)).from_address(_ptr(a[6]))
+    ptrs = (ctypes.c_void_p * (3 * ns)).from_address(lr.ptr(a[1]))
+    hw = (ctypes.c_int * (2 * ns)).from_address(lr.ptr(a[2]))
+    bias = (ctypes.c_void_p * 3).from_address(lr.ptr(a[3]))
+    ld = (ctypes.c_int * 3).from_address(lr.ptr(a[4]))
+    gr = (ctypes.c_int * (4 * ng)).from_address(lr.ptr(a[6]))
     groups = [tuple(gr[4 * g:4 * g + 4]) for g in range(ng)]
     return ([list(ptrs[3 * s:3 * s + 3]) for s in range(ns)],
             [(hw[2 * s], hw[2 * s + 1]) for s in range(ns)], list(bias), list(ld), groups)
@@ -627,8 +230,8 @@ def _check_classes(m, T, a, seg, folds):
     nums = {h: seg.net.n[h] for h in HEADS}
     assert ld == [(nums[h] + 63) // 64 * 64 for h in HEADS]
     for k, h in enumerate(HEADS):        # the heads' biases: the state dict's, pad rows zero
-        _, b = _w1x1(folds, ('dec', '%s_head.1.weight' % h, None), ld[k])
-        assert _fp32_bits(T(biasp[k], ld[k]), b), h
+        _, b = lr.w1x1(folds, ('dec', '%s_head.1.weight' % h, None), ld[k])
+        assert lr.fp32_bits(T(biasp[k], ld[k]), b), h
     ctot = sum(g[2] for g in groups)
     probs = T(a[12], B, ctot, Ho, Wo)
     labels = T(a[13], B, 3, Ho, Wo)
@@ -641,17 +244,17 @@ def _check_classes(m, T, a, seg, folds):
             bias = T(biasp[hd], ld[hd])[c0:c0 + n].double()[None, :, None, None]
             for s in range(ns):
                 h, w = hws[s]
-                lg = _nchw(T(ptrs[s][hd]), B, h, w, ld[hd], c0, n)[b:b + 1].double()
-                l = _up64(lg, Ho, Wo) + bias
-                Ls = _up64(lg.abs(), Ho, Wo) + bias.abs()
+                lg = lr.nchw(T(ptrs[s][hd]), B, h, w, ld[hd], c0, n)[b:b + 1].double()
+                l = lr.up64(lg, Ho, Wo) + bias
+                Ls = lr.up64(lg.abs(), Ho, Wo) + bias.abs()
                 p = p + F.softmax(l, 1)
                 L = L + Ls
             S = p * (1 + L + L.max(1, keepdim=True)[0]) + TINY
-            e = _err_u(probs[b:b + 1, outc:outc + n], p, S)
+            e = lr.err_u(probs[b:b + 1, outc:outc + n], p, S)
             if e > worst[0]:
                 worst = (e, 'image %d group %d (%d wide)' % (b, g, n))
             ps.append(p[0])
-            tols.append(2 * BOUNDS['probs'] * U * S[0].max(0)[0])
+            tols.append(2 * BOUNDS['probs'] * lr.U * S[0].max(0)[0])
             outc += n
         # the labels: object, material (with its offset), the owning object's part
         lab = torch.zeros(3, Ho, Wo, dtype=torch.int64, device='cuda')
@@ -695,27 +298,27 @@ def _sel(B):
 def _check_run(meter, run, seg, folds, images, B):
     T = _Tensors(run, seg, [images])
     plan = _plan()
-    _resolve(plan, run.calls)
-    bad = [w for w, ok in _check_operands(plan, run.calls, T, folds).items() if not ok]
+    lr.resolve(plan, run.calls)
+    bad = [w for w, ok in lr.check_operands(plan, run.calls, T, folds).items() if not ok]
     assert not bad, bad
-    assert not _net_operands_exact(seg.net, folds)
+    assert not lr.net_operands_exact(_convs(seg.net), folds)
     sel = _sel(B)
     labels = None
     for i, (step, (name, a)) in enumerate(zip(plan, run.calls)):
         if name == 'rw_seg_input':
             _check_input(meter, T, a, images)
         elif name == 'rw_narrow_conv3x3':
-            _check_stem(meter, T, a, sel)
+            lr.check_stem(meter, T, a, sel)
         elif name == 'rw_conv3x3_bias_act':
-            _check_conv3x3(meter, T, a, sel, step.where)
+            lr.check_conv3x3(meter, T, a, sel, step.where)
         elif name == 'rw_rowgemm':
-            _check_rowgemm(meter, T, a, B, sel, step.where)
+            lr.check_rowgemm(meter, T, a, B, sel, step.where)
         elif name == 'rw_seg_map':
-            _check_map(meter, T, a, sel, step.where, run.slices.get(i))
+            lr.check_map(meter, T, name, a, sel, step.where, run.slices.get(i))
         elif name == 'rw_relu_pool':
-            _check_relu_pool(T, a, step.where)
+            lr.check_relu_pool(T, a, step.where)
         elif name == 'rw_seg_maxpool':
-            _check_maxpool(T, a)
+            lr.check_maxpool(T, a)
         elif name == 'rw_seg_prroi':
             _check_prroi(meter, T, a, step.where)
         elif name == 'rw_seg_classes':
@@ -730,7 +333,7 @@ def _check_run(meter, run, seg, folds, images, B):
 def wide():
     labels = so.wide_labels()
     enc, dec = so.seeded_state_dicts(labels)
-    return labels, enc, dec, _Folds(enc, dec)
+    return labels, enc, dec, lr.Folds(enc, dec)
 
 
 def _images(B, H, seed, u8=False):
@@ -764,12 +367,12 @@ def _observed(monkeypatch, seg, img, ds):
     an unobserved run and the public raw_seg_prediction / segment_batch, bit for bit"""
     with torch.no_grad():
         plain = [t.clone() for t in seg._run(img, ds, True, True)]
-        run, out = _observe(monkeypatch, lambda: seg._run(img, ds, True, True))
+        run, out = lr.observe(monkeypatch, lambda: seg._run(img, ds, True, True))
         pred, part = seg.raw_seg_prediction(img, downsample=ds)
         segs = seg.segment_batch(img, downsample=ds)
     assert all(torch.equal(o, p) for o, p in zip(out, plain)), 'the observed run differs'
     pub = torch.cat([pred['object'], pred['material']] + [part[i] for i in range(len(part))], 1)
-    assert _fp32_bits(pub, out[0])
+    assert lr.fp32_bits(pub, out[0])
     assert torch.equal(segs[:, :3], out[1])
     return run, out, segs
 
@@ -786,7 +389,7 @@ def test_segmenter_launch_by_launch(monkeypatch, wide, case):
     img = _images(B, H, c['seed'], c['u8'])
     run, (probs, labels), segs = _observed(monkeypatch, seg, img, c['ds'])
     assert probs.shape[2:] == (H // c['ds'], H // c['ds'])
-    meter = _Meter(case)
+    meter = lr.Meter('segmenter-layers', case, BOUNDS)
     got = _check_run(meter, run, seg, wide[3], img, B)
     assert got.data_ptr() == labels.data_ptr()
     if c['segdiv'] == 'quad':
@@ -806,7 +409,7 @@ def test_negative_control_swapped_blocks(monkeypatch, wide):
     run, _, _ = _observed(monkeypatch, seg, img, 1)
     T = _Tensors(run, seg, [img])
     plan = _plan()
-    _resolve(plan, run.calls)
+    lr.resolve(plan, run.calls)
     swapped = {}
     for k, v in enc.items():
         for a, b in (('layer3.1.', 'layer3.2.'), ('layer3.2.', 'layer3.1.')):
@@ -815,11 +418,11 @@ def test_negative_control_swapped_blocks(monkeypatch, wide):
                 break
         swapped[k] = v
     with torch.no_grad():
-        good = _check_operands(plan, run.calls, T, folds)
-        bad = _check_operands(plan, run.calls, T, _Folds(swapped, dec))
+        good = lr.check_operands(plan, run.calls, T, folds)
+        bad = lr.check_operands(plan, run.calls, T, lr.Folds(swapped, dec))
     assert all(good.values())
     hit = sorted(w for w, ok in bad.items() if not ok)
     want = sorted(w for w in bad if w.startswith(('layer3.1.', 'layer3.2.')))
     print('\n[segmenter-layers] swapped layer3.1 / layer3.2: %d launches fail: %s' % (len(hit), hit))
     assert len(want) == 10 and hit == want
-    assert len(_net_operands_exact(seg.net, _Folds(swapped, dec))) == 6
+    assert len(lr.net_operands_exact(_convs(seg.net), lr.Folds(swapped, dec))) == 6
