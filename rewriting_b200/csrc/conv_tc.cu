@@ -21,9 +21,10 @@
 //
 // Warp roles (384 threads): warpgroups 0 and 1 each issue wgmma for 64 of the tile's 128 rows and
 // run the epilogue on their register accumulators, raised to 232 registers by setmaxnreg;
-// warpgroup 2 is the producer, lowered to 40, whose warp 8 issues the TMA loads.  A 7-stage ring
-// of 32 KB stages (BK = 32, 64-byte swizzle); the consumers keep one wgmma group in flight and
-// release each stage one k-block behind.
+// warpgroup 2 is the producer, lowered to 40, whose warp 8 issues the TMA loads.  A 6-stage ring
+// of 32 KB stages (BK = 32, 64-byte swizzle; BN = 64: 7 x 24 KB); the consumers keep one wgmma
+// group in flight and release each stage one k-block behind.  The next layer's planes leave the
+// epilogue through per-warp shared-memory slots and TMA stores.
 // Persistent 2-CTA clusters: the two CTAs take adjacent m-tiles with the same (phase, n), so they
 // read the same weight tile on every k-block; each loads one 64-row half of it and multicasts the
 // half to both, cutting each CTA's L2 reads per k-block from 32 KB to 24 KB.
@@ -39,11 +40,10 @@ namespace {
 
 constexpr int BM = 128;
 // the tile's output channels, BN, is a template parameter: 128, or 64 where Cout % 128 != 0
-// k-block of 32 channels = one 64-byte swizzle row: a 32 KB stage, so that seven fit in shared
-// memory and the producer runs up to six k-blocks ahead of the MMAs
+// k-block of 32 channels = one 64-byte swizzle row: a 32 KB stage (BN = 128), so that six fit in
+// shared memory next to the epilogue's plane slots
 constexpr int BK = 32;
 constexpr int MMA_K = 16;
-constexpr int kStages = 7;
 constexpr int kNumThreads = 384;   // warps 0-7: wgmma + epilogue, warpgroup 2: producer
 constexpr int kTmaWarp = 8;
 // register split after setmaxnreg: 128 x 40 + 256 x 232 = 384 x 168, the launch allocation
@@ -61,17 +61,33 @@ constexpr int kCluster = 2;
 // (K=512 -> pixel error 5.2e-4, K=1024 -> 8.1e-4, K >= 2304 fails the 1e-3 bound)
 constexpr int kChunkKB = 16;
 
+// The next layer's hi / lo planes leave through shared memory: each consumer warp packs its 16
+// rows of one 64-channel half into a slot per plane (16 rows x 128 bytes, 128-byte swizzle) with
+// stmatrix, and one TMA store writes the slot to the [rows][Cout] plane.  (As 4-byte LSU stores,
+// each touching 8 rows of the plane, they take half of the epilogue: DESIGN.md §6.)
+constexpr int kSlotBytes = 16 * 64 * 2;
+constexpr int kSlots = 2 * 8;          // hi and lo of each consumer warp: 32 KB
+
 template <int BN>
 struct ConvSmem {
   static constexpr int kABytes = BM * BK * 2;          // one plane: 8 KB
   static constexpr int kBBytes = BN * BK * 2;          // one plane: 8 KB (BN = 64: 4 KB)
   static constexpr int kStageBytes = 2 * kABytes + 2 * kBBytes;
-  static constexpr int kTotal = kStages * kStageBytes + 512 /*align slack*/ + 256 /*barriers*/;
+  // BN = 128: six 32 KB stages leave room for the plane slots (seven measured no faster than
+  // six, DESIGN.md §6); BN = 64: seven 24 KB stages
+  static constexpr int kStages = BN == 128 ? 6 : 7;
+  static constexpr int kSlotOfs = kStages * kStageBytes;
+  static constexpr int kBarOfs = kSlotOfs + kSlots * kSlotBytes;
+  static constexpr int kTotal = kBarOfs + 1024 /*align slack*/ + 256 /*barriers*/;
+  // the slots are 1024-byte aligned, the period of the 128-byte swizzle
+  static_assert(kSlotOfs % 1024 == 0, "conv_tc: plane slots off the swizzle period");
 };
-// 512-byte alignment serves the 64-byte swizzle atoms; the total must stay within the 227 KB a
-// block may opt in to
+// 1024-byte alignment serves the swizzle atoms of the ring and the slots; the total must stay within
+// the 227 KB a block may opt in to
 static_assert(ConvSmem<128>::kTotal <= 232448, "conv_tc: shared memory over the per-block limit");
+static_assert(ConvSmem<64>::kTotal <= 232448, "conv_tc: shared memory over the per-block limit");
 
+template <int kStages>
 struct Barriers {
   uint64_t full[kStages];
   uint64_t empty[kStages];
@@ -96,19 +112,24 @@ __device__ __forceinline__ void decode_tile(int tile, int nphase, int nsched, in
 // BN = 64 (Cout % 128 != 0, the 64-channel layers of the 512² generator): wgmma.m64n64k16 on a
 // 64-row weight tile, still multicast as two 32-row halves across the CTA pair; the epilogue is
 // the same code over 32 accumulators per thread instead of 64.
+// map_n_hi / map_n_lo: the next layer's planes [p.rows][Cout], 64 x 16 boxes with 128-byte
+// swizzle (read only when p.next_hi is set).
 template <int BN, int EPI, bool PROF>
 __global__ void __launch_bounds__(kNumThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
                const __grid_constant__ CUtensorMap map_a_lo,
                const __grid_constant__ CUtensorMap map_w_hi,
-               const __grid_constant__ CUtensorMap map_w_lo, const ConvTcParams p) {
+               const __grid_constant__ CUtensorMap map_w_lo,
+               const __grid_constant__ CUtensorMap map_n_hi,
+               const __grid_constant__ CUtensorMap map_n_lo, const ConvTcParams p) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 511) &
-                                             ~static_cast<uintptr_t>(511));
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
+                                             ~static_cast<uintptr_t>(1023));
   using S = ConvSmem<BN>;
+  constexpr int kStages = S::kStages;
   constexpr int NR = BN / 2;    // accumulator registers per thread
   constexpr int NJ = BN / 8;    // 8-column groups per thread row
-  Barriers* bars = reinterpret_cast<Barriers*>(smem + kStages * S::kStageBytes);
+  Barriers<kStages>* bars = reinterpret_cast<Barriers<kStages>*>(smem + S::kBarOfs);
 
   // broadcast from lane 0: the compiler then knows the role branches are warp-uniform, which it
   // needs to give the consumer code the registers setmaxnreg grants
@@ -158,10 +179,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
         for (int r = 0; r < kCluster; ++r) mbar_arrive_cluster(mapa_shared(&bars->empty[s], r));
       }
     };
-    // PROF: wait full, MMA issue, chunk drain + promotion, epilogue, tiles, total
+    // PROF: wait full, MMA issue, chunk drain + promotion, epilogue, tiles, total, and two parts
+    // of the epilogue: ToRGB partials, next layer's planes (the rest of it is the per-element
+    // terms: constant loads, scale, noise, bias, activation, fp32 stores)
     // (32-bit clock differences: a launch runs for far fewer than 2^32 cycles)
     auto clk = [] { return static_cast<uint32_t>(clock()); };
-    uint32_t prof[6] = {0, 0, 0, 0, 0, 0};
+    uint32_t prof[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     uint32_t tp0 = 0, tp1 = 0;
     if constexpr (PROF) prof[5] = 0u - clk();
     int stage = 0;
@@ -224,6 +247,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
       uint32_t tid;
       asm volatile("mov.u32 %0, %%tid.x;\n" : "=r"(tid));
       const int row0 = m0 + ((tid >> 7) << 6) + (((tid >> 5) & 3) << 4) + ((tid & 31) >> 2);
+      // image and validity of the thread's two rows, for the next layer's planes after the row loop
+      const int Hv = p.ph_Hv[ph], Wv = p.ph_Wv[ph];
+      int rb[2];
+      bool rvalid[2];
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
         const int prow = row0 + 8 * i;
@@ -231,9 +258,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
         const int rem = prow - b * img;
         const int yy = rem / p.Wp;
         const int xx = rem - yy * p.Wp;
-        const int Hv = p.ph_Hv[ph], Wv = p.ph_Wv[ph];
         const bool in_rows = prow < p.rows;
         const bool valid = in_rows && (yy < Hv) && (xx < Wv);
+        rb[i] = b;
+        rvalid[i] = valid;
         const float* scl = (p.scale_bo && in_rows) ? p.scale_bo + static_cast<size_t>(b) * p.Cout : nullptr;
         float* outp = (p.out != nullptr && p.out_mode == 0 && valid)
                           ? p.out + p.ph_out_ofs[ph] + static_cast<size_t>(b) * p.out_sb +
@@ -300,42 +328,6 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
                 outp[static_cast<size_t>(n0 + 8 * j + 2 * c + e) * p.out_sc] = acc[4 * j + 2 * i + e];
           }
         }
-        if (EPI == 0 && p.rgb_w != nullptr) {
-          // one partial per 64-channel group: rgb_part[(n_tile*BN/64 + half)][b][c][y*Wv+x]; the
-          // four lanes of a row hold 16 of the group's channels each
-          const float* rw0 = p.rgb_w + (static_cast<size_t>(valid ? b : 0) * 3) * p.Cout + n0 + 2 * c;
-          const float* rw1 = rw0 + p.Cout;
-          const float* rw2 = rw1 + p.Cout;
-#pragma unroll
-          for (int half = 0; half < BN / 64; ++half) {
-            float r0 = 0.f, r1 = 0.f, r2 = 0.f;
-            if (valid) {
-#pragma unroll
-              for (int j = 8 * half; j < 8 * half + 8; ++j)
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                  const float t = acc[4 * j + 2 * i + e];
-                  r0 = fmaf(__ldg(rw0 + 8 * j + e), t, r0);
-                  r1 = fmaf(__ldg(rw1 + 8 * j + e), t, r1);
-                  r2 = fmaf(__ldg(rw2 + 8 * j + e), t, r2);
-                }
-            }
-#pragma unroll
-            for (int s = 1; s < 4; s <<= 1) {
-              r0 += __shfl_xor_sync(0xffffffffu, r0, s);
-              r1 += __shfl_xor_sync(0xffffffffu, r1, s);
-              r2 += __shfl_xor_sync(0xffffffffu, r2, s);
-            }
-            if (valid && c == 0) {
-              const size_t hw = static_cast<size_t>(Hv) * Wv;
-              float* rp = p.rgb_part + ((static_cast<size_t>(n_tile * (BN / 64) + half) * p.B + b) * 3) * hw +
-                          static_cast<size_t>(yy) * Wv + xx;
-              rp[0] = r0;
-              rp[hw] = r1;
-              rp[2 * hw] = r2;
-            }
-          }
-        }
         // channels-last raw rows are written for every row (pad rows are never read back)
         if (p.out != nullptr && p.out_mode == 1 && in_rows) {
           float* orow = p.out + (static_cast<size_t>(ph) * p.rows + prow) * p.Cout + n0 + 2 * c;
@@ -343,26 +335,118 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
           for (int j = 0; j < NJ; ++j)
             *reinterpret_cast<float2*>(orow + 8 * j) = make_float2(acc[4 * j + 2 * i], acc[4 * j + 2 * i + 1]);
         }
-        if (EPI == 0 && p.next_hi != nullptr && in_rows) {
-          const float* ns = p.next_scale + static_cast<size_t>(valid ? b : 0) * p.Cout + n0 + 2 * c;
-          const size_t ofs = static_cast<size_t>(prow) * p.Cout + n0 + 2 * c;
-          uint32_t* nh = reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(p.next_hi) + ofs);
-          uint32_t* nl = reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(p.next_lo) + ofs);
+      }
+      if (EPI == 0 && p.rgb_w != nullptr) {
+        if constexpr (PROF) tp1 = clk();
+        // one partial per 64-channel group: rgb_part[(n_tile*BN/64 + half)][b][c][y*Wv+x]; the
+        // four lanes of a row hold 16 of the group's channels each.  Both rows of the thread in
+        // one pass, which loads the weights once where the rows lie in the same image (all but
+        // the rows at an image boundary).  Pad rows sum too (only their own lanes see the sums)
+        // but store nothing.
+        const int wb0 = rvalid[0] ? rb[0] : 0, wb1 = rvalid[1] ? rb[1] : 0;
+        const float* wa = p.rgb_w + static_cast<size_t>(wb0) * 3 * p.Cout + n0 + 2 * c;
+        const float* wb = p.rgb_w + static_cast<size_t>(wb1) * 3 * p.Cout + n0 + 2 * c;
 #pragma unroll
-          for (int j = 0; j < NJ; ++j) {
-            float k0 = 0.f, k1 = 0.f;
-            if (valid) {
-              const float2 sv = __ldg(reinterpret_cast<const float2*>(ns + 8 * j));
-              k0 = sv.x * acc[4 * j + 2 * i];
-              k1 = sv.y * acc[4 * j + 2 * i + 1];
+        for (int half = 0; half < BN / 64; ++half) {
+          float r[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+          if (wb0 == wb1) {
+#pragma unroll
+            for (int j = 8 * half; j < 8 * half + 8; ++j)
+#pragma unroll
+              for (int e = 0; e < 2; ++e)
+#pragma unroll
+                for (int q = 0; q < 3; ++q) {
+                  const float w = __ldg(wa + q * p.Cout + 8 * j + e);
+                  r[0][q] = fmaf(w, acc[4 * j + e], r[0][q]);
+                  r[1][q] = fmaf(w, acc[4 * j + 2 + e], r[1][q]);
+                }
+          } else {
+#pragma unroll
+            for (int j = 8 * half; j < 8 * half + 8; ++j)
+#pragma unroll
+              for (int e = 0; e < 2; ++e)
+#pragma unroll
+                for (int q = 0; q < 3; ++q) {
+                  r[0][q] = fmaf(__ldg(wa + q * p.Cout + 8 * j + e), acc[4 * j + e], r[0][q]);
+                  r[1][q] = fmaf(__ldg(wb + q * p.Cout + 8 * j + e), acc[4 * j + 2 + e], r[1][q]);
+                }
+          }
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+#pragma unroll
+            for (int sh = 1; sh < 4; sh <<= 1)
+#pragma unroll
+              for (int q = 0; q < 3; ++q) r[i][q] += __shfl_xor_sync(0xffffffffu, r[i][q], sh);
+            if (rvalid[i] && c == 0) {
+              const int rem = row0 + 8 * i - rb[i] * img;
+              const int yy = rem / p.Wp;
+              const size_t hw = static_cast<size_t>(Hv) * Wv;
+              float* rp = p.rgb_part +
+                          ((static_cast<size_t>(n_tile * (BN / 64) + half) * p.B + rb[i]) * 3) * hw +
+                          static_cast<size_t>(yy) * Wv + (rem - yy * p.Wp);
+              rp[0] = r[i][0];
+              rp[hw] = r[i][1];
+              rp[2 * hw] = r[i][2];
             }
-            const __nv_bfloat162 hh = __floats2bfloat162_rn(k0, k1);
-            const float2 hf = __bfloat1622float2(hh);
-            const __nv_bfloat162 ll = __floats2bfloat162_rn(k0 - hf.x, k1 - hf.y);
-            nh[4 * j] = *reinterpret_cast<const uint32_t*>(&hh);
-            nl[4 * j] = *reinterpret_cast<const uint32_t*>(&ll);
           }
         }
+        if constexpr (PROF) prof[6] += clk() - tp1;
+      }
+      if (EPI == 0 && p.next_hi != nullptr) {
+        if constexpr (PROF) tp1 = clk();
+        // per 64-channel half: the bf16 hi / lo words of both rows (pad rows get zeros, the next
+        // layer's implicit zero padding), stmatrix'd into the warp's two slots, 16 x 16 words per
+        // stmatrix.x4 (matrices: rows 0-7 / 8-15 of column groups 2k, 2k + 1), then one TMA store
+        // per plane; rows past p.rows are clipped by it.  Lane t addresses row r = 8 (t / 8 % 2) +
+        // t % 8, 16-byte chunk 2k + t / 16 of its 128-byte slot row, swizzled by r % 8.
+        const int wq = static_cast<int>(tid >> 5);
+        const uint32_t slot_hi = smem_u32(smem + S::kSlotOfs + 2 * wq * kSlotBytes);
+        const uint32_t slot_lo = slot_hi + kSlotBytes;
+        const uint32_t r = ((tid >> 3) & 1) * 8 + (tid & 7);
+        const uint32_t jx = (tid >> 4) & 1;
+        const int srow = m0 + ((tid >> 7) << 6) + (((tid >> 5) & 3) << 4);
+#pragma unroll
+        for (int half = 0; half < BN / 64; ++half) {
+          uint32_t nxh[2][8], nxl[2][8];
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            const float* ns = p.next_scale + static_cast<size_t>(rvalid[i] ? rb[i] : 0) * p.Cout + n0 + 2 * c;
+#pragma unroll
+            for (int jj = 0; jj < 8; ++jj) {
+              const int j = 8 * half + jj;
+              float k0 = 0.f, k1 = 0.f;
+              if (rvalid[i]) {
+                const float2 sv = __ldg(reinterpret_cast<const float2*>(ns + 8 * j));
+                k0 = sv.x * acc[4 * j + 2 * i];
+                k1 = sv.y * acc[4 * j + 2 * i + 1];
+              }
+              const __nv_bfloat162 hh = __floats2bfloat162_rn(k0, k1);
+              const float2 hf = __bfloat1622float2(hh);
+              const __nv_bfloat162 ll = __floats2bfloat162_rn(k0 - hf.x, k1 - hf.y);
+              nxh[i][jj] = *reinterpret_cast<const uint32_t*>(&hh);
+              nxl[i][jj] = *reinterpret_cast<const uint32_t*>(&ll);
+            }
+          }
+          // the slots are free once the warp's previous stores have read them
+          if (lane == 0) tma_store_wait_read_n<0>();
+          __syncwarp();
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const int j = 2 * k;
+            const uint32_t a = r * 128 + (((2 * k + jx) ^ (r & 7)) << 4);
+            const uint32_t wh[4] = {nxh[0][j], nxh[1][j], nxh[0][j + 1], nxh[1][j + 1]};
+            const uint32_t wl[4] = {nxl[0][j], nxl[1][j], nxl[0][j + 1], nxl[1][j + 1]};
+            stmatrix_x4(slot_hi + a, wh);
+            stmatrix_x4(slot_lo + a, wl);
+          }
+          fence_proxy_async_smem();
+          __syncwarp();
+          if (lane == 0) {
+            tma_store_2d(&map_n_hi, slot_hi, n0 + 64 * half, srow);
+            tma_store_2d(&map_n_lo, slot_lo, n0 + 64 * half, srow);
+          }
+        }
+        if constexpr (PROF) prof[7] += clk() - tp1;
       }
       if constexpr (PROF) { prof[3] += clk() - tp0; prof[4] += 1; }
     }
@@ -371,7 +455,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
       if (lane == 0) {
         long long* dst = p.debug_prof + (static_cast<size_t>(blockIdx.x) * 8 + warp) * 8;
 #pragma unroll
-        for (int i = 0; i < 8; ++i) dst[i] = i < 6 ? prof[i] : 0;
+        for (int i = 0; i < 8; ++i) dst[i] = prof[i];
       }
     }
   } else {
@@ -415,6 +499,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi,
   // no CTA leaves while another CTA of its cluster can still multicast into its shared memory or
   // arrive on its barriers
   cluster_sync();
+  // nor while its plane stores still read their slots.  (Waited for here rather than at the end
+  // of the consumer branch, where ptxas then injects a warpgroup.wait into the main loop.)
+  if (EPI == 0 && warp < kTmaWarp && lane == 0) tma_store_wait_all();
 }
 
 }  // namespace
@@ -423,7 +510,7 @@ template <int BN, int EPI, bool PROF>
 static int conv_tc_launch_epi(const ConvTcParams& p, const void* a_hi, const void* a_lo,
                               const void* w_hi, const void* w_lo, int wk_total,
                               cudaStream_t stream) {
-  CUtensorMap ma_hi, ma_lo, mw_hi, mw_lo;
+  CUtensorMap ma_hi, ma_lo, mw_hi, mw_lo, mn_hi, mn_lo;
   int rc;
   // 64-byte swizzle: a box row is one k-block of BK = 32 channels
   const uint64_t a_cols = p.a_cols > 0 ? p.a_cols : p.Cin;
@@ -435,6 +522,16 @@ static int conv_tc_launch_epi(const ConvTcParams& p, const void* a_hi, const voi
   if ((rc = make_tmap_nd_bf16(&ma_lo, a_lo, 2, a_dims, a_str, a_box, nullptr, 3))) return rc;
   if ((rc = make_tmap_nd_bf16(&mw_hi, w_hi, 2, w_dims, w_str, w_box, nullptr, 3))) return rc;
   if ((rc = make_tmap_nd_bf16(&mw_lo, w_lo, 2, w_dims, w_str, w_box, nullptr, 3))) return rc;
+  // the next layer's planes: one warp's 16 rows x 64 channels per store, 128-byte swizzle
+  std::memset(&mn_hi, 0, sizeof(mn_hi));
+  std::memset(&mn_lo, 0, sizeof(mn_lo));
+  if (EPI == 0 && p.next_hi != nullptr) {
+    const uint64_t n_dims[2] = {static_cast<uint64_t>(p.Cout), static_cast<uint64_t>(p.rows)};
+    const uint64_t n_str[1] = {static_cast<uint64_t>(p.Cout) * 2};
+    const uint32_t n_box[2] = {64, 16};
+    if ((rc = make_tmap_nd_bf16(&mn_hi, p.next_hi, 2, n_dims, n_str, n_box, nullptr, 2))) return rc;
+    if ((rc = make_tmap_nd_bf16(&mn_lo, p.next_lo, 2, n_dims, n_str, n_box, nullptr, 2))) return rc;
+  }
 
   cudaLaunchConfig_t cfg = {};
   cudaLaunchAttribute attr[1];
@@ -469,7 +566,8 @@ static int conv_tc_launch_epi(const ConvTcParams& p, const void* a_hi, const voi
   const int num_units = (m_tiles + kCluster - 1) / kCluster * n_tiles * p.nphase;
   const int clusters = max_clusters < num_units ? max_clusters : num_units;
   cfg.gridDim = dim3(kCluster * clusters);
-  rc = check_cuda(cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN, EPI, PROF>, ma_hi, ma_lo, mw_hi, mw_lo, p),
+  rc = check_cuda(cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN, EPI, PROF>, ma_hi, ma_lo, mw_hi, mw_lo,
+                                     mn_hi, mn_lo, p),
                   "conv_tc launch");
   if (rc) return rc;
   return check_cuda(cudaGetLastError(), "conv_tc launch");
@@ -501,7 +599,8 @@ int conv_tc_launch(const ConvTcParams& p, const void* a_hi, const void* a_lo, co
     }
   // the epilogue's accesses, at offsets that keep each base pointer's alignment (Cout % 64 == 0,
   // even column): float2 loads of next_scale, and of scale_bo on the pad rows of a channels-last
-  // store; float2 stores of channels-last out; bf16 pairs stored as uint32 into next_hi / next_lo
+  // store; float2 stores of channels-last out; bf16 pairs into next_hi / next_lo, which TMA stores
+  // also need 16-byte aligned (checked below)
   const struct {
     const void* ptr;
     unsigned align;
@@ -521,6 +620,11 @@ int conv_tc_launch(const ConvTcParams& p, const void* a_hi, const void* a_lo, co
   for (const auto& n : need)
     if (n.ptr != nullptr && (reinterpret_cast<uintptr_t>(n.ptr) & (n.align - 1)) != 0) {
       set_last_error("conv_tc: %s (%p) is not %u-byte aligned", n.name, n.ptr, n.align);
+      return RW_ERR_BAD_ARG;
+    }
+  for (int i = 6; i < 8; ++i)      // next_hi, next_lo
+    if (need[i].ptr != nullptr && (reinterpret_cast<uintptr_t>(need[i].ptr) & 15u) != 0) {
+      set_last_error("conv_tc: %s (%p) is not 16-byte aligned (TMA store)", need[i].name, need[i].ptr);
       return RW_ERR_BAD_ARG;
     }
   // 128-channel tiles wherever Cout allows them; 64 only for the 64-channel layers

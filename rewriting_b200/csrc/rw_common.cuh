@@ -165,6 +165,48 @@ __device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const CUte
       : "memory");
 }
 
+// TMA stores (shared -> global, bulk async-group completion).  Each store is committed as a group
+// of its own; the smem source must not be rewritten before a wait_group.read has covered it, and
+// the writes that filled it need a fence_proxy_async_smem() before the store is issued.
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, uint32_t smem_src, int32_t c0,
+                                             int32_t c1) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];\n" ::"l"(
+          reinterpret_cast<uint64_t>(m)),
+      "r"(smem_src), "r"(c0), "r"(c1)
+      : "memory");
+  asm volatile("cp.async.bulk.commit_group;\n" ::: "memory");
+}
+__device__ __forceinline__ void tma_store_5d(const CUtensorMap* m, uint32_t smem_src, int32_t c0,
+                                             int32_t c1, int32_t c2, int32_t c3, int32_t c4) {
+  asm volatile(
+      "cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];\n" ::"l"(
+          reinterpret_cast<uint64_t>(m)),
+      "r"(smem_src), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
+      : "memory");
+  asm volatile("cp.async.bulk.commit_group;\n" ::: "memory");
+}
+// at most N of this thread's store groups still read shared memory
+template <int N>
+__device__ __forceinline__ void tma_store_wait_read_n() {
+  asm volatile("cp.async.bulk.wait_group.read %0;\n" ::"n"(N) : "memory");
+}
+// every store group of this thread is complete (issued before the CTA exits)
+__device__ __forceinline__ void tma_store_wait_all() {
+  asm volatile("cp.async.bulk.wait_group 0;\n" ::: "memory");
+}
+
+// ---------------------------------------------------------------------------
+// stmatrix: four 8x8 b16 matrices: register i of lane t is row t/4, 32-bit column t%4 of matrix
+// i; lane t supplies the address of row t%8 of matrix t/8.  The wgmma accumulator fragment of an
+// 8-column group, packed to bf16 pairs, is one such matrix per 8-row half.
+// ---------------------------------------------------------------------------
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};\n" ::"r"(addr),
+               "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3])
+               : "memory");
+}
+
 // ---------------------------------------------------------------------------
 // wgmma: warpgroup MMA, bf16 x bf16 -> fp32 register accumulators, operands in shared memory
 // ---------------------------------------------------------------------------

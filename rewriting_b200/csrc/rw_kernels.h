@@ -42,7 +42,8 @@ struct ConvTcParams {
   // out_mode 1: channels-last rows  out[(ph*rows + p)*Cout + o]  for every row p < rows
   int out_mode;
   // fused producer outputs (generation fast path): the NEXT layer's key planes
-  //   next_{hi,lo}[p][o] = split_bf16(next_scale[b,o] * y)   (zero at pad positions)
+  //   next_{hi,lo}[p][o] = split_bf16(next_scale[b,o] * y)   (zero at pad positions), written by
+  //   TMA stores: 16-byte aligned
   void* next_hi;
   void* next_lo;
   const float* next_scale;   // [B, Cout] style of the consuming layer

@@ -128,10 +128,6 @@ __device__ __forceinline__ void lds_v4(uint32_t a, float& x, float& y, float& z,
 
 // named barriers: 1, 2 = mailbox of a channel half; 3 + q = the two warps of lane quarter q
 constexpr int kBarPair = 3;
-template <int N>
-__device__ __forceinline__ void tma_store_wait_read_n() {
-  asm volatile("cp.async.bulk.wait_group.read %0;\n" ::"n"(N) : "memory");
-}
 
 struct UpItem {
   int bg, band, cg;
@@ -151,27 +147,6 @@ __device__ __forceinline__ UpItem decode_item(int item, const UpFusedParams& p) 
   it.y_first = ya - 2 < 0 ? 0 : ya - 2;
   it.y_end = yb;
   return it;
-}
-
-// four 8x8 b16 matrices: register i of lane t is row t/4, 32-bit column t%4 of matrix i; lane t
-// supplies the address of row t%8 of matrix t/8
-__device__ __forceinline__ void stmatrix_x4(uint32_t addr, const uint32_t (&r)[4]) {
-  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};\n" ::"r"(addr),
-               "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3])
-               : "memory");
-}
-
-__device__ __forceinline__ void tma_store_5d(const CUtensorMap* m, uint32_t smem_src, int32_t c0,
-                                             int32_t c1, int32_t c2, int32_t c3, int32_t c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];\n" ::"l"(
-          reinterpret_cast<uint64_t>(m)),
-      "r"(smem_src), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
-  asm volatile("cp.async.bulk.commit_group;\n" ::: "memory");
-}
-__device__ __forceinline__ void tma_store_wait_all() {
-  asm volatile("cp.async.bulk.wait_group 0;\n" ::: "memory");
 }
 
 // PROF = true: bring-up variant that accumulates, per epilogue warp, the cycles spent in each phase

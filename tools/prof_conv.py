@@ -5,7 +5,9 @@ last layer) and ToRGB partials, no fp32 output.
 1. Cycles per tile that a consumer warp spends in each phase (clock()-instrumented variant,
    rw_debug_conv_profile): waiting on full barriers, issuing the main loop's MMAs, chunk drains +
    promotion, the epilogue.  The tensor pipe idles during the epilogue, since both consumer
-   warpgroups of a CTA reach it together.
+   warpgroups of a CTA reach it together.  The epilogue is split further into the per-element
+   terms (constant loads, scale, noise, bias, activation), the ToRGB partials and the next
+   layer's planes.
 2. CUDA-event time of the product kernel, warm, mean over `--iters` launches, for every styled
    conv of the 256^2 generator at batch 32 (layers 2, 4, ..., 14).
 
@@ -22,6 +24,8 @@ from rewriting_b200 import _cabi, ops  # noqa: E402
 LAYERS = {2: (512, 4), 4: (512, 8), 6: (512, 16), 8: (512, 32), 10: (512, 64), 12: (256, 128),
           14: (128, 256)}
 PHASES = ['wait full barrier', 'MMA issue', 'chunk drain + promotion', 'epilogue']
+# debug_prof slots 6, 7; the per-element terms are the rest of the epilogue (slot 3)
+EPI_PARTS = ['ToRGB partials', "next layer's planes"]
 
 
 def make_args(B, Cin, Cout, H, last):
@@ -80,6 +84,10 @@ def phase_profile(name, B, Cin, Cout, H, last, iters):
           (name, B, Cin, Cout, H, us, tiles / active.sum(), p[:, :, 5][active].mean() / 1e3))
     for i, n in enumerate(PHASES):
         print('  %-26s %8.0f cycles/tile' % (n, p[:, :, i].sum() / tiles))
+    parts = [p[:, :, 6 + i].sum() / tiles for i in range(len(EPI_PARTS))]
+    print('    %-24s %8.0f' % ('per-element terms', p[:, :, 3].sum() / tiles - sum(parts)))
+    for n, v in zip(EPI_PARTS, parts):
+        print('    %-24s %8.0f' % (n, v))
     del keep
 
 
