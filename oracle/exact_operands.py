@@ -4,8 +4,9 @@ reads, so that `got - ref` is the kernel's own accumulation error.
 Every product the kernels form is hi·hi + lo·hi + hi·lo of bf16 planes.  Each bf16·bf16 product and
 every sum of a few thousand of them is exact in float64 (to ~2^-40), so `three` below returns the
 kernel's product without rounding, together with the per-output sum of |terms| that its error is
-measured against.  Used by tests/test_gpu_tc_accumulation.py (one kernel at a time) and
-tests/test_gpu_fastpath_layers.py (the generation fast path, layer by layer).
+measured against.  Used by tests/test_gpu_tc_accumulation.py (one kernel at a time),
+tests/test_gpu_fastpath_layers.py (the generation fast path, layer by layer) and
+tests/test_gpu_backward_layers.py (the StyledConv backward, launch by launch).
 """
 import torch
 
@@ -53,3 +54,26 @@ def wupf64(u_hi, u_lo, Cout, Cin):
     float64 conv_transpose2d weights [Cin, Cout, 3, 3]."""
     return tuple(t.view(Cout // 16, 2, 9, 8, Cin).permute(0, 1, 3, 2, 4).reshape(Cout, 3, 3, Cin)
                  .permute(3, 0, 1, 2).double() for t in (u_hi, u_lo))
+
+
+def wdgrad(t, Cout, Cin):
+    """`dgrad` weight planes ([Cin][flipped tap][Cout], rw_prep_weights transpose_io = 1, flip 1)
+    in the Parameter's layout [Cout, Cin, 3, 3]: plane[i][8 - tap][o] holds W[o, i, tap]."""
+    return t.view(Cin, 9, Cout).flip(1).permute(2, 0, 1).reshape(Cout, Cin, 3, 3)
+
+
+def wdgrad_up(t, Cout, Cin):
+    """`dgrad_up` weight planes ([Cin][tap][Cout], taps not flipped) in the Parameter's layout
+    [Cout, Cin, 3, 3]."""
+    return t.view(Cin, 9, Cout).permute(2, 0, 1).reshape(Cout, Cin, 3, 3)
+
+
+def phase_planes(t, B, C, H, W):
+    """Four-phase gradient planes [B·(H+1)·(W+1)][4·C] (column block ph = a·2 + b of row (b, m, n)
+    holds position (2m + a, 2n + b) of a [B, C, 2H+1, 2W+1] map) as (map, pads): the map
+    [B, C, 2H+1, 2W+1] and the positions past it, row 2H+1 and column 2W+1 of the [2H+2, 2W+2]
+    grid the planes tile, which must be zero."""
+    g = t.view(B, H + 1, W + 1, 2, 2, C).permute(0, 5, 1, 3, 2, 4).reshape(B, C, 2 * H + 2,
+                                                                            2 * W + 2)
+    pads = torch.cat([g[:, :, 2 * H + 1, :].reshape(-1), g[:, :, :, 2 * W + 1].reshape(-1)])
+    return g[:, :, :2 * H + 1, :2 * W + 1], pads

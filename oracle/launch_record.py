@@ -1,5 +1,6 @@
 """TEST INFRASTRUCTURE ONLY — the launch recorder and the per-launch checks that the segmenters'
-launch-by-launch tests (tests/test_gpu_segmenter_layers.py, tests/test_gpu_semseg_layers.py) share.
+launch-by-launch tests (tests/test_gpu_segmenter_layers.py, tests/test_gpu_semseg_layers.py) share;
+tests/test_gpu_backward_layers.py records the StyledConv backward with it (`autograd=True`).
 
 `observe` runs a forward with `torch.empty` / `torch.empty_like` and `_cabi.call` wrapped: every
 tensor the run allocates and every launch (entry point and arguments, in order) is recorded, and
@@ -42,15 +43,40 @@ _IO = {
     'rw_seg_avgpool': (0, None, (6,)),
     'rw_seg_classes': (None, None, (12, 13)),
     'rw_semseg_classes': (None, None, (14, 15)),
+    # the StyledConv forward and backward (tests/test_gpu_backward_layers.py)
+    'rw_prep_keys': (0, None, (6, 7, 8)),
+    'rw_prep_weights': (0, None, (6, 7, 8)),
+    'rw_demod': (0, None, (6,)),
+    'rw_modconv_fwd': (0, None, (15,)),
+    'rw_modconv_up_fused_y': (0, None, (11,)),
+    'rw_modconv_up_fwd': (0, None, (10,)),
+    'rw_blur_up_act': (0, None, (11,)),
+    'rw_torgb': (0, None, (10,)),
+    'rw_act_grad_reduce': (0, None, (10, 11, 12, 13)),
+    'rw_blur_adj_phase_keys': (0, None, (7, 8)),
+    'rw_prep_phase_keys': (0, None, (6, 7)),
+    'rw_modconv_up_dgrad': (0, None, (10,)),
+    'rw_conv_wgrad': (0, None, (8,)),
+    'rw_conv_up_wgrad': (0, None, (8,)),
+    'rw_dgrad_finish': (0, None, (0, 6)),
+    'rw_style_grad_finish': (0, None, (8,)),
+    'rw_wgrad_finish': (0, None, (9,)),
+    'rw_torgb_mod_bwd': (3, None, (9, 10, 11)),
+    'rw_upfirdn2d': (0, None, (15,)),
+    'rw_fused_bias_act': (0, None, (10,)),
 }
 # the map passes' (C, hi, lo, ldc, coff) argument indices
 _SLICE = {'rw_seg_map': (3, 12, 13, 14, 15), 'rw_seg_map_phase': (4, 14, 15, 16, 17)}
+# operands a launch overwrites in place (snapshotted before it) and workspace arguments
+_INPLACE = {'rw_dgrad_finish': (0,)}
+_WORKSPACE = {'rw_conv_wgrad': 9, 'rw_conv_up_wgrad': 9, 'rw_torgb_mod_bwd': 12}
 
 
 # ------------------------------------------------------------------ observation
 class Run(object):
     def __init__(self):
         self.calls, self.tensors, self.slices = [], [], {}
+        self.before = {}        # launch index -> {argument index: the operand before the launch}
 
 
 def ptr(a):
@@ -66,13 +92,21 @@ def _poison(t):
         t.fill_(POISON if t.dtype == torch.int64 else torch.iinfo(t.dtype).min)
 
 
-def observe(monkeypatch, fn, poison=False):
+def observe(monkeypatch, fn, poison=False, autograd=False):
     """(record, fn()) with every allocation and launch of fn recorded; each slice write of a map
     pass is followed by a comparison of the planes' other channels with their state before it.
-    With `poison` every allocation is filled with NaN / POISON first."""
-    from rewriting_b200 import _cabi
+    With `poison` every allocation is filled with NaN / POISON first.
+
+    `autograd` (the StyledConv backward): the run starts with empty weight-plane and workspace
+    caches (`ops._WEIGHT_CACHE`, `ops._WS`), so both are allocated, poisoned and filled inside it;
+    every tensor the ops layer hands a kernel (`ops._f32c`: autograd's incoming gradients, the
+    saved inputs) is recorded too; an operand a launch overwrites in place is snapshotted into
+    `run.before` first; with `poison`, every workspace is refilled with NaN right before each
+    launch that takes it, so no launch can depend on what an earlier one left there."""
+    from rewriting_b200 import _cabi, ops
     run = Run()
     real_empty, real_empty_like, real_call = torch.empty, torch.empty_like, _cabi.call
+    real_f32c = ops._f32c
 
     def keep(t):
         if poison:
@@ -86,6 +120,12 @@ def observe(monkeypatch, fn, poison=False):
     def empty_like(*a, **k):
         return keep(real_empty_like(*a, **k))
 
+    def f32c(t):
+        t = real_f32c(t)
+        if t is not None:
+            run.tensors.append(t)
+        return t
+
     def find(p):
         for t in reversed(run.tensors):
             if t.data_ptr() == p:
@@ -95,6 +135,11 @@ def observe(monkeypatch, fn, poison=False):
     def call(name, *args):
         i = len(run.calls)
         run.calls.append((name, args))
+        if autograd:
+            if name in _INPLACE:
+                run.before[i] = {j: find(ptr(args[j])).clone() for j in _INPLACE[name]}
+            if poison and name in _WORKSPACE:
+                find(ptr(args[_WORKSPACE[name]])).fill_(float('nan'))
         if name not in _SLICE:
             return real_call(name, *args)
         ic, ih, il, ild, ico = _SLICE[name]
@@ -116,9 +161,20 @@ def observe(monkeypatch, fn, poison=False):
         m.setattr(torch, 'empty', empty)
         m.setattr(torch, 'empty_like', empty_like)
         m.setattr(_cabi, 'call', call)
+        if autograd:
+            m.setattr(ops, '_f32c', f32c)
+            m.setattr(ops, '_WS', {})
+            m.setattr(ops, '_WEIGHT_CACHE', {})
         out = fn()
-    torch.cuda.synchronize()
+        torch.cuda.synchronize()
     return run, out
+
+
+def _numel(shape):
+    n = 1
+    for s in shape:
+        n *= s
+    return n
 
 
 class Tensors(object):
@@ -135,8 +191,22 @@ class Tensors(object):
             self.map.setdefault(t.data_ptr(), t)
 
     def __call__(self, a, *shape):
-        t = self.map[ptr(a)]
-        return t.reshape(shape) if shape else t
+        p = ptr(a)
+        t = self.map.get(p)
+        if not shape:
+            return self.map[p]
+        if t is None or t.numel() != _numel(shape):   # a part of a recorded tensor (a row of a
+            t = self.inside(p, shape)                 # [3, B, C] reduction)
+        return t.reshape(shape)
+
+    def inside(self, p, shape):
+        n = _numel(shape)
+        for t in self.map.values():
+            e = t.element_size()
+            if t.is_contiguous() and t.data_ptr() <= p and p + n * e <= t.data_ptr() + t.numel() * e:
+                off = (p - t.data_ptr()) // e
+                return t.view(-1)[off:off + n]
+        raise KeyError('%#x' % p)
 
 
 def conv_tensors(convs):
