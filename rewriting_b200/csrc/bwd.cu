@@ -13,8 +13,8 @@
 //   style_grad_finish                -> g_style incl. the demodulation term
 //
 // All reductions are block-local trees (bit-reproducible, no atomics).
+#include "../../include/rewriting_b200.h"
 #include "rw_common.cuh"
-#include "rw_kernels.h"
 
 namespace rw {
 
@@ -332,10 +332,21 @@ inline int plane_threads(int HW, int vec) {
 
 }  // namespace
 
-int act_grad_reduce_launch(const float* gy, const float* y, const float* noise,
-                           long long noise_bstride, const float* noise_w, const float* bias,
-                           int act, int B, int C, int HW, float* g_pre, float* s_sum,
-                           float* s_dot, float* s_noise, cudaStream_t stream) {
+}  // namespace rw
+
+using namespace rw;
+
+extern "C" {
+
+int rw_act_grad_reduce(const float* gy, const float* y, const float* noise,
+                       long long noise_bstride, const float* noise_w, const float* bias, int act,
+                       int B, int C, int HW, float* g_pre, float* s_sum, float* s_dot,
+                       float* s_noise, rw_stream_t stream) {
+  if (!gy || !y || !s_sum || !s_dot || !s_noise || B < 0 || C < 1 || HW < 0 ||
+      (noise && !noise_w)) {
+    set_last_error("rw_act_grad_reduce: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   const long long planes = static_cast<long long>(B) * C;
   if (planes <= 0 || HW <= 0) return RW_OK;
   if (planes > 0x7fffffffLL) {
@@ -349,8 +360,12 @@ int act_grad_reduce_launch(const float* gy, const float* y, const float* noise,
   return check_cuda(cudaGetLastError(), "act_grad_reduce launch");
 }
 
-int blur_adj_phase_launch(const float* g_pre, const float* scale_bc, const float* k4, int B, int C,
-                          int H, int W, void* hi, void* lo, cudaStream_t stream) {
+int rw_blur_adj_phase_keys(const float* g_pre, const float* scale_bc, const float* k4, int B,
+                           int C, int H, int W, void* hi, void* lo, rw_stream_t stream) {
+  if (!g_pre || !k4 || !hi || !lo || B < 1 || H < 1 || W < 1) {
+    set_last_error("rw_blur_adj_phase_keys: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   if (C % 64 != 0) {
     set_last_error("blur_adj_phase: C=%d must be a multiple of 64", C);
     return RW_ERR_BAD_ARG;
@@ -367,8 +382,12 @@ int blur_adj_phase_launch(const float* g_pre, const float* scale_bc, const float
   return check_cuda(cudaGetLastError(), "blur_adj_phase launch");
 }
 
-int dgrad_finish_launch(float* dk, const float* x, const float* style, int B, int C, int HW,
-                        float* gs_raw, cudaStream_t stream) {
+int rw_dgrad_finish(float* dk, const float* x, const float* style, int B, int C, int HW,
+                    float* gs_raw, rw_stream_t stream) {
+  if (!dk || !x || !style || !gs_raw || B < 0 || C < 1 || HW < 0) {
+    set_last_error("rw_dgrad_finish: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   const long long planes = static_cast<long long>(B) * C;
   if (planes <= 0 || HW <= 0) return RW_OK;
   if (planes > 0x7fffffffLL) {
@@ -381,22 +400,30 @@ int dgrad_finish_launch(float* dk, const float* x, const float* style, int B, in
   return check_cuda(cudaGetLastError(), "dgrad_finish launch");
 }
 
-int wgrad_finish_launch(const float* dwt, const float* w, const float* s_dot, const float* dm,
-                        const float* style, int B, int Cout, int Cin, float sc, float* gw,
-                        cudaStream_t stream) {
+int rw_wgrad_finish(const float* dwt, const float* w, const float* s_dot, const float* dm,
+                    const float* style, int B, int Cout, int Cin, float sc, float* gw,
+                    rw_stream_t stream) {
+  if (!dwt || !w || !gw || Cout < 1 || Cin < 1 || (s_dot && (!dm || !style || B < 1))) {
+    set_last_error("rw_wgrad_finish: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   const int n = Cout * Cin;
   wgrad_finish_kernel<<<(n + 127) / 128, 128, 0, stream>>>(dwt, w, s_dot, dm, style, B, Cout, Cin,
                                                            sc, gw);
   return check_cuda(cudaGetLastError(), "wgrad_finish launch");
 }
 
-int style_grad_finish_launch(const float* gs_raw, const float* style, const float* s_dot,
-                             const float* dm, const float* wsq, int B, int Cout, int Cin,
-                             float* g_style, cudaStream_t stream) {
+int rw_style_grad_finish(const float* gs_raw, const float* style, const float* s_dot,
+                         const float* dm, const float* wsq, int B, int Cout, int Cin,
+                         float* g_style, rw_stream_t stream) {
+  if (!style || !g_style || B < 1 || Cin < 1 || (s_dot && (!dm || !wsq || Cout < 1))) {
+    set_last_error("rw_style_grad_finish: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   const int n = B * Cin;
   style_grad_finish_kernel<<<(n + 127) / 128, 128, 0, stream>>>(gs_raw, style, s_dot, dm, wsq, B,
                                                                 Cout, Cin, g_style);
   return check_cuda(cudaGetLastError(), "style_grad_finish launch");
 }
 
-}  // namespace rw
+}  // extern "C"

@@ -31,10 +31,56 @@
 #include <cstdlib>
 #include <cstring>
 
+#include "../../include/rewriting_b200.h"
 #include "rw_common.cuh"
-#include "rw_kernels.h"
 
 namespace rw {
+
+struct ConvTcParams {
+  int rows;          // padded-flat rows = B * Hp * Wp  (GEMM M)
+  int Cin;           // GEMM K per tap
+  int Cout;          // GEMM N
+  // Up to 4 "phases" share one launch (the 4 polyphase components of a stride-2
+  // conv_transpose): tile index = (m, n, phase) with phase fastest, so the CTAs that
+  // run concurrently read the same A tiles (L2 hits instead of 4 DRAM passes).
+  int nphase;
+  int ph_ntaps[4];
+  int ph_shift[4][9];   // row shift applied to the A operand for this tap
+  int ph_kofs[4][9];    // column offset of this tap inside the weight matrix
+  int ph_acol[4][9];    // column offset of this tap inside the A planes (0 unless A holds
+                        // several channel-concatenated tensors, e.g. the 4 gradient phases)
+  int a_cols;           // total columns of the A planes (0 -> Cin)
+  int ph_Hv[4], ph_Wv[4];       // valid output extent inside the padded grid
+  long long ph_out_ofs[4];      // element offset of this phase's output origin
+  int Hp, Wp;        // padded grid of one image
+  int B;             // batch (only needed for the rgb partial layout)
+  // epilogue
+  const float* scale_bo;  // [B, Cout] per-sample per-channel scale (demod / style) or null
+  const float* bias;      // [Cout] or null
+  const float* noise;     // [B, noise_bstride] or null, indexed y*Wv + x
+  long long noise_bstride;
+  const float* noise_w;   // device scalar (read by the kernel: no host sync per layer)
+  int act;                // 1 -> leaky_relu(0.2) * act_gain
+  float act_gain;         // 0 -> sqrt(2) (FusedLeakyReLU); ProgGAN's nn.LeakyReLU uses 1
+  float* out;             // may be null when only planes / rgb partials are wanted
+  long long out_sb, out_sc, out_sy, out_sx;  // element strides: batch, channel, y, x
+  // out_mode 0: strided (NCHW-like) store at valid positions only
+  // out_mode 1: channels-last rows  out[(ph*rows + p)*Cout + o]  for every row p < rows
+  int out_mode;
+  // fused producer outputs (generation fast path): the NEXT layer's key planes
+  //   next_{hi,lo}[p][o] = split_bf16(next_scale[b,o] * y)   (zero at pad positions), written by
+  //   TMA stores: 16-byte aligned
+  void* next_hi;
+  void* next_lo;
+  const float* next_scale;   // [B, Cout] style of the consuming layer
+  // and this layer's ToRGB partial sums over the tile's 128 output channels
+  //   rgb_part[nt][b][c][y*Wv+x] = sum_{o in tile} rgb_w[b][c][o] * y[b,o,y,x]
+  float* rgb_part;
+  const float* rgb_w;        // [B, 3, Cout] modulated 1x1 weights
+  // non-null: launch the clock()-instrumented variant, which writes per-phase cycles of every
+  // consumer warp to debug_prof[grid][8][8] (rw_debug_conv_profile)
+  long long* debug_prof;
+};
 
 namespace {
 
@@ -584,8 +630,10 @@ static int conv_tc_launch_bn(const ConvTcParams& p, const void* a_hi, const void
   return conv_tc_launch_epi<BN, 0, false>(p, a_hi, a_lo, w_hi, w_lo, wk_total, stream);
 }
 
-int conv_tc_launch(const ConvTcParams& p, const void* a_hi, const void* a_lo, const void* w_hi,
-                   const void* w_lo, int wk_total, cudaStream_t stream) {
+// the one launch behind every entry point below: checks the shape and the epilogue's alignment,
+// then picks the tile width and the epilogue variant
+static int conv_tc_launch(const ConvTcParams& p, const void* a_hi, const void* a_lo,
+                          const void* w_hi, const void* w_lo, int wk_total, cudaStream_t stream) {
   // the stated limit (DESIGN.md §1) stays Cin % 64, although the kernel only needs Cin % BK
   if (p.Cin % 64 != 0 || p.Cout % 64 != 0 || p.nphase < 1 || p.nphase > 4 || p.rows <= 0) {
     set_last_error("conv_tc: unsupported shape Cin=%d Cout=%d nphase=%d rows=%d", p.Cin, p.Cout,
@@ -632,4 +680,249 @@ int conv_tc_launch(const ConvTcParams& p, const void* a_hi, const void* a_lo, co
   return conv_tc_launch_bn<64>(p, a_hi, a_lo, w_hi, w_lo, wk_total, stream);
 }
 
+// the 3x3 same-size conv over the padded-flat grid of B images H x W: one phase of 9 taps,
+// NCHW output strides
+static int fill_conv3x3(ConvTcParams& p, const char* who, int B, int Cin, int Cout, int H, int W) {
+  memset(&p, 0, sizeof(p));
+  p.Hp = H + 1;
+  p.Wp = W + 1;
+  p.B = B;
+  p.nphase = 1;
+  p.ph_Hv[0] = H;
+  p.ph_Wv[0] = W;
+  const long long rows = static_cast<long long>(B) * p.Hp * p.Wp;
+  if (rows > 0x7fffffffLL) {
+    set_last_error("%s: too many rows", who);
+    return RW_ERR_BAD_ARG;
+  }
+  p.rows = static_cast<int>(rows);
+  p.Cin = Cin;
+  p.Cout = Cout;
+  p.ph_ntaps[0] = 9;
+  for (int u = 0; u < 3; ++u)
+    for (int v = 0; v < 3; ++v) {
+      p.ph_shift[0][u * 3 + v] = (u - 1) * p.Wp + (v - 1);
+      p.ph_kofs[0][u * 3 + v] = (u * 3 + v) * Cin;
+    }
+  p.out_sb = static_cast<long long>(Cout) * H * W;
+  p.out_sc = static_cast<long long>(H) * W;
+  p.out_sy = W;
+  p.out_sx = 1;
+  return RW_OK;
+}
+
+static int modconv_up_impl(const void* kp_hi, const void* kp_lo, const void* wt_hi,
+                           const void* wt_lo, const float* scale_bo, int B, int Cin, int Cout,
+                           int H, int W, float* t_out, int channels_last, rw_stream_t stream) {
+  if (!kp_hi || !kp_lo || !wt_hi || !wt_lo || !t_out || B < 1) {
+    set_last_error("rw_modconv_up_fwd: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  // conv_transpose2d(stride 2, pad 0, k 3): out[2m+a, 2n+b] gathers
+  //   a == 0: (u=0, in row m), (u=2, in row m-1);  a == 1: (u=1, in row m)   (same along x)
+  // over the padded-flat grid every phase is a row-GEMM with <= 4 shifted taps.
+  const int Hp = H + 1, Wp = W + 1;
+  const int Ht = 2 * H + 1, Wt = 2 * W + 1;
+  const long long rows = static_cast<long long>(B) * Hp * Wp;
+  if (rows > 0x7fffffffLL) {
+    set_last_error("rw_modconv_up_fwd: too many rows");
+    return RW_ERR_BAD_ARG;
+  }
+  ConvTcParams p;
+  memset(&p, 0, sizeof(p));
+  p.Hp = Hp;
+  p.Wp = Wp;
+  p.B = B;
+  p.rows = static_cast<int>(rows);
+  p.Cin = Cin;
+  p.Cout = Cout;
+  p.nphase = 4;
+  p.scale_bo = scale_bo;
+  p.out = t_out;
+  p.out_sb = static_cast<long long>(Cout) * Ht * Wt;
+  p.out_sc = static_cast<long long>(Ht) * Wt;
+  p.out_sy = 2LL * Wt;
+  p.out_sx = 2;
+  p.out_mode = channels_last ? 1 : 0;
+  // heaviest phase first within every (m, n) group: (0,0) has 4 taps, (1,1) has 1
+  for (int a = 0; a < 2; ++a) {
+    for (int b = 0; b < 2; ++b) {
+      const int ph = a * 2 + b;
+      p.ph_Hv[ph] = Hp - a;
+      p.ph_Wv[ph] = Wp - b;
+      p.ph_out_ofs[ph] = static_cast<long long>(a) * Wt + b;
+      int us[2], dys[2], nu;
+      int vs[2], dxs[2], nv;
+      if (a == 0) { nu = 2; us[0] = 0; dys[0] = 0; us[1] = 2; dys[1] = -1; }
+      else        { nu = 1; us[0] = 1; dys[0] = 0; }
+      if (b == 0) { nv = 2; vs[0] = 0; dxs[0] = 0; vs[1] = 2; dxs[1] = -1; }
+      else        { nv = 1; vs[0] = 1; dxs[0] = 0; }
+      int n = 0;
+      for (int iu = 0; iu < nu; ++iu)
+        for (int iv = 0; iv < nv; ++iv) {
+          p.ph_shift[ph][n] = dys[iu] * Wp + dxs[iv];
+          p.ph_kofs[ph][n] = (us[iu] * 3 + vs[iv]) * Cin;
+          ++n;
+        }
+      p.ph_ntaps[ph] = n;
+    }
+  }
+  return conv_tc_launch(p, kp_hi, kp_lo, wt_hi, wt_lo, 9 * Cin, stream);
+}
+
+static int modconv_fused_impl(const void* kp_hi, const void* kp_lo, const void* wt_hi,
+                              const void* wt_lo, const float* scale_bo, const float* noise,
+                              long long noise_bstride, const float* noise_w, const float* bias,
+                              int act, int B, int Cin, int Cout, int H, int W, float* out,
+                              const float* next_scale, void* next_hi, void* next_lo,
+                              const float* rgb_w, float* rgb_part, long long* prof_out,
+                              rw_stream_t stream) {
+  if (!kp_hi || !kp_lo || !wt_hi || !wt_lo || B < 1 || (noise && !noise_w) ||
+      ((next_hi != nullptr) != (next_lo != nullptr)) || (next_hi && !next_scale) ||
+      ((rgb_w != nullptr) != (rgb_part != nullptr)) || (!out && !next_hi && !rgb_part)) {
+    set_last_error("rw_modconv_fwd_fused: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  ConvTcParams p;
+  int rc = fill_conv3x3(p, "rw_modconv_fwd_fused", B, Cin, Cout, H, W);
+  if (rc) return rc;
+  p.scale_bo = scale_bo;
+  p.bias = bias;
+  p.noise = noise;
+  p.noise_bstride = noise_bstride;
+  p.noise_w = noise_w;
+  p.act = act;
+  p.out = out;
+  p.next_hi = next_hi;
+  p.next_lo = next_lo;
+  p.next_scale = next_scale;
+  p.rgb_w = rgb_w;
+  p.rgb_part = rgb_part;
+  p.debug_prof = prof_out;
+  return conv_tc_launch(p, kp_hi, kp_lo, wt_hi, wt_lo, 9 * Cin, stream);
+}
+
 }  // namespace rw
+
+using namespace rw;
+
+extern "C" {
+
+int rw_modconv_fwd(const void* kp_hi, const void* kp_lo, const void* wt_hi, const void* wt_lo,
+                   const float* scale_bo, const float* noise, long long noise_bstride,
+                   const float* noise_w, const float* bias, int act, int B, int Cin, int Cout,
+                   int H, int W, float* out, rw_stream_t stream) {
+  if (!kp_hi || !kp_lo || !wt_hi || !wt_lo || !out || B < 1 || (noise && !noise_w)) {
+    set_last_error("rw_modconv_fwd: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  ConvTcParams p;
+  int rc = fill_conv3x3(p, "rw_modconv_fwd", B, Cin, Cout, H, W);
+  if (rc) return rc;
+  p.scale_bo = scale_bo;
+  p.bias = bias;
+  p.noise = noise;
+  p.noise_bstride = noise_bstride;
+  p.noise_w = noise_w;
+  p.act = act;
+  p.out = out;
+  return conv_tc_launch(p, kp_hi, kp_lo, wt_hi, wt_lo, 9 * Cin, stream);
+}
+
+int rw_modconv_up_fwd(const void* kp_hi, const void* kp_lo, const void* wt_hi, const void* wt_lo,
+                      const float* scale_bo, int B, int Cin, int Cout, int H, int W, float* t_out,
+                      rw_stream_t stream) {
+  return modconv_up_impl(kp_hi, kp_lo, wt_hi, wt_lo, scale_bo, B, Cin, Cout, H, W, t_out, 0, stream);
+}
+
+int rw_modconv_up_fwd_cl(const void* kp_hi, const void* kp_lo, const void* wt_hi,
+                         const void* wt_lo, const float* scale_bo, int B, int Cin, int Cout, int H,
+                         int W, float* t_cl, rw_stream_t stream) {
+  return modconv_up_impl(kp_hi, kp_lo, wt_hi, wt_lo, scale_bo, B, Cin, Cout, H, W, t_cl, 1, stream);
+}
+
+int rw_conv3x3_bias_act(const void* kp_hi, const void* kp_lo, const void* wt_hi, const void* wt_lo,
+                        const float* bias, int act, float act_gain, int B, int Cin, int Cout, int H,
+                        int W, float* out, rw_stream_t stream) {
+  if (!kp_hi || !kp_lo || !wt_hi || !wt_lo || !out || B < 1) {
+    set_last_error("rw_conv3x3_bias_act: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  ConvTcParams p;
+  int rc = fill_conv3x3(p, "rw_conv3x3_bias_act", B, Cin, Cout, H, W);
+  if (rc) return rc;
+  p.bias = bias;
+  p.act = act;
+  p.act_gain = act_gain;
+  p.out = out;
+  return conv_tc_launch(p, kp_hi, kp_lo, wt_hi, wt_lo, 9 * Cin, stream);
+}
+
+int rw_modconv_fwd_fused(const void* kp_hi, const void* kp_lo, const void* wt_hi,
+                         const void* wt_lo, const float* scale_bo, const float* noise,
+                         long long noise_bstride, const float* noise_w, const float* bias, int act,
+                         int B, int Cin, int Cout, int H, int W, float* out,
+                         const float* next_scale, void* next_hi, void* next_lo,
+                         const float* rgb_w, float* rgb_part, rw_stream_t stream) {
+  return modconv_fused_impl(kp_hi, kp_lo, wt_hi, wt_lo, scale_bo, noise, noise_bstride, noise_w,
+                            bias, act, B, Cin, Cout, H, W, out, next_scale, next_hi, next_lo, rgb_w,
+                            rgb_part, nullptr, stream);
+}
+
+int rw_debug_conv_profile(const void* kp_hi, const void* kp_lo, const void* wt_hi,
+                          const void* wt_lo, const float* scale_bo, const float* noise,
+                          long long noise_bstride, const float* noise_w, const float* bias, int act,
+                          int B, int Cin, int Cout, int H, int W, float* out,
+                          const float* next_scale, void* next_hi, void* next_lo,
+                          const float* rgb_w, float* rgb_part, long long* prof_out,
+                          rw_stream_t stream) {
+  if (!prof_out) {
+    set_last_error("rw_debug_conv_profile: prof_out is null");
+    return RW_ERR_BAD_ARG;
+  }
+  return modconv_fused_impl(kp_hi, kp_lo, wt_hi, wt_lo, scale_bo, noise, noise_bstride, noise_w,
+                            bias, act, B, Cin, Cout, H, W, out, next_scale, next_hi, next_lo, rgb_w,
+                            rgb_part, prof_out, stream);
+}
+
+// tap (u,v) of the stride-2 conv_transpose reads gradient phase (u&1, v&1) at row shift
+// (u>>1)*(W+1) + (v>>1) of the INPUT-resolution padded grid.
+int rw_modconv_up_dgrad(const void* gph_hi, const void* gph_lo, const void* wt_hi,
+                        const void* wt_lo, const float* scale_bi, int B, int Cin, int Cout, int H,
+                        int W, float* dk, rw_stream_t stream) {
+  if (!gph_hi || !gph_lo || !wt_hi || !wt_lo || !dk || B < 1) {
+    set_last_error("rw_modconv_up_dgrad: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  // GEMM: M = input pixels, K = 9 taps x Cout (gradient channels), N = Cin
+  ConvTcParams p;
+  int rc = fill_conv3x3(p, "rw_modconv_up_dgrad", B, /*Cin(K)=*/Cout, /*Cout(N)=*/Cin, H, W);
+  if (rc) return rc;
+  p.a_cols = 4 * Cout;
+  for (int u = 0; u < 3; ++u)
+    for (int v = 0; v < 3; ++v) {
+      const int t = u * 3 + v;
+      p.ph_shift[0][t] = (u >> 1) * p.Wp + (v >> 1);
+      p.ph_acol[0][t] = ((u & 1) * 2 + (v & 1)) * Cout;
+      p.ph_kofs[0][t] = t * Cout;
+    }
+  p.scale_bo = scale_bi;
+  p.out = dk;
+  return conv_tc_launch(p, gph_hi, gph_lo, wt_hi, wt_lo, 9 * Cout, stream);
+}
+
+int rw_rowgemm(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo, int rows, int K,
+               int N, float* out, rw_stream_t stream) {
+  if (!a_hi || !a_lo || !w_hi || !w_lo || !out || rows < 1 || K % 64 != 0 || N % 64 != 0) {
+    set_last_error("rw_rowgemm: bad argument (rows=%d K=%d N=%d)", rows, K, N);
+    return RW_ERR_BAD_ARG;
+  }
+  ConvTcParams p;
+  memset(&p, 0, sizeof(p));
+  p.rows = rows; p.Cin = K; p.Cout = N; p.nphase = 1; p.ph_ntaps[0] = 1;
+  p.Hp = 1; p.Wp = rows; p.ph_Hv[0] = 1; p.ph_Wv[0] = rows;   // one "image" = all rows
+  p.out = out; p.out_sb = 0; p.out_sc = 1; p.out_sy = 0; p.out_sx = N;  // row-major [rows][N]
+  return conv_tc_launch(p, a_hi, a_lo, w_hi, w_lo, K, stream);
+}
+
+}  // extern "C"

@@ -16,8 +16,8 @@
 // popcount of their AND — a binary GEMM over the labels present only, never over all C.
 #include <cmath>
 
+#include "../../include/rewriting_b200.h"
 #include "rw_common.cuh"
-#include "rw_kernels.h"
 
 namespace rw {
 
@@ -247,8 +247,14 @@ bool sizes_ok(int B, int U, int h, int w, int H, int W, const Grid& g) {
 
 }  // namespace
 
-int upsample_bilinear_launch(const float* act, int B, int U, int h, int w, int H, int W, double sy,
-                             double oy, double sx, double ox, float* rows, cudaStream_t stream) {
+}  // namespace rw
+
+using namespace rw;
+
+extern "C" {
+
+int rw_upsample_bilinear(const float* act, int B, int U, int h, int w, int H, int W, double sy,
+                         double oy, double sx, double ox, float* rows, rw_stream_t stream) {
   const Grid g{sy, oy, sx, ox};
   if (!act || !rows || !sizes_ok(B, U, h, w, H, W, g)) {
     set_last_error("upsample_bilinear: bad argument B=%d U=%d %dx%d -> %dx%d (sizes 1..1024, grid "
@@ -261,10 +267,10 @@ int upsample_bilinear_launch(const float* act, int B, int U, int h, int w, int H
   return check_cuda(cudaGetLastError(), "upsample_bilinear");
 }
 
-int dissect_counts_launch(const float* act, const float* level, const long long* labels, int B, int U,
-                          int h, int w, int H, int W, int K, int C, double sy, double oy, double sx,
-                          double ox, long long* isect, long long* unit_total, long long* label_total,
-                          long long* count, cudaStream_t stream) {
+int rw_dissect_counts(const float* act, const float* level, const long long* labels, int B, int U,
+                      int h, int w, int H, int W, int K, int C, double sy, double oy, double sx,
+                      double ox, long long* isect, long long* unit_total, long long* label_total,
+                      long long* count, rw_stream_t stream) {
   const Grid g{sy, oy, sx, ox};
   if (!act || !level || !labels || !isect || !unit_total || !label_total || !count ||
       !sizes_ok(B, U, h, w, H, W, g) || K < 1 || K > 8 || C < 2 || C > 32768 ||
@@ -295,4 +301,4 @@ int dissect_counts_launch(const float* act, const float* level, const long long*
   return check_cuda(cudaGetLastError(), "dissect_counts");
 }
 
-}  // namespace rw
+}  // extern "C"

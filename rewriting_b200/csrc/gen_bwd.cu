@@ -1,8 +1,8 @@
 // gen_bwd.cu — backward of the StyleGAN2 generator's modulated 1x1 ToRGB conv under autograd (its
 // forward is torgb_kernel of simt.cu).  fp32 on CUDA cores; every output is summed in a fixed order
 // with no atomics, so two calls on the same input give the same bits.
+#include "../../include/rewriting_b200.h"
 #include "rw_common.cuh"
-#include "rw_kernels.h"
 
 namespace rw {
 
@@ -190,16 +190,26 @@ int torgb_mod_chunks(int H, int W) {
 
 }  // namespace
 
-size_t torgb_mod_bwd_workspace_bytes(int B, int C, int H, int W) {
+}  // namespace rw
+
+using namespace rw;
+
+extern "C" {
+
+size_t rw_torgb_mod_bwd_workspace_bytes(int B, int C, int H, int W) {
   if (!torgb_mod_shape_ok(B, C, H, W)) return 0;
   // part [B][chunks][3][C], then t [B][3][C]
   return (static_cast<size_t>(B) * (torgb_mod_chunks(H, W) + 1) * 3 * C) * sizeof(float);
 }
 
-int torgb_mod_bwd_launch(const float* x, const float* style, const float* w, const float* gy, int B,
-                         int C, int H, int W, float scale, float* gx, float* gs, float* gw,
-                         void* workspace, size_t workspace_bytes, cudaStream_t stream) {
-  const size_t need = torgb_mod_bwd_workspace_bytes(B, C, H, W);
+int rw_torgb_mod_bwd(const float* x, const float* style, const float* w, const float* gy, int B,
+                     int C, int H, int W, float scale, float* gx, float* gs, float* gw,
+                     void* workspace, size_t workspace_bytes, rw_stream_t stream) {
+  if (!x || !style || !w || !gy || !workspace || (!gx && !gs && !gw)) {
+    set_last_error("rw_torgb_mod_bwd: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  const size_t need = rw_torgb_mod_bwd_workspace_bytes(B, C, H, W);
   if (need == 0 || workspace_bytes < need) {
     set_last_error("torgb_mod_bwd: bad shape or workspace %zu < %zu bytes (B=%d C=%d H=%d W=%d)",
                    workspace_bytes, need, B, C, H, W);
@@ -228,4 +238,4 @@ int torgb_mod_bwd_launch(const float* x, const float* style, const float* w, con
   return check_cuda(cudaGetLastError(), "torgb_mod_wsum launch");
 }
 
-}  // namespace rw
+}  // extern "C"

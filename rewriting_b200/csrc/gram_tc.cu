@@ -16,10 +16,35 @@
 // + hi*lo), fp32 accumulate in registers.  Row ranges are split across CTAs;
 // partial tiles go to a workspace that a second kernel reduces in a fixed order
 // (bit-reproducible, unlike atomics).
+#include <cstring>
+
+#include "../../include/rewriting_b200.h"
 #include "rw_common.cuh"
-#include "rw_kernels.h"
 
 namespace rw {
+
+struct GramTcParams {
+  int rows;            // contraction length (rows r in [0, rows))
+  int rows_a, rows_b;  // allocated rows of the A / B planes (for the TMA bounds)
+  int Cm, Cn;          // channels of A (-> M) and B (-> N)
+  int shift_a, shift_b;
+  int ntaps;              // >= 1; grid.z
+  int tap_shift_a[9];     // extra row shift of the A operand per tap
+  int tap_acol[9];        // column offset inside the A planes per tap
+  int a_cols;             // total columns of the A planes (0 -> Cm)
+  int tap_shift_b[9];     // extra row shift of the B operand per tap
+  int tap_col_ofs[9];     // column offset of this tap's block inside a partial row
+  int splits;          // row-range splits (partials reduced deterministically afterwards)
+  float* partial;      // [splits][Cm][ldp] fp32 workspace
+  long long ldp;       // leading dimension (elements) of one partial matrix row
+  int upper_only;      // 1: skip tiles strictly below the diagonal (symmetric A==B)
+};
+
+// the col-GEMM's tile extent along a channel dimension of C (C % 64 == 0): 128 where it divides C
+inline int gram_tile_width(int C) { return C % 128 == 0 ? 128 : 64; }
+inline int gram_tiles(int Cm, int Cn) {
+  return (Cm / gram_tile_width(Cm)) * (Cn / gram_tile_width(Cn));
+}
 
 namespace {
 
@@ -264,8 +289,8 @@ static int gram_tc_launch_tile(const GramTcParams& p, const CUtensorMap& ma_hi,
   return check_cuda(cudaGetLastError(), "gram_tc launch");
 }
 
-int gram_tc_launch(const GramTcParams& p, const void* a_hi, const void* a_lo, const void* b_hi,
-                   const void* b_lo, cudaStream_t stream) {
+static int gram_tc_launch(const GramTcParams& p, const void* a_hi, const void* a_lo,
+                          const void* b_hi, const void* b_lo, cudaStream_t stream) {
   if (p.Cm % 64 != 0 || p.Cn % 64 != 0 || p.Cm < 64 || p.Cn < 64 || p.rows <= 0 || p.splits < 1 ||
       p.ntaps < 1 || p.ntaps > 9) {
     set_last_error("gram_tc: unsupported shape Cm=%d Cn=%d rows=%d splits=%d", p.Cm, p.Cn, p.rows,
@@ -298,13 +323,129 @@ int gram_tc_launch(const GramTcParams& p, const void* a_hi, const void* a_lo, co
   return gram_tc_launch_tile<64, 64>(p, ma_hi, ma_lo, mb_hi, mb_lo, stream);
 }
 
-int reduce_partials_launch(const float* partial, int splits, int M, int N, long long ldp,
-                           float* out, long long ldo, int accumulate, int mirror_upper,
-                           cudaStream_t stream) {
+// out[m*ldo+n] (= or +=) sum_s partial[s][m][n]; optional symmetric mirror of the
+// upper triangle into the lower one.
+static int reduce_partials_launch(const float* partial, int splits, int M, int N, long long ldp,
+                                  float* out, long long ldo, int accumulate, int mirror_upper,
+                                  cudaStream_t stream) {
   dim3 grid((N + 31) / 32, (M + 31) / 32);
   reduce_partials_kernel<<<grid, 256, 0, stream>>>(partial, splits, M, N, ldp, out, ldo, accumulate,
                                                    mirror_upper);
   return check_cuda(cudaGetLastError(), "reduce_partials launch");
 }
 
+// split heuristic shared by the workspace query and the launches; upper_only (symmetric output)
+// runs only the tiles on and above the diagonal
+static int gram_splits(int Cm, int Cn, long long rows, int ntaps, bool upper_only) {
+  const int mt = Cm / gram_tile_width(Cm);
+  const int tiles = upper_only ? mt * (mt + 1) / 2 : gram_tiles(Cm, Cn);
+  const long long total_rb = (rows + 63) / 64;
+  const int sms = device_sm_count();
+  long long s = (sms + static_cast<long long>(tiles) * ntaps - 1) / (static_cast<long long>(tiles) * ntaps);
+  if (s > total_rb) s = total_rb;
+  if (s < 1) s = 1;
+  if (s > 64) s = 64;
+  return static_cast<int>(s);
+}
+
+// The col-GEMM behind every gram entry point.  p holds the shape (Cm, Cn, ntaps, upper_only,
+// a_cols) and the tap tables; this sets the row range, the splits and the partials' layout, checks
+// the workspace, launches, and reduces the partials into out [Cm][ntaps * Cn] (+= when accumulate,
+// mirrored into the lower triangle when upper_only).
+static int gram_run(const char* who, GramTcParams& p, long long rows, const void* a_hi,
+                    const void* a_lo, const void* b_hi, const void* b_lo, float* out, int accumulate,
+                    void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  p.rows = p.rows_a = p.rows_b = static_cast<int>(rows);
+  p.splits = gram_splits(p.Cm, p.Cn, rows, p.ntaps, p.upper_only != 0);
+  p.ldp = static_cast<long long>(p.ntaps) * p.Cn;
+  p.partial = static_cast<float*>(workspace);
+  const size_t need = static_cast<size_t>(p.splits) * p.Cm * p.ldp * sizeof(float);
+  if (workspace_bytes < need) {
+    set_last_error("%s: workspace %zu < %zu bytes", who, workspace_bytes, need);
+    return RW_ERR_BAD_ARG;
+  }
+  int rc = gram_tc_launch(p, a_hi, a_lo, b_hi, b_lo, stream);
+  if (rc) return rc;
+  return reduce_partials_launch(p.partial, p.splits, p.Cm, static_cast<int>(p.ldp), p.ldp, out,
+                                p.ldp, accumulate, p.upper_only, stream);
+}
+
 }  // namespace rw
+
+using namespace rw;
+
+extern "C" {
+
+size_t rw_gram_workspace_bytes(int Cm, int Cn, long long rows, int ntaps) {
+  if (Cm < 64 || Cn < 64 || Cm % 64 != 0 || Cn % 64 != 0 || ntaps < 1) return 0;
+  // the symmetric path uses fewer tiles -> more splits; size for the larger of the two
+  const int s1 = gram_splits(Cm, Cn, rows, ntaps, false);
+  const int s2 = gram_splits(Cm, Cn, rows, ntaps, Cm == Cn);
+  const int s = s1 > s2 ? s1 : s2;
+  return static_cast<size_t>(s) * Cm * static_cast<size_t>(Cn) * ntaps * sizeof(float);
+}
+
+int rw_second_moment_accum(const void* hi, const void* lo, long long rows, int C, float* mom2,
+                           void* workspace, size_t workspace_bytes, rw_stream_t stream) {
+  if (rows == 0) return RW_OK;
+  if (!hi || !lo || !mom2 || !workspace || rows < 0 || rows > 0x7fffffffLL || C < 64 || C % 64 != 0) {
+    set_last_error("rw_second_moment_accum: bad argument (rows=%lld C=%d)", rows, C);
+    return RW_ERR_BAD_ARG;
+  }
+  GramTcParams p;
+  memset(&p, 0, sizeof(p));
+  p.Cm = p.Cn = C;
+  p.ntaps = 1;
+  p.upper_only = 1;
+  return gram_run("rw_second_moment_accum", p, rows, hi, lo, hi, lo, mom2, /*accumulate=*/1,
+                  workspace, workspace_bytes, stream);
+}
+
+int rw_conv_wgrad(const void* g_hi, const void* g_lo, const void* kp_hi, const void* kp_lo,
+                  long long rows, int Cout, int Cin, int Wp, float* dw_toi, void* workspace,
+                  size_t workspace_bytes, rw_stream_t stream) {
+  if (!g_hi || !g_lo || !kp_hi || !kp_lo || !dw_toi || !workspace || rows <= 0 ||
+      rows > 0x7fffffffLL) {
+    set_last_error("rw_conv_wgrad: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  GramTcParams p;
+  memset(&p, 0, sizeof(p));
+  p.Cm = Cout;
+  p.Cn = Cin;
+  p.ntaps = 9;
+  for (int u = 0; u < 3; ++u)
+    for (int v = 0; v < 3; ++v) {
+      p.tap_shift_b[u * 3 + v] = (u - 1) * Wp + (v - 1);
+      p.tap_col_ofs[u * 3 + v] = (u * 3 + v) * Cin;
+    }
+  return gram_run("rw_conv_wgrad", p, rows, g_hi, g_lo, kp_hi, kp_lo, dw_toi, /*accumulate=*/0,
+                  workspace, workspace_bytes, stream);
+}
+
+int rw_conv_up_wgrad(const void* gph_hi, const void* gph_lo, const void* kp_hi, const void* kp_lo,
+                     long long rows, int Cout, int Cin, int Wp, float* dw_toi, void* workspace,
+                     size_t workspace_bytes, rw_stream_t stream) {
+  if (!gph_hi || !gph_lo || !kp_hi || !kp_lo || !dw_toi || !workspace || rows <= 0 ||
+      rows > 0x7fffffffLL) {
+    set_last_error("rw_conv_up_wgrad: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  GramTcParams p;
+  memset(&p, 0, sizeof(p));
+  p.Cm = Cout;
+  p.Cn = Cin;
+  p.a_cols = 4 * Cout;
+  p.ntaps = 9;
+  for (int u = 0; u < 3; ++u)
+    for (int v = 0; v < 3; ++v) {
+      const int t = u * 3 + v;
+      p.tap_shift_a[t] = (u >> 1) * Wp + (v >> 1);
+      p.tap_acol[t] = ((u & 1) * 2 + (v & 1)) * Cout;
+      p.tap_col_ofs[t] = t * Cin;
+    }
+  return gram_run("rw_conv_up_wgrad", p, rows, gph_hi, gph_lo, kp_hi, kp_lo, dw_toi,
+                  /*accumulate=*/0, workspace, workspace_bytes, stream);
+}
+
+}  // extern "C"

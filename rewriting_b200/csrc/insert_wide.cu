@@ -27,8 +27,8 @@
 // each key value feeds 9 taps as in the plain conv.  The blur and its adjoint run on the planes
 // in the workspace: T, g (2h x 2w) and gT = demod * blur^T(g), from which the weight gradient is
 // dW[o,i,u,v] = sc * sum gT[2y+u, 2x+v] k[i,y,x] - (the demod term, unchanged).
+#include "../../include/rewriting_b200.h"
 #include "rw_common.cuh"
-#include "rw_kernels.h"
 #include "insert_linear.cuh"
 
 namespace rw {
@@ -609,8 +609,8 @@ int wide_launch_mode(const InsertLoopParams& p, const float* blur, void* workspa
                                                 : "NULL blur kernel");
     return RW_ERR_BAD_ARG;
   }
-  const size_t need = kUp ? insert_up_workspace_bytes(p.Cout, p.B, p.h, p.w)
-                          : insert_wide_workspace_bytes(p.Cout, p.B, p.h, p.w);
+  const size_t need = kUp ? rw_insert_up_workspace_bytes(p.Cout, p.B, p.h, p.w)
+                          : rw_insert_wide_workspace_bytes(p.Cout, p.B, p.h, p.w);
   if (workspace == nullptr || workspace_bytes < need) {
     set_last_error("%s: workspace %zu B < %zu B needed", who, workspace_bytes, need);
     return RW_ERR_BAD_ARG;
@@ -643,13 +643,19 @@ int wide_launch_mode(const InsertLoopParams& p, const float* blur, void* workspa
 
 }  // namespace
 
-size_t insert_wide_workspace_bytes(int Cout, int B, int h, int w) {
+}  // namespace rw
+
+using namespace rw;
+
+extern "C" {
+
+size_t rw_insert_wide_workspace_bytes(int Cout, int B, int h, int w) {
   if (Cout < 1 || B < 1 || h < 1 || w < 1) return 0;
   const size_t cout4 = (static_cast<size_t>(Cout) + OC - 1) / OC * OC;
   return 2 * cout4 * static_cast<size_t>(B) * h * w * sizeof(float);
 }
 
-size_t insert_up_workspace_bytes(int Cout, int B, int h, int w) {
+size_t rw_insert_up_workspace_bytes(int Cout, int B, int h, int w) {
   if (Cout < 1 || B < 1 || h < 1 || w < 1) return 0;
   const size_t cout4 = (static_cast<size_t>(Cout) + OC - 1) / OC * OC;
   const size_t t_px = static_cast<size_t>(2 * h + 1) * (2 * w + 1);   // T and gT
@@ -657,24 +663,36 @@ size_t insert_up_workspace_bytes(int Cout, int B, int h, int w) {
   return cout4 * static_cast<size_t>(B) * (2 * t_px + g_px) * sizeof(float);
 }
 
-int insert_wide_launch(const InsertLoopParams& p, void* workspace, size_t workspace_bytes,
-                       cudaStream_t stream) {
+int rw_insert_loop_wide(const rw_insert_args* a, void* workspace, size_t workspace_bytes,
+                        rw_stream_t stream) {
+  InsertLoopParams p;
+  int rc = insert_params(a, "rw_insert_loop_wide", p);
+  if (rc) return rc;
   return wide_launch_mode<false, false>(p, nullptr, workspace, workspace_bytes, stream);
 }
 
-int linear_insert_wide_launch(const InsertLoopParams& p, void* workspace, size_t workspace_bytes,
-                              cudaStream_t stream) {
+int rw_linear_insert_loop_wide(const rw_linear_insert_args* a, void* workspace,
+                               size_t workspace_bytes, rw_stream_t stream) {
+  InsertLoopParams p;
+  int rc = linear_insert_params(a, "rw_linear_insert_loop_wide", p);
+  if (rc) return rc;
   return wide_launch_mode<true, false>(p, nullptr, workspace, workspace_bytes, stream);
 }
 
-int insert_up_launch(const InsertLoopParams& p, const float* blur, void* workspace,
-                     size_t workspace_bytes, cudaStream_t stream) {
+int rw_insert_loop_up(const rw_insert_args* a, const float blur[16], void* workspace,
+                      size_t workspace_bytes, rw_stream_t stream) {
+  InsertLoopParams p;
+  int rc = insert_params(a, "rw_insert_loop_up", p);
+  if (rc) return rc;
   return wide_launch_mode<false, true>(p, blur, workspace, workspace_bytes, stream);
 }
 
-int linear_insert_up_launch(const InsertLoopParams& p, const float* blur, void* workspace,
-                            size_t workspace_bytes, cudaStream_t stream) {
+int rw_linear_insert_loop_up(const rw_linear_insert_args* a, const float blur[16], void* workspace,
+                             size_t workspace_bytes, rw_stream_t stream) {
+  InsertLoopParams p;
+  int rc = linear_insert_params(a, "rw_linear_insert_loop_up", p);
+  if (rc) return rc;
   return wide_launch_mode<true, true>(p, blur, workspace, workspace_bytes, stream);
 }
 
-}  // namespace rw
+}  // extern "C"

@@ -15,8 +15,8 @@
 //            taps summed in order), written if asked for; or the masked L1 sum_c |im1 - im0| read
 //            from the image sets directly; either way the per-image sums of D*w and w over
 //            1024-pixel tiles into a workspace, then a fixed-order finish per image.
+#include "../../include/rewriting_b200.h"
 #include "rw_common.cuh"
-#include "rw_kernels.h"
 
 namespace rw {
 
@@ -256,7 +256,7 @@ int combine_run(CombineParams& P, bool l1, bool u8, double* num, double* den, vo
   P.ntiles = static_cast<int>((hw + kTile - 1) / kTile);
   P.part = nullptr;
   if (num) {
-    const size_t need = lpips_combine_workspace_bytes(P.B, P.H, P.W);
+    const size_t need = rw_lpips_combine_workspace_bytes(P.B, P.H, P.W);
     if (!workspace || workspace_bytes < need || (reinterpret_cast<uintptr_t>(workspace) & 7u)) {
       set_last_error("%s: workspace %zu < %zu bytes or not 8-byte aligned", what, workspace_bytes, need);
       return RW_ERR_BAD_ARG;
@@ -273,8 +273,18 @@ int combine_run(CombineParams& P, bool l1, bool u8, double* num, double* den, vo
 
 }  // namespace
 
-int lpips_input_launch(const void* im0, const void* im1, int u8, int B, int H, int W, float* out,
-                       cudaStream_t stream) {
+}  // namespace rw
+
+using namespace rw;
+
+extern "C" {
+
+int rw_lpips_input(const void* im0, const void* im1, int u8, int B, int H, int W, float* out,
+                   rw_stream_t stream) {
+  if (!im0 || !im1 || !out) {
+    set_last_error("rw_lpips_input: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   if (bad_image_shape(B, H, W) || (u8 != 0 && u8 != 1)) {
     set_last_error("lpips_input: bad shape or format B=%d H=%d W=%d u8=%d", B, H, W, u8);
     return RW_ERR_BAD_ARG;
@@ -287,8 +297,12 @@ int lpips_input_launch(const void* im0, const void* im1, int u8, int B, int H, i
   return check_cuda(cudaGetLastError(), "lpips_input");
 }
 
-int lpips_head_launch(const float* a, const float* bias, const float* lin_w, int B, int C, int h,
-                      int w, float* d, cudaStream_t stream) {
+int rw_lpips_head(const float* a, const float* bias, const float* lin_w, int B, int C, int h, int w,
+                  float* d, rw_stream_t stream) {
+  if (!a || !lin_w || !d) {
+    set_last_error("rw_lpips_head: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   const long long hw = static_cast<long long>(h) * w;
   if (B < 1 || C < 1 || h < 1 || w < 1 || B > 65535 || (hw + 31) / 32 > 0x7fffffffLL ||
       C * hw >= (1LL << 40)) {
@@ -300,15 +314,19 @@ int lpips_head_launch(const float* a, const float* bias, const float* lin_w, int
   return check_cuda(cudaGetLastError(), "lpips_head");
 }
 
-size_t lpips_combine_workspace_bytes(int B, int H, int W) {
+size_t rw_lpips_combine_workspace_bytes(int B, int H, int W) {
   if (bad_image_shape(B, H, W)) return 0;
   const long long ntiles = (static_cast<long long>(H) * W + kTile - 1) / kTile;
   return static_cast<size_t>(B) * ntiles * 2 * sizeof(double);
 }
 
-int lpips_combine_launch(int nmaps, const float* const* maps, const int* map_hw, int B, int H, int W,
-                         const float* mask, int mask_b, float* D, double* num, double* den,
-                         void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+int rw_lpips_combine(int nmaps, const float* const* maps, const int* map_hw, int B, int H, int W,
+                     const float* mask, int mask_b, float* D, double* num, double* den,
+                     void* workspace, size_t workspace_bytes, rw_stream_t stream) {
+  if (!maps || !map_hw) {
+    set_last_error("rw_lpips_combine: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   if (nmaps < 1 || nmaps > kMaxMaps) {
     set_last_error("lpips_combine: nmaps=%d outside 1..%d", nmaps, kMaxMaps);
     return RW_ERR_BAD_ARG;
@@ -329,9 +347,13 @@ int lpips_combine_launch(int nmaps, const float* const* maps, const int* map_hw,
   return combine_run(P, false, false, num, den, workspace, workspace_bytes, stream, "lpips_combine");
 }
 
-int masked_l1_launch(const void* im0, const void* im1, int u8, int B, int H, int W, const float* mask,
-                     int mask_b, double* num, double* den, void* workspace, size_t workspace_bytes,
-                     cudaStream_t stream) {
+int rw_masked_l1(const void* im0, const void* im1, int u8, int B, int H, int W, const float* mask,
+                 int mask_b, double* num, double* den, void* workspace, size_t workspace_bytes,
+                 rw_stream_t stream) {
+  if (!im0 || !im1) {
+    set_last_error("rw_masked_l1: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   if ((u8 != 0 && u8 != 1) || !num) {
     set_last_error("masked_l1: u8 must be 0 or 1 and num, den given (u8=%d)", u8);
     return RW_ERR_BAD_ARG;
@@ -343,4 +365,4 @@ int masked_l1_launch(const void* im0, const void* im1, int u8, int B, int H, int
   return combine_run(P, true, u8 != 0, num, den, workspace, workspace_bytes, stream, "masked_l1");
 }
 
-}  // namespace rw
+}  // extern "C"

@@ -4,8 +4,8 @@
 // 1024² generators) and the 1x1 ToRGB.  Every kernel reads and writes fp32 NCHW, sums in a fixed
 // order (two calls on the same input are bit-identical), and takes no tensor-core path: these
 // layers are narrow, so their cost is memory and the shared-memory operand reuse below.
+#include "../../include/rewriting_b200.h"
 #include "rw_common.cuh"
-#include "rw_kernels.h"
 
 namespace rw {
 
@@ -433,40 +433,10 @@ bool sizes_ok(long long B, long long a, long long b, long long H, long long W) {
 
 }  // namespace
 
-int proggan_input_fwd_launch(const float* z, const float* w, const float* bias, float wscale, int B,
-                             int Z, int C, float* out, cudaStream_t stream) {
-  if (B < 1 || Z < 1 || C < 1 || C > 2147483647 / 16) {
-    set_last_error("proggan_input_fwd: bad shape B=%d Z=%d C=%d", B, Z, C);
-    return RW_ERR_BAD_ARG;
-  }
-  dim3 grid(C, (B + 15) / 16);
-  input_layer_fwd_kernel<<<grid, 256, 0, stream>>>(z, w, B, Z, C, wscale, bias, out);
-  return check_cuda(cudaGetLastError(), "proggan_input_fwd launch");
-}
-
-int proggan_input_bwd_launch(const float* z, const float* w, const float* gy, int B, int Z, int C,
-                             float* gz, float* gw, cudaStream_t stream) {
-  if (B < 1 || Z < 1 || C < 1 || !aligned16(gy) || (gz && !aligned16(w)) || (gw && !aligned16(gw))) {
-    set_last_error("proggan_input_bwd: bad shape or alignment (B=%d Z=%d C=%d; w, gy and gw need "
-                   "16-byte alignment)", B, Z, C);
-    return RW_ERR_BAD_ARG;
-  }
-  if (gz) {
-    dim3 grid((Z + 127) / 128, (B + kInBwdB - 1) / kInBwdB);
-    input_layer_dgrad_kernel<<<grid, 128, 0, stream>>>(gy, w, B, Z, C, gz);
-    int rc = check_cuda(cudaGetLastError(), "proggan_input_bwd dgrad launch");
-    if (rc) return rc;
-  }
-  if (gw) {
-    dim3 grid((Z + 255) / 256, C);
-    input_layer_wgrad_kernel<<<grid, 256, 0, stream>>>(gy, z, B, Z, C, gw);
-    return check_cuda(cudaGetLastError(), "proggan_input_bwd wgrad launch");
-  }
-  return RW_OK;
-}
-
-int narrow_conv3x3_launch(const float* x, const float* w, const float* bias, float wscale, int B,
-                          int Cin, int Cout, int H, int W, int flip, float* out, cudaStream_t stream) {
+// flip = 1: the dgrad (conv with W[i][o][8 - tap]; Cin / Cout are the dgrad's)
+static int narrow_conv3x3_launch(const float* x, const float* w, const float* bias, float wscale,
+                                 int B, int Cin, int Cout, int H, int W, int flip, float* out,
+                                 cudaStream_t stream) {
   if (!sizes_ok(B, Cin, Cout, H, W) || (Cout + kNcCo - 1) / kNcCo > 65535) {
     set_last_error("narrow_conv3x3: bad shape B=%d Cin=%d Cout=%d H=%d W=%d", B, Cin, Cout, H, W);
     return RW_ERR_BAD_ARG;
@@ -487,15 +457,103 @@ int narrow_conv3x3_launch(const float* x, const float* w, const float* bias, flo
   return check_cuda(cudaGetLastError(), "narrow_conv3x3 launch");
 }
 
-size_t narrow_conv3x3_wgrad_workspace_bytes(int B, int Cin, int Cout, int H, int W) {
+// shared by rw_torgb1x1 and rw_proggan_output_block
+static int torgb1x1_launch(const float* x, const float* w, const float* bias, float wscale,
+                           int clamp, int norm, int B, int Cin, int Cout, int H, int W, float* out,
+                           cudaStream_t stream) {
+  if (!sizes_ok(B, Cin, Cout, H, W) || Cout > kRgbMax) {
+    set_last_error("torgb1x1: bad shape B=%d Cin=%d Cout=%d (1..%d) H=%d W=%d", B, Cin, Cout,
+                   kRgbMax, H, W);
+    return RW_ERR_BAD_ARG;
+  }
+  const long long hw = static_cast<long long>(H) * W;
+  const long long blocks = (B * hw + 255) / 256;
+  if (norm)
+    torgb1x1_kernel<true><<<static_cast<unsigned>(blocks), 256, 0, stream>>>(x, w, B, Cin, Cout, hw,
+                                                                             wscale, bias, clamp, out);
+  else
+    torgb1x1_kernel<false><<<static_cast<unsigned>(blocks), 256, 0, stream>>>(x, w, B, Cin, Cout, hw,
+                                                                              wscale, bias, clamp, out);
+  return check_cuda(cudaGetLastError(), "torgb1x1 launch");
+}
+
+}  // namespace rw
+
+using namespace rw;
+
+extern "C" {
+
+int rw_proggan_input_fwd(const float* z, const float* w, const float* bias, float wscale, int B,
+                         int Z, int C, float* out, rw_stream_t stream) {
+  if (!z || !w || !out) {
+    set_last_error("rw_proggan_input_fwd: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  if (B < 1 || Z < 1 || C < 1 || C > 2147483647 / 16) {
+    set_last_error("proggan_input_fwd: bad shape B=%d Z=%d C=%d", B, Z, C);
+    return RW_ERR_BAD_ARG;
+  }
+  dim3 grid(C, (B + 15) / 16);
+  input_layer_fwd_kernel<<<grid, 256, 0, stream>>>(z, w, B, Z, C, wscale, bias, out);
+  return check_cuda(cudaGetLastError(), "proggan_input_fwd launch");
+}
+
+int rw_proggan_input_bwd(const float* z, const float* w, const float* gy, int B, int Z, int C,
+                         float* gz, float* gw, rw_stream_t stream) {
+  if (!gy || (!gz && !gw) || (gz && !w) || (gw && !z)) {
+    set_last_error("rw_proggan_input_bwd: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  if (B < 1 || Z < 1 || C < 1 || !aligned16(gy) || (gz && !aligned16(w)) || (gw && !aligned16(gw))) {
+    set_last_error("proggan_input_bwd: bad shape or alignment (B=%d Z=%d C=%d; w, gy and gw need "
+                   "16-byte alignment)", B, Z, C);
+    return RW_ERR_BAD_ARG;
+  }
+  if (gz) {
+    dim3 grid((Z + 127) / 128, (B + kInBwdB - 1) / kInBwdB);
+    input_layer_dgrad_kernel<<<grid, 128, 0, stream>>>(gy, w, B, Z, C, gz);
+    int rc = check_cuda(cudaGetLastError(), "proggan_input_bwd dgrad launch");
+    if (rc) return rc;
+  }
+  if (gw) {
+    dim3 grid((Z + 255) / 256, C);
+    input_layer_wgrad_kernel<<<grid, 256, 0, stream>>>(gy, z, B, Z, C, gw);
+    return check_cuda(cudaGetLastError(), "proggan_input_bwd wgrad launch");
+  }
+  return RW_OK;
+}
+
+int rw_narrow_conv3x3(const float* x, const float* w, const float* bias, float wscale, int B,
+                      int Cin, int Cout, int H, int W, float* out, rw_stream_t stream) {
+  if (!x || !w || !out) {
+    set_last_error("rw_narrow_conv3x3: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  return narrow_conv3x3_launch(x, w, bias, wscale, B, Cin, Cout, H, W, 0, out, stream);
+}
+
+int rw_narrow_conv3x3_dgrad(const float* gy, const float* w, int B, int Cin, int Cout, int H, int W,
+                            float* gx, rw_stream_t stream) {
+  if (!gy || !w || !gx) {
+    set_last_error("rw_narrow_conv3x3_dgrad: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  // conv(gy, W') over Cout input channels to Cin output channels
+  return narrow_conv3x3_launch(gy, w, nullptr, 1.f, B, Cout, Cin, H, W, 1, gx, stream);
+}
+
+size_t rw_narrow_conv3x3_wgrad_workspace_bytes(int B, int Cin, int Cout, int H, int W) {
   if (!sizes_ok(B, Cin, Cout, H, W)) return 0;
   return static_cast<size_t>(narrow_wgrad_splits(B, Cin, Cout, H, W)) * Cout * Cin * 9 * sizeof(float);
 }
 
-int narrow_conv3x3_wgrad_launch(const float* x, const float* gy, int B, int Cin, int Cout, int H,
-                                int W, float* gw, void* workspace, size_t workspace_bytes,
-                                cudaStream_t stream) {
-  const size_t need = narrow_conv3x3_wgrad_workspace_bytes(B, Cin, Cout, H, W);
+int rw_narrow_conv3x3_wgrad(const float* x, const float* gy, int B, int Cin, int Cout, int H, int W,
+                            float* gw, void* workspace, size_t workspace_bytes, rw_stream_t stream) {
+  if (!x || !gy || !gw || !workspace) {
+    set_last_error("rw_narrow_conv3x3_wgrad: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  const size_t need = rw_narrow_conv3x3_wgrad_workspace_bytes(B, Cin, Cout, H, W);
   if (need == 0 || workspace_bytes < need) {
     set_last_error("narrow_conv3x3_wgrad: bad shape or workspace %zu < %zu bytes (B=%d Cin=%d "
                    "Cout=%d H=%d W=%d)", workspace_bytes, need, B, Cin, Cout, H, W);
@@ -513,27 +571,21 @@ int narrow_conv3x3_wgrad_launch(const float* x, const float* gy, int B, int Cin,
   return sum_splits(part, splits, static_cast<long long>(Cout) * Cin * 9, gw, stream);
 }
 
-int torgb1x1_launch(const float* x, const float* w, const float* bias, float wscale, int clamp,
-                    int norm, int B, int Cin, int Cout, int H, int W, float* out,
-                    cudaStream_t stream) {
-  if (!sizes_ok(B, Cin, Cout, H, W) || Cout > kRgbMax) {
-    set_last_error("torgb1x1: bad shape B=%d Cin=%d Cout=%d (1..%d) H=%d W=%d", B, Cin, Cout,
-                   kRgbMax, H, W);
+int rw_torgb1x1(const float* x, const float* w, int B, int Cin, int Cout, int H, int W, float* out,
+                rw_stream_t stream) {
+  if (!x || !w || !out) {
+    set_last_error("rw_torgb1x1: bad argument");
     return RW_ERR_BAD_ARG;
   }
-  const long long hw = static_cast<long long>(H) * W;
-  const long long blocks = (B * hw + 255) / 256;
-  if (norm)
-    torgb1x1_kernel<true><<<static_cast<unsigned>(blocks), 256, 0, stream>>>(x, w, B, Cin, Cout, hw,
-                                                                             wscale, bias, clamp, out);
-  else
-    torgb1x1_kernel<false><<<static_cast<unsigned>(blocks), 256, 0, stream>>>(x, w, B, Cin, Cout, hw,
-                                                                              wscale, bias, clamp, out);
-  return check_cuda(cudaGetLastError(), "torgb1x1 launch");
+  return torgb1x1_launch(x, w, nullptr, 1.f, 0, 0, B, Cin, Cout, H, W, out, stream);
 }
 
-int torgb1x1_dgrad_launch(const float* gy, const float* w, int B, int Cin, int Cout, int H, int W,
-                          float* gx, cudaStream_t stream) {
+int rw_torgb1x1_dgrad(const float* gy, const float* w, int B, int Cin, int Cout, int H, int W,
+                      float* gx, rw_stream_t stream) {
+  if (!gy || !w || !gx) {
+    set_last_error("rw_torgb1x1_dgrad: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   if (!sizes_ok(B, Cin, Cout, H, W) || Cout > kRgbMax) {
     set_last_error("torgb1x1_dgrad: bad shape B=%d Cin=%d Cout=%d H=%d W=%d", B, Cin, Cout, H, W);
     return RW_ERR_BAD_ARG;
@@ -544,14 +596,18 @@ int torgb1x1_dgrad_launch(const float* gy, const float* w, int B, int Cin, int C
   return check_cuda(cudaGetLastError(), "torgb1x1_dgrad launch");
 }
 
-size_t torgb1x1_wgrad_workspace_bytes(int B, int Cin, int Cout, int H, int W) {
+size_t rw_torgb1x1_wgrad_workspace_bytes(int B, int Cin, int Cout, int H, int W) {
   if (!sizes_ok(B, Cin, Cout, H, W) || Cout > kRgbMax) return 0;
   return static_cast<size_t>(torgb_wgrad_splits(B, H, W)) * Cout * Cin * sizeof(float);
 }
 
-int torgb1x1_wgrad_launch(const float* x, const float* gy, int B, int Cin, int Cout, int H, int W,
-                          float* gw, void* workspace, size_t workspace_bytes, cudaStream_t stream) {
-  const size_t need = torgb1x1_wgrad_workspace_bytes(B, Cin, Cout, H, W);
+int rw_torgb1x1_wgrad(const float* x, const float* gy, int B, int Cin, int Cout, int H, int W,
+                      float* gw, void* workspace, size_t workspace_bytes, rw_stream_t stream) {
+  if (!x || !gy || !gw || !workspace) {
+    set_last_error("rw_torgb1x1_wgrad: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  const size_t need = rw_torgb1x1_wgrad_workspace_bytes(B, Cin, Cout, H, W);
   if (need == 0 || workspace_bytes < need) {
     set_last_error("torgb1x1_wgrad: bad shape or workspace %zu < %zu bytes (B=%d Cin=%d Cout=%d "
                    "H=%d W=%d)", workspace_bytes, need, B, Cin, Cout, H, W);
@@ -566,4 +622,14 @@ int torgb1x1_wgrad_launch(const float* x, const float* gy, int B, int Cin, int C
   return sum_splits(part, splits, static_cast<long long>(Cout) * Cin, gw, stream);
 }
 
-}  // namespace rw
+int rw_proggan_output_block(const float* x, const float* w, const float* bias, float wscale,
+                            int clamp, int B, int Cin, int Cout, int H, int W, float* out,
+                            rw_stream_t stream) {
+  if (!x || !w || !bias || !out) {
+    set_last_error("rw_proggan_output_block: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  return torgb1x1_launch(x, w, bias, wscale, clamp ? 1 : 0, 1, B, Cin, Cout, H, W, out, stream);
+}
+
+}  // extern "C"

@@ -15,8 +15,8 @@
 //
 // Key crop layout: kpT [B][h+2][w+2][Cin] fp32 (zero border, channels-last) so
 // that lanes <-> input channels gives coalesced 128-byte loads.
+#include "../../include/rewriting_b200.h"
 #include "rw_common.cuh"
-#include "rw_kernels.h"
 #include "insert_linear.cuh"
 
 namespace rw {
@@ -415,35 +415,6 @@ static int launch_insert(const InsertLoopParams& p, size_t smem, cudaStream_t st
 
 }  // namespace
 
-}  // namespace rw
-
-namespace rw {
-
-int project_rank_launch_signed(const float* w, const float* base, const float* d, int rank,
-                               int Cout, int Cin, int taps, float sign, float* out,
-                               cudaStream_t stream) {
-  if (rank < 1 || rank > 64) {
-    set_last_error("project_rank: rank=%d out of range [1,64]", rank);
-    return RW_ERR_BAD_ARG;
-  }
-  const size_t smem = (static_cast<size_t>(Cin) * taps + static_cast<size_t>(rank) * taps) * 4;
-  if (smem > 200 * 1024) {
-    set_last_error("project_rank: row too large for shared memory (%zu B)", smem);
-    return RW_ERR_UNSUPPORTED;
-  }
-  static size_t attr = 0;
-  if (smem > 48 * 1024 && smem > attr) {
-    int rc = check_cuda(cudaFuncSetAttribute(project_rank_kernel,
-                                             cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                             static_cast<int>(smem)),
-                        "project_rank smem attr");
-    if (rc) return rc;
-    attr = smem;
-  }
-  project_rank_kernel<<<Cout, kThreads, smem, stream>>>(w, base, d, rank, Cin, taps, sign, out);
-  return check_cuda(cudaGetLastError(), "project_rank launch");
-}
-
 template <bool kLinear>
 static int insert_loop_launch_mode(const InsertLoopParams& p, cudaStream_t stream) {
   if (p.w > kMaxW || p.B > 4 || p.B < 1 || p.Cin % 32 != 0 || p.rank > kMaxRank || p.rank < 1 ||
@@ -466,12 +437,52 @@ static int insert_loop_launch_mode(const InsertLoopParams& p, cudaStream_t strea
   return launch_insert<16, kLinear>(p, smem, stream);
 }
 
-int insert_loop_launch(const InsertLoopParams& p, cudaStream_t stream) {
+}  // namespace rw
+
+using namespace rw;
+
+extern "C" {
+
+int rw_project_rank(const float* w, const float* base, const float* d, int rank, int Cout,
+                    int Cin, int taps, float sign, float* out, rw_stream_t stream) {
+  if (!w || !d || !out) {
+    set_last_error("rw_project_rank: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  if (rank < 1 || rank > 64) {
+    set_last_error("project_rank: rank=%d out of range [1,64]", rank);
+    return RW_ERR_BAD_ARG;
+  }
+  const size_t smem = (static_cast<size_t>(Cin) * taps + static_cast<size_t>(rank) * taps) * 4;
+  if (smem > 200 * 1024) {
+    set_last_error("project_rank: row too large for shared memory (%zu B)", smem);
+    return RW_ERR_UNSUPPORTED;
+  }
+  static size_t attr = 0;
+  if (smem > 48 * 1024 && smem > attr) {
+    int rc = check_cuda(cudaFuncSetAttribute(project_rank_kernel,
+                                             cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             static_cast<int>(smem)),
+                        "project_rank smem attr");
+    if (rc) return rc;
+    attr = smem;
+  }
+  project_rank_kernel<<<Cout, kThreads, smem, stream>>>(w, base, d, rank, Cin, taps, sign, out);
+  return check_cuda(cudaGetLastError(), "project_rank launch");
+}
+
+int rw_insert_loop(const rw_insert_args* a, rw_stream_t stream) {
+  InsertLoopParams p;
+  int rc = insert_params(a, "rw_insert_loop", p);
+  if (rc) return rc;
   return insert_loop_launch_mode<false>(p, stream);
 }
 
-int linear_insert_loop_launch(const InsertLoopParams& p, cudaStream_t stream) {
+int rw_linear_insert_loop(const rw_linear_insert_args* a, rw_stream_t stream) {
+  InsertLoopParams p;
+  int rc = linear_insert_params(a, "rw_linear_insert_loop", p);
+  if (rc) return rc;
   return insert_loop_launch_mode<true>(p, stream);
 }
 
-}  // namespace rw
+}  // extern "C"

@@ -26,8 +26,8 @@
 //   semseg   the semantic head's logits up-sampled, a softmax over all classes and then one per
 //            category over those probabilities, summed over the sizes; probabilities and / or one
 //            label channel per category (argmax mapped to a label, the mask rule, a merge offset)
+#include "../../include/rewriting_b200.h"
 #include "rw_common.cuh"
-#include "rw_kernels.h"
 
 namespace rw {
 
@@ -497,7 +497,13 @@ int seg_input_common(const char* what, const void* im, int u8, int B, int H, int
 
 }  // namespace
 
-int seg_input_launch(const void* im, int u8, int B, int H, int W, int S, float* out, cudaStream_t stream) {
+}  // namespace rw
+
+using namespace rw;
+
+extern "C" {
+
+int rw_seg_input(const void* im, int u8, int B, int H, int W, int S, float* out, rw_stream_t stream) {
   // torch.tensor([102.9801, 115.9465, 122.7717]): the doubles rounded to float once
   const InputNorm N = {255.f,
                        {static_cast<float>(102.9801), static_cast<float>(115.9465), static_cast<float>(122.7717)},
@@ -505,8 +511,8 @@ int seg_input_launch(const void* im, int u8, int B, int H, int W, int S, float* 
   return seg_input_common("seg_input", im, u8, B, H, W, S, N, out, stream);
 }
 
-int seg_input_norm_launch(const void* im, int u8, int B, int H, int W, int S, const float* mean,
-                          const float* stdev, int bgr, float* out, cudaStream_t stream) {
+int rw_seg_input_norm(const void* im, int u8, int B, int H, int W, int S, const float* mean,
+                      const float* stdev, int bgr, float* out, rw_stream_t stream) {
   bool ok = mean && stdev && (bgr == 0 || bgr == 1);
   for (int c = 0; ok && c < 3; ++c)
     ok = isfinite(mean[c]) && isfinite(stdev[c]) && stdev[c] != 0.f;
@@ -518,16 +524,16 @@ int seg_input_norm_launch(const void* im, int u8, int B, int H, int W, int S, co
   return seg_input_common("seg_input_norm", im, u8, B, H, W, S, N, out, stream);
 }
 
-int seg_map_launch(const float* a, int a_cl, int B, int C, int Hin, int Win, int mode, int Ho, int Wo,
-                   const float* bias, const float* res, int relu, void* hi, void* lo, int ldc,
-                   int coff, float* out, cudaStream_t stream) {
-  return seg_map_phase_launch(a, a_cl, 1, B, C, Hin, Win, mode, Ho, Wo, bias, res, relu, 1, hi, lo,
-                              ldc, coff, out, stream);
+int rw_seg_map(const float* a, int a_cl, int B, int C, int Hin, int Win, int mode, int Ho, int Wo,
+               const float* bias, const float* res, int relu, void* hi, void* lo, int ldc,
+               int coff, float* out, rw_stream_t stream) {
+  return rw_seg_map_phase(a, a_cl, 1, B, C, Hin, Win, mode, Ho, Wo, bias, res, relu, 1, hi, lo, ldc,
+                          coff, out, stream);
 }
 
-int seg_map_phase_launch(const float* a, int a_cl, int sd, int B, int C, int Hin, int Win, int mode,
-                         int Ho, int Wo, const float* bias, const float* res, int relu, int dd,
-                         void* hi, void* lo, int ldc, int coff, float* out, cudaStream_t stream) {
+int rw_seg_map_phase(const float* a, int a_cl, int sd, int B, int C, int Hin, int Win, int mode,
+                     int Ho, int Wo, const float* bias, const float* res, int relu, int dd,
+                     void* hi, void* lo, int ldc, int coff, float* out, rw_stream_t stream) {
   bool ok = a && sd >= 1 && sd <= 8 && dd >= 1 && dd <= 8 && B >= 1 &&
             static_cast<long long>(dd) * dd * B <= 65535 && C >= 64 && C % 64 == 0 &&
             C / 64 <= 65535 && Hin >= 1 && Win >= 1 && Ho >= 1 && Wo >= 1 &&
@@ -559,7 +565,7 @@ int seg_map_phase_launch(const float* a, int a_cl, int sd, int B, int C, int Hin
   return check_cuda(cudaGetLastError(), "seg_map");
 }
 
-int seg_maxpool_launch(const float* x, int B, int C, int H, int W, float* out, cudaStream_t stream) {
+int rw_seg_maxpool(const float* x, int B, int C, int H, int W, float* out, rw_stream_t stream) {
   if (!x || !out || B < 1 || C < 1 || H < 1 || W < 1 || static_cast<long long>(B) * C * H * W >= (1LL << 40)) {
     set_last_error("seg_maxpool: bad argument B=%d C=%d H=%d W=%d", B, C, H, W);
     return RW_ERR_BAD_ARG;
@@ -570,7 +576,7 @@ int seg_maxpool_launch(const float* x, int B, int C, int H, int W, float* out, c
   return check_cuda(cudaGetLastError(), "seg_maxpool");
 }
 
-int seg_prroi_launch(const float* x, int B, int C, int H, int W, int s, float* out, cudaStream_t stream) {
+int rw_seg_prroi(const float* x, int B, int C, int H, int W, int s, float* out, rw_stream_t stream) {
   if (!x || !out || B < 1 || C < 1 || H < 1 || W < 1 || s < 1 || s > 4096 ||
       static_cast<long long>(B) * C * H * W >= (1LL << 40)) {
     set_last_error("seg_prroi: bad argument B=%d C=%d H=%d W=%d s=%d", B, C, H, W, s);
@@ -581,7 +587,7 @@ int seg_prroi_launch(const float* x, int B, int C, int H, int W, int s, float* o
   return check_cuda(cudaGetLastError(), "seg_prroi");
 }
 
-int seg_avgpool_launch(const float* x, int B, int C, int H, int W, int s, float* out, cudaStream_t stream) {
+int rw_seg_avgpool(const float* x, int B, int C, int H, int W, int s, float* out, rw_stream_t stream) {
   if (!x || !out || B < 1 || C < 1 || H < 1 || W < 1 || s < 1 || s > 4096 ||
       static_cast<long long>(B) * C * H * W >= (1LL << 40) ||
       static_cast<long long>(B) * C * s * s >= (1LL << 40)) {
@@ -593,10 +599,10 @@ int seg_avgpool_launch(const float* x, int B, int C, int H, int W, int s, float*
   return check_cuda(cudaGetLastError(), "seg_avgpool");
 }
 
-int seg_classes_launch(int nsizes, const float* const* logits, const int* map_hw, const float* const* bias,
-                       const int* ld, int ngroups, const int* groups, const long long* trans,
-                       long long mat_offset, int B, int Ho, int Wo, float* probs, long long* labels,
-                       cudaStream_t stream) {
+int rw_seg_classes(int nsizes, const float* const* logits, const int* map_hw, const float* const* bias,
+                   const int* ld, int ngroups, const int* groups, const long long* trans,
+                   long long mat_offset, int B, int Ho, int Wo, float* probs, long long* labels,
+                   rw_stream_t stream) {
   const char* what = "seg_classes";
   if (nsizes < 1 || nsizes > kMaxSizes || !logits || !map_hw || !bias || !ld || !groups ||
       ngroups < 1 || ngroups > kMaxGroups || B < 1 || B > 65535 || Ho < 1 || Wo < 1 ||
@@ -652,11 +658,11 @@ int seg_classes_launch(int nsizes, const float* const* logits, const int* map_hw
   return check_cuda(cudaGetLastError(), what);
 }
 
-int semseg_classes_launch(int nsizes, const float* const* logits, const int* map_hw, const float* bias,
-                          int ld, int ncls, int ncat, const int* cat_start, const int* cat_chan,
-                          const int* cat_label, const int* cat_mask, int B, int Ho, int Wo,
-                          float* probs, long long* labels, int lchan, int lcoff, long long offset,
-                          cudaStream_t stream) {
+int rw_semseg_classes(int nsizes, const float* const* logits, const int* map_hw, const float* bias,
+                      int ld, int ncls, int ncat, const int* cat_start, const int* cat_chan,
+                      const int* cat_label, const int* cat_mask, int B, int Ho, int Wo,
+                      float* probs, long long* labels, int lchan, int lcoff, long long offset,
+                      rw_stream_t stream) {
   const char* what = "semseg_classes";
   if (nsizes < 1 || nsizes > kMaxSizes || !logits || !map_hw || !bias || ncls < 1 ||
       ncls > kMaxSemClasses || ld < ncls || ncat < 1 || ncat > kMaxCats || !cat_start || !cat_chan ||
@@ -718,4 +724,4 @@ int semseg_classes_launch(int nsizes, const float* const* logits, const int* map
   return check_cuda(cudaGetLastError(), what);
 }
 
-}  // namespace rw
+}  // extern "C"

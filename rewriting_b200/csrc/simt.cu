@@ -8,8 +8,8 @@
 // tensor cores (these are byte-movement bound, SURVEY.md §8d).
 #include <cstdlib>
 
+#include "../../include/rewriting_b200.h"
 #include "rw_common.cuh"
-#include "rw_kernels.h"
 
 namespace rw {
 
@@ -1120,8 +1120,64 @@ inline int grid_for(long long n, int threads, int cap = 132 * 16) {
 
 }  // namespace
 
-int prep_keys_launch(const float* x, const float* style, int B, int C, int H, int W, void* kp_hi,
-                     void* kp_lo, float* k_out, cudaStream_t stream) {
+// shared by rw_rgb_combine and rw_rgb_combine_u8
+static int rgb_combine_launch(const float* part, int nparts, int B, int H, int W, const float* bias,
+                              const float* prev, const float* k4, float* out, unsigned char* out_u8,
+                              cudaStream_t stream) {
+  if ((W & 3) != 0 || (prev && ((H | W) & 1)) || static_cast<long long>(B) * 3 > 65535 ||
+      (!out && !out_u8) ||
+      (reinterpret_cast<uintptr_t>(part) & 15u) || (reinterpret_cast<uintptr_t>(out) & 15u)) {
+    set_last_error("rgb_combine: W=%d must be a multiple of 4 (even H, W with a skip), B*3 <= 65535, "
+                   "16-byte aligned buffers", W);
+    return RW_ERR_BAD_ARG;
+  }
+  const int quads = W / 4;
+  const int bx = quads >= 64 ? 64 : (quads >= 32 ? 32 : (quads >= 16 ? 16 : (quads >= 8 ? 8 : (quads >= 4 ? 4 : (quads >= 2 ? 2 : 1)))));
+  const int by = 256 / bx > H ? H : 256 / bx;
+  dim3 block(bx, by);
+  dim3 grid((quads + bx - 1) / bx, (H + by - 1) / by, B * 3);
+  const long long part_stride = static_cast<long long>(B) * 3 * H * W;
+  rgb_combine_kernel<<<grid, block, 0, stream>>>(part, nparts, part_stride, H, W, bias, prev, k4,
+                                                 out, out_u8);
+  return check_cuda(cudaGetLastError(), "rgb_combine launch");
+}
+
+// shared by rw_styles and rw_equal_linear
+static int styles_launch(const float* latent, int B, int n_latent, int K, float scale,
+                         float bias_mul, int act, int n, const float* const* w,
+                         const float* const* bias, float* const* out, const int* lat,
+                         const int* chans, cudaStream_t stream) {
+  if (n < 1 || n > 32) {
+    set_last_error("styles: %d layers (max 32)", n);
+    return RW_ERR_BAD_ARG;
+  }
+  // NOTE the equalised-lr convention: out = x . (W * scale)^T + bias * bias_mul; the scale is
+  // applied to the accumulated sum here (one rounding per output instead of one per weight)
+  GemmJobs jobs;
+  jobs.n = n;
+  for (int i = 0; i < n; ++i) {
+    jobs.a[i] = latent + static_cast<size_t>(lat[i]) * K;
+    jobs.w[i] = w[i];
+    jobs.bias[i] = bias[i];
+    jobs.out[i] = out[i];
+    jobs.n_out[i] = chans[i];
+  }
+  return gemm_jobs_launch<0>(jobs, B, K, static_cast<long long>(n_latent) * K, scale, bias_mul, act,
+                             0.f, stream);
+}
+
+}  // namespace rw
+
+using namespace rw;
+
+extern "C" {
+
+int rw_prep_keys(const float* x, const float* style, int B, int C, int H, int W, void* kp_hi,
+                 void* kp_lo, float* k_out, rw_stream_t stream) {
+  if (!x || !kp_hi || !kp_lo || B < 1 || H < 1 || W < 1) {
+    set_last_error("rw_prep_keys: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   if (C % 64 != 0) {
     set_last_error("prep_keys: C=%d must be a multiple of 64", C);
     return RW_ERR_BAD_ARG;
@@ -1134,7 +1190,12 @@ int prep_keys_launch(const float* x, const float* style, int B, int C, int H, in
   return check_cuda(cudaGetLastError(), "prep_keys launch");
 }
 
-int split_rows_launch(const float* a, long long n, void* hi, void* lo, cudaStream_t stream) {
+int rw_split_rows(const float* a, long long n, void* hi, void* lo, rw_stream_t stream) {
+  if (n == 0) return RW_OK;
+  if (!a || !hi || !lo || n < 0) {
+    set_last_error("rw_split_rows: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   const int threads = 256;
   const long long n4 = (n + 3) / 4;
   const int blocks = static_cast<int>((n4 + threads - 1) / threads);
@@ -1143,8 +1204,12 @@ int split_rows_launch(const float* a, long long n, void* hi, void* lo, cudaStrea
   return check_cuda(cudaGetLastError(), "split_rows launch");
 }
 
-int prep_weights_launch(const float* w, int Cout, int Cin, float scale, int transpose_io,
-                        int flip_taps, void* wt_hi, void* wt_lo, float* wsq, cudaStream_t stream) {
+int rw_prep_weights(const float* w, int Cout, int Cin, float scale, int transpose_io,
+                    int flip_taps, void* wt_hi, void* wt_lo, float* wsq, rw_stream_t stream) {
+  if (!w || !wt_hi || !wt_lo || Cout < 1 || Cin < 1) {
+    set_last_error("rw_prep_weights: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   const int n = Cout * Cin;
   prep_weights_kernel<<<(n + 255) / 256, 256, 0, stream>>>(
       w, Cout, Cin, scale, transpose_io, flip_taps, static_cast<__nv_bfloat16*>(wt_hi),
@@ -1152,8 +1217,12 @@ int prep_weights_launch(const float* w, int Cout, int Cin, float scale, int tran
   return check_cuda(cudaGetLastError(), "prep_weights launch");
 }
 
-int demod_launch(const float* style, const float* wsq, int B, int Cout, int Cin, float eps,
-                 float* demod, cudaStream_t stream) {
+int rw_demod(const float* style, const float* wsq, int B, int Cout, int Cin, float eps,
+             float* demod, rw_stream_t stream) {
+  if (!style || !wsq || !demod) {
+    set_last_error("rw_demod: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   const long long warps = static_cast<long long>(B) * Cout;
   const int threads = 256;
   const int blocks = static_cast<int>((warps * 32 + threads - 1) / threads);
@@ -1161,9 +1230,13 @@ int demod_launch(const float* style, const float* wsq, int B, int Cout, int Cin,
   return check_cuda(cudaGetLastError(), "demod launch");
 }
 
-int blur_up_act_launch(const float* t, int B, int C, int Hin, int Win, const float* kernel4x4,
-                       const float* noise, long long noise_bstride, const float* noise_w,
-                       const float* bias, int act, float* y, cudaStream_t stream) {
+int rw_blur_up_act(const float* t, int B, int C, int Hin, int Win, const float* kernel4x4,
+                   const float* noise, long long noise_bstride, const float* noise_w,
+                   const float* bias, int act, float* y, rw_stream_t stream) {
+  if (!t || !kernel4x4 || !y || (noise && !noise_w)) {
+    set_last_error("rw_blur_up_act: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   const int Ht = 2 * Hin + 1, Wt = 2 * Win + 1;
   const int Ho = 2 * Hin, Wo = 2 * Win;
   if (static_cast<long long>(B) * C > 65535LL * 1) {
@@ -1180,9 +1253,13 @@ int blur_up_act_launch(const float* t, int B, int C, int Hin, int Win, const flo
   return check_cuda(cudaGetLastError(), "blur_up_act launch");
 }
 
-int upfirdn2d_launch(const float* in, const float* kernel, int major, int in_h, int in_w, int kh,
-                     int kw, int up_x, int up_y, int down_x, int down_y, int px0, int px1, int py0,
-                     int py1, float* out, int out_h, int out_w, cudaStream_t stream) {
+int rw_upfirdn2d(const float* in, const float* kernel, int major, int in_h, int in_w, int kh,
+                 int kw, int up_x, int up_y, int down_x, int down_y, int px0, int px1, int py0,
+                 int py1, float* out, int out_h, int out_w, rw_stream_t stream) {
+  if (!in || !kernel || !out || up_x < 1 || up_y < 1 || down_x < 1 || down_y < 1) {
+    set_last_error("rw_upfirdn2d: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   (void)px1;
   (void)py1;
   const long long total = static_cast<long long>(major) * out_h * out_w;
@@ -1195,19 +1272,27 @@ int upfirdn2d_launch(const float* in, const float* kernel, int major, int in_h, 
   return check_cuda(cudaGetLastError(), "upfirdn2d launch");
 }
 
-int bias_act_launch(const float* x, const float* bias, const float* ref, int act, int grad,
-                    float alpha, float scale, long long n, int step_b, int size_b, float* y,
-                    cudaStream_t stream) {
-  if (n <= 0) return RW_OK;
+int rw_fused_bias_act(const float* x, const float* bias, const float* ref, int act, int grad,
+                      float alpha, float scale, long long n, int step_b, int size_b, float* y,
+                      rw_stream_t stream) {
+  if (n == 0) return RW_OK;
+  if (!x || !y || n < 0) {
+    set_last_error("rw_fused_bias_act: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   bias_act_kernel<<<grid_for(n, 256), 256, 0, stream>>>(x, bias, ref, act, grad, alpha, scale, n,
                                                         step_b > 0 ? step_b : 1,
                                                         size_b > 0 ? size_b : 1, y);
   return check_cuda(cudaGetLastError(), "bias_act launch");
 }
 
-int torgb_launch(const float* x, const float* style, const float* w, const float* bias,
-                 const float* skip, int B, int C, int H, int W, float scale, float* out,
-                 cudaStream_t stream) {
+int rw_torgb(const float* x, const float* style, const float* w, const float* bias,
+             const float* skip, int B, int C, int H, int W, float scale, float* out,
+             rw_stream_t stream) {
+  if (!x || !style || !w || !bias || !out || C > 4096) {
+    set_last_error("rw_torgb: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   const int HW = H * W;
   dim3 grid((HW + 255) / 256, B);
   torgb_kernel<<<grid, 256, 3 * C * sizeof(float), stream>>>(x, style, w, bias, skip, C, HW, scale,
@@ -1215,8 +1300,12 @@ int torgb_launch(const float* x, const float* style, const float* w, const float
   return check_cuda(cudaGetLastError(), "torgb launch");
 }
 
-int add_noise_launch(const float* x, const float* noise, long long noise_bstride, const float* noise_w,
-                     int B, int C, int HW, float* y, cudaStream_t stream) {
+int rw_add_noise(const float* x, const float* noise, long long noise_bstride,
+                 const float* noise_w, int B, int C, int HW, float* y, rw_stream_t stream) {
+  if (!x || !noise || !y || !noise_w) {
+    set_last_error("rw_add_noise: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   const long long total = static_cast<long long>(B) * C * HW;
   if (total <= 0) return RW_OK;
   add_noise_kernel<<<grid_for(total, 256), 256, 0, stream>>>(x, noise, noise_bstride, noise_w, C,
@@ -1224,10 +1313,14 @@ int add_noise_launch(const float* x, const float* noise, long long noise_bstride
   return check_cuda(cudaGetLastError(), "add_noise launch");
 }
 
-int blur_up_fused_launch(const float* t_cl, int B, int C, int Hin, int Win, const float* k4,
-                         const float* noise, long long noise_bstride, const float* noise_w,
-                         const float* bias, const float* next_scale, void* next_hi, void* next_lo,
-                         cudaStream_t stream) {
+int rw_blur_up_fused(const float* t_cl, int B, int C, int Hin, int Win, const float* k4,
+                     const float* noise, long long noise_bstride, const float* noise_w,
+                     const float* bias, const float* next_scale, void* next_hi, void* next_lo,
+                     rw_stream_t stream) {
+  if (!t_cl || !k4 || !noise || !noise_w || !bias || !next_scale || !next_hi || !next_lo) {
+    set_last_error("rw_blur_up_fused: bad argument (every pointer is required)");
+    return RW_ERR_BAD_ARG;
+  }
   if (C % BF_C != 0) {
     set_last_error("blur_up_fused: C=%d must be a multiple of 64", C);
     return RW_ERR_BAD_ARG;
@@ -1264,57 +1357,61 @@ int blur_up_fused_launch(const float* t_cl, int B, int C, int Hin, int Win, cons
   return check_cuda(cudaGetLastError(), "blur_up_pipe launch");
 }
 
-int rgb_combine_launch(const float* part, int nparts, int B, int H, int W, const float* bias,
-                       const float* prev, const float* k4, float* out, unsigned char* out_u8,
-                       cudaStream_t stream) {
-  if ((W & 3) != 0 || (prev && ((H | W) & 1)) || static_cast<long long>(B) * 3 > 65535 ||
-      (!out && !out_u8) ||
-      (reinterpret_cast<uintptr_t>(part) & 15u) || (reinterpret_cast<uintptr_t>(out) & 15u)) {
-    set_last_error("rgb_combine: W=%d must be a multiple of 4 (even H, W with a skip), B*3 <= 65535, "
-                   "16-byte aligned buffers", W);
+int rw_rgb_combine(const float* part, int nparts, int B, int H, int W, const float* bias,
+                   const float* prev, const float* kernel4x4, float* out, rw_stream_t stream) {
+  if (!part || nparts < 1 || !bias || !out || (prev && !kernel4x4)) {
+    set_last_error("rw_rgb_combine: bad argument");
     return RW_ERR_BAD_ARG;
   }
-  const int quads = W / 4;
-  const int bx = quads >= 64 ? 64 : (quads >= 32 ? 32 : (quads >= 16 ? 16 : (quads >= 8 ? 8 : (quads >= 4 ? 4 : (quads >= 2 ? 2 : 1)))));
-  const int by = 256 / bx > H ? H : 256 / bx;
-  dim3 block(bx, by);
-  dim3 grid((quads + bx - 1) / bx, (H + by - 1) / by, B * 3);
-  const long long part_stride = static_cast<long long>(B) * 3 * H * W;
-  rgb_combine_kernel<<<grid, block, 0, stream>>>(part, nparts, part_stride, H, W, bias, prev, k4,
-                                                 out, out_u8);
-  return check_cuda(cudaGetLastError(), "rgb_combine launch");
+  return rgb_combine_launch(part, nparts, B, H, W, bias, prev, kernel4x4, out, nullptr, stream);
 }
 
-int styles_launch(const float* latent, int B, int n_latent, int K, float scale, float bias_mul,
-                  int act, int n, const float* const* w, const float* const* bias,
-                  float* const* out, const int* lat, const int* chans, cudaStream_t stream) {
-  if (n < 1 || n > 32) {
-    set_last_error("styles: %d layers (max 32)", n);
+int rw_rgb_combine_u8(const float* part, int nparts, int B, int H, int W, const float* bias,
+                      const float* prev, const float* kernel4x4, float* out,
+                      unsigned char* out_u8_nhwc, rw_stream_t stream) {
+  if (!part || nparts < 1 || !bias || (!out && !out_u8_nhwc) || (prev && !kernel4x4)) {
+    set_last_error("rw_rgb_combine_u8: bad argument");
     return RW_ERR_BAD_ARG;
   }
-  // NOTE the equalised-lr convention: out = x . (W * scale)^T + bias * bias_mul; the scale is
-  // applied to the accumulated sum here (one rounding per output instead of one per weight)
-  GemmJobs jobs;
-  jobs.n = n;
-  for (int i = 0; i < n; ++i) {
-    jobs.a[i] = latent + static_cast<size_t>(lat[i]) * K;
-    jobs.w[i] = w[i];
-    jobs.bias[i] = bias[i];
-    jobs.out[i] = out[i];
-    jobs.n_out[i] = chans[i];
-  }
-  return gemm_jobs_launch<0>(jobs, B, K, static_cast<long long>(n_latent) * K, scale, bias_mul, act,
-                             0.f, stream);
+  return rgb_combine_launch(part, nparts, B, H, W, bias, prev, kernel4x4, out, out_u8_nhwc, stream);
 }
 
-int pixel_norm_launch(const float* z, int B, int K, float* out, cudaStream_t stream) {
+int rw_styles(const float* latent, int B, int n_latent, int K, float scale, int n,
+              const float* const* w, const float* const* bias, float* const* out, const int* lat,
+              const int* chans, rw_stream_t stream) {
+  if (!latent || !w || !bias || !out || !lat || !chans || B < 1) {
+    set_last_error("rw_styles: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  return styles_launch(latent, B, n_latent, K, scale, 1.f, 0, n, w, bias, out, lat, chans, stream);
+}
+
+int rw_equal_linear(const float* x, int B, int K, const float* w, const float* bias, int Cout,
+                    float scale, float bias_mul, int act, float* out, rw_stream_t stream) {
+  if (!x || !w || !bias || !out || B < 1 || K < 1 || Cout < 1) {
+    set_last_error("rw_equal_linear: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  const int lat = 0;
+  return styles_launch(x, B, 1, K, scale, bias_mul, act, 1, &w, &bias, &out, &lat, &Cout, stream);
+}
+
+int rw_pixel_norm(const float* z, int B, int K, float* out, rw_stream_t stream) {
+  if (!z || !out || B < 1 || K < 1) {
+    set_last_error("rw_pixel_norm: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   const int blocks = (B * 32 + 255) / 256;
   pixel_norm_kernel<<<blocks, 256, 0, stream>>>(z, B, K, out);
   return check_cuda(cudaGetLastError(), "pixel_norm launch");
 }
 
-int pixel_norm_nchw_launch(const float* x, int B, int C, int H, int W, int up2, float* out,
-                           cudaStream_t stream) {
+int rw_pixel_norm_nchw(const float* x, int B, int C, int H, int W, int up2, float* out,
+                       rw_stream_t stream) {
+  if (!x || !out) {
+    set_last_error("rw_pixel_norm_nchw: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   const long long n = static_cast<long long>(B) * H * W;
   if (n <= 0 || C < 1 || (up2 && (reinterpret_cast<uintptr_t>(out) & 7u))) {
     set_last_error("pixel_norm_nchw: bad shape / alignment");
@@ -1325,8 +1422,11 @@ int pixel_norm_nchw_launch(const float* x, int B, int C, int H, int W, int up2, 
   return check_cuda(cudaGetLastError(), "pixel_norm_nchw launch");
 }
 
-int nearest_up2_launch(const float* x, long long planes, int H, int W, float* out,
-                       cudaStream_t stream) {
+int rw_nearest_up2(const float* x, long long planes, int H, int W, float* out, rw_stream_t stream) {
+  if (!x || !out) {
+    set_last_error("rw_nearest_up2: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   const long long n = planes * H * W;
   if (n <= 0 || (reinterpret_cast<uintptr_t>(out) & 7u)) {
     set_last_error("nearest_up2: bad shape / alignment");
@@ -1337,8 +1437,12 @@ int nearest_up2_launch(const float* x, long long planes, int H, int W, float* ou
   return check_cuda(cudaGetLastError(), "nearest_up2 launch");
 }
 
-int pixel_norm_nchw_bwd_launch(const float* x, const float* gy, int B, int C, int H, int W, int up2,
-                               float* gx, cudaStream_t stream) {
+int rw_pixel_norm_nchw_bwd(const float* x, const float* gy, int B, int C, int H, int W, int up2,
+                           float* gx, rw_stream_t stream) {
+  if (!x || !gy || !gx) {
+    set_last_error("rw_pixel_norm_nchw_bwd: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   if (B < 1 || C < 1 || H < 1 || W < 1 || (up2 && (reinterpret_cast<uintptr_t>(gy) & 7u))) {
     set_last_error("pixel_norm_nchw_bwd: bad shape / alignment");
     return RW_ERR_BAD_ARG;
@@ -1349,8 +1453,12 @@ int pixel_norm_nchw_bwd_launch(const float* x, const float* gy, int B, int C, in
   return check_cuda(cudaGetLastError(), "pixel_norm_nchw_bwd launch");
 }
 
-int nearest_up2_bwd_launch(const float* gy, long long planes, int H, int W, float* gx,
-                           cudaStream_t stream) {
+int rw_nearest_up2_bwd(const float* gy, long long planes, int H, int W, float* gx,
+                       rw_stream_t stream) {
+  if (!gy || !gx) {
+    set_last_error("rw_nearest_up2_bwd: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   if (planes < 1 || H < 1 || W < 1 || (reinterpret_cast<uintptr_t>(gy) & 7u)) {
     set_last_error("nearest_up2_bwd: bad shape / alignment");
     return RW_ERR_BAD_ARG;
@@ -1361,10 +1469,13 @@ int nearest_up2_bwd_launch(const float* gy, long long planes, int H, int W, floa
   return check_cuda(cudaGetLastError(), "nearest_up2_bwd launch");
 }
 
-int demod_multi_launch(int B, float eps, int n, const float* const* style,
-                       const float* const* wsq, float* const* out, const int* cout,
-                       const int* cin, const int* kind, const float* wscale,
-                       cudaStream_t stream) {
+int rw_demod_multi(int B, float eps, int n, const float* const* style, const float* const* wsq,
+                   float* const* out, const int* cout, const int* cin, const int* kind,
+                   const float* wscale, rw_stream_t stream) {
+  if (!style || !wsq || !out || !cout || !cin || !kind || !wscale || B < 1) {
+    set_last_error("rw_demod_multi: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   if (n < 1 || n > 32) {
     set_last_error("demod_multi: %d jobs (max 32)", n);
     return RW_ERR_BAD_ARG;
@@ -1413,8 +1524,12 @@ int demod_multi_launch(int B, float eps, int n, const float* const* style,
   return check_cuda(cudaGetLastError(), "demod_multi launch");
 }
 
-int prep_phase_keys_launch(const float* g, const float* scale_bc, int B, int C, int H, int W,
-                           void* hi, void* lo, cudaStream_t stream) {
+int rw_prep_phase_keys(const float* g, const float* scale_bc, int B, int C, int H, int W,
+                       void* hi, void* lo, rw_stream_t stream) {
+  if (!g || !hi || !lo || B < 1) {
+    set_last_error("rw_prep_phase_keys: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
   if (C % 64 != 0) {
     set_last_error("prep_phase_keys: C=%d must be a multiple of 64", C);
     return RW_ERR_BAD_ARG;
@@ -1427,4 +1542,4 @@ int prep_phase_keys_launch(const float* g, const float* scale_bc, int B, int C, 
   return check_cuda(cudaGetLastError(), "prep_phase_keys launch");
 }
 
-}  // namespace rw
+}  // extern "C"

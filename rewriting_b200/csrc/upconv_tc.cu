@@ -42,10 +42,31 @@
 // registers to the two consumer warpgroups (setmaxnreg) and whose warp 8 issues the TMA loads.
 #include <cstring>
 
+#include "../../include/rewriting_b200.h"
 #include "rw_common.cuh"
-#include "rw_kernels.h"
 
 namespace rw {
+
+struct UpFusedParams {
+  int B, Cin, Cout, H, W;      // input resolution H x W (W a power of two, 4..128)
+  const float* demod;          // [B, Cout]
+  const float* bias;           // [Cout]
+  const float* noise;          // [B, noise_bstride], indexed Y * 2W + X at OUTPUT resolution
+  long long noise_bstride;
+  const float* noise_w;        // device scalar
+  const float* k4;             // 4x4 blur kernel (rank one)
+  const float* next_scale;     // [B, Cout] style of the consuming layer
+  void* next_hi;               // [B][2H+1][2W+1][Cout] bf16 planes (pad row / column zeroed)
+  void* next_lo;
+  // layer-level mode (the autograd op's forward): y_out != null writes the layer's own output
+  // y [B][Cout][2H][2W] fp32 instead of the next layer's planes; demod / noise / noise_w may then
+  // be null (= 1 / no noise) and act = 0 skips bias + leaky-ReLU
+  float* y_out;
+  int act;
+  int ncg, nbands, nitems;     // filled by the launcher
+  long long* debug_prof;       // per (CTA, epilogue warp) cycle counters [grid][8][16], or null
+                               // (rw_debug_upconv_profile)
+};
 
 namespace {
 
@@ -627,12 +648,9 @@ upconv_fused_kernel(const __grid_constant__ CUtensorMap map_a_hi,
 
 }  // namespace
 
-int make_tmap_nd_bf16(CUtensorMap* out, const void* base, int rank, const uint64_t* dims,
-                      const uint64_t* strides_bytes, const uint32_t* box, const uint32_t* estrides,
-                      int swizzle);
-
-int upconv_fused_launch(const UpFusedParams& pin, const void* a_hi, const void* a_lo,
-                        const void* w_hi, const void* w_lo, cudaStream_t stream) {
+// weights: bf16 hi/lo planes [Cout/16][channel half][9 taps][8][Cin]  (rw_prep_weights, transpose_io = 2)
+static int upconv_fused_launch(const UpFusedParams& pin, const void* a_hi, const void* a_lo,
+                               const void* w_hi, const void* w_lo, cudaStream_t stream) {
   UpFusedParams p = pin;
   const int W = p.W, H = p.H;
   if (W < 4 || W > UM || (W & (W - 1)) != 0 || H < 1 || p.Cin % UBK != 0 || p.Cout % UNC != 0 ||
@@ -727,4 +745,69 @@ int upconv_fused_launch(const UpFusedParams& pin, const void* a_hi, const void* 
   return launch(upconv_fused_kernel<false, false>, attr_planes);
 }
 
+// the fused upsampling conv's parameters common to its entry points; next_* are null in
+// layer-level mode (y_out)
+static UpFusedParams up_fused_params(int B, int Cin, int Cout, int H, int W, const float* demod,
+                                     const float* kernel4x4, const float* noise,
+                                     long long noise_bstride, const float* noise_w,
+                                     const float* bias, const float* next_scale, void* next_hi,
+                                     void* next_lo) {
+  UpFusedParams p;
+  memset(&p, 0, sizeof(p));
+  p.B = B; p.Cin = Cin; p.Cout = Cout; p.H = H; p.W = W;
+  p.demod = demod; p.bias = bias; p.noise = noise; p.noise_bstride = noise_bstride;
+  p.noise_w = noise_w; p.k4 = kernel4x4; p.next_scale = next_scale;
+  p.next_hi = next_hi; p.next_lo = next_lo;
+  return p;
+}
+
 }  // namespace rw
+
+using namespace rw;
+
+extern "C" {
+
+int rw_modconv_up_fused(const void* kp_hi, const void* kp_lo, const void* wt_hi, const void* wt_lo,
+                        const float* demod, const float* kernel4x4, const float* noise,
+                        long long noise_bstride, const float* noise_w, const float* bias,
+                        const float* next_scale, void* next_hi, void* next_lo, int B, int Cin,
+                        int Cout, int H, int W, rw_stream_t stream) {
+  if (!kp_hi || !kp_lo || !wt_hi || !wt_lo || !demod || !kernel4x4 || !noise || !noise_w || !bias ||
+      !next_scale || !next_hi || !next_lo || (noise_bstride & 1)) {
+    set_last_error("rw_modconv_up_fused: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  const UpFusedParams p = up_fused_params(B, Cin, Cout, H, W, demod, kernel4x4, noise,
+                                          noise_bstride, noise_w, bias, next_scale, next_hi, next_lo);
+  return upconv_fused_launch(p, kp_hi, kp_lo, wt_hi, wt_lo, stream);
+}
+
+int rw_modconv_up_fused_y(const void* kp_hi, const void* kp_lo, const void* wt_hi, const void* wt_lo,
+                          const float* demod, const float* kernel4x4, const float* noise,
+                          long long noise_bstride, const float* noise_w, const float* bias, int act,
+                          float* y, int B, int Cin, int Cout, int H, int W, rw_stream_t stream) {
+  if (!kp_hi || !kp_lo || !wt_hi || !wt_lo || !kernel4x4 || !y || (noise && (noise_bstride & 3)) ||
+      ((noise != nullptr) != (noise_w != nullptr))) {
+    set_last_error("rw_modconv_up_fused_y: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  UpFusedParams p = up_fused_params(B, Cin, Cout, H, W, demod, kernel4x4, noise, noise_bstride,
+                                    noise_w, bias, nullptr, nullptr, nullptr);
+  p.y_out = y;
+  p.act = act;
+  return upconv_fused_launch(p, kp_hi, kp_lo, wt_hi, wt_lo, stream);
+}
+
+int rw_debug_upconv_profile(const void* kp_hi, const void* kp_lo, const void* wt_hi,
+                            const void* wt_lo, const float* demod, const float* kernel4x4,
+                            const float* noise, long long noise_bstride, const float* noise_w,
+                            const float* bias, const float* next_scale, void* next_hi, void* next_lo,
+                            int B, int Cin, int Cout, int H, int W, long long* prof_out,
+                            rw_stream_t stream) {
+  UpFusedParams p = up_fused_params(B, Cin, Cout, H, W, demod, kernel4x4, noise, noise_bstride,
+                                    noise_w, bias, next_scale, next_hi, next_lo);
+  p.debug_prof = prof_out;
+  return upconv_fused_launch(p, kp_hi, kp_lo, wt_hi, wt_lo, stream);
+}
+
+}  // extern "C"

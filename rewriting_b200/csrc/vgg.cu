@@ -10,8 +10,8 @@
 //               value or by a NaN (the first maximum wins ties, a NaN wins over numbers); the
 //               gradient lands on that element as 0 + gy, every other element gets 0
 //   threshold_backward  out <= 0 ? 0 : g   (so a NaN output passes its gradient)
+#include "../../include/rewriting_b200.h"
 #include "rw_common.cuh"
-#include "rw_kernels.h"
 
 namespace rw {
 
@@ -165,8 +165,9 @@ inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 
 }  // namespace
 
-int relu_pool_launch(const float* a, const float* bias, const float* gy, int B, int C, int H, int W,
-                     int pool, void* hi, void* lo, float* out, cudaStream_t stream) {
+// the forward (gy == null) and the backward of rw_relu_pool
+static int relu_pool_launch(const float* a, const float* bias, const float* gy, int B, int C, int H,
+                            int W, int pool, void* hi, void* lo, float* out, cudaStream_t stream) {
   const char* what = gy ? "relu_pool_bwd" : "relu_pool";
   if (B < 1 || C < 1 || H < 1 || W < 1 || B > 65535 ||
       static_cast<long long>(B) * C * (H + 1) * (W + 1) >= (1LL << 40)) {
@@ -195,3 +196,27 @@ int relu_pool_launch(const float* a, const float* bias, const float* gy, int B, 
 }
 
 }  // namespace rw
+
+using namespace rw;
+
+extern "C" {
+
+int rw_relu_pool(const float* a, const float* bias, int B, int C, int H, int W, int pool,
+                 void* out_hi, void* out_lo, float* out, rw_stream_t stream) {
+  if (!a) {
+    set_last_error("rw_relu_pool: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  return relu_pool_launch(a, bias, nullptr, B, C, H, W, pool, out_hi, out_lo, out, stream);
+}
+
+int rw_relu_pool_bwd(const float* a, const float* bias, const float* gy, int B, int C, int H, int W,
+                     int pool, void* g_hi, void* g_lo, float* g, rw_stream_t stream) {
+  if (!a || !gy) {
+    set_last_error("rw_relu_pool_bwd: bad argument");
+    return RW_ERR_BAD_ARG;
+  }
+  return relu_pool_launch(a, bias, gy, B, C, H, W, pool, g_hi, g_lo, g, stream);
+}
+
+}  // extern "C"

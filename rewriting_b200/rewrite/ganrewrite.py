@@ -60,7 +60,7 @@ def fused_insert_kernel(B, Cin, Cout, h, w, linear=False):
     if B > 4 or Cin % 32 != 0:
         return None
     prefix = 'rw_linear_' if linear else 'rw_'
-    # shared memory of rw_insert_loop (csrc/rewrite.cu insert_loop_launch): 4 weight rows +
+    # shared memory of rw_insert_loop (csrc/rewrite.cu insert_loop_launch_mode): 4 weight rows +
     # 4 gradient rows + 8 crop-sized vectors + small tables (+ the Λ state), within 225 KB
     small = 8 * Cin * 9 + 8 * B * h * w + 1440 + (3 * 4 * 32 * 9 if linear else 0)
     if w <= 16 and B * h * w <= 4096 and small * 4 <= 225 * 1024:

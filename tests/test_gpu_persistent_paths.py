@@ -475,7 +475,7 @@ def test_blur_up_fused_every_cta_two_tiles_ragged_vs_fp64(separable, blur):
 
 # ================================================================== split-K with empty splits
 def _gram_splits(tiles, rows, ntaps):
-    """Replica of gram_splits (csrc/api.cu) and the row-block partition of gram_tc: returns
+    """Replica of gram_splits (csrc/gram_tc.cu) and the row-block partition of gram_tc: returns
     (splits, splits that own no row block)."""
     total_rb = -(-rows // 64)
     s = -(-_sms() // (tiles * ntaps))

@@ -153,7 +153,7 @@ def _conv_pred(K):
 
 def _gram_pred(rows, tiles, ntaps):
     """gram_tc: row-blocks of 64 (four k16 steps x three wgmma = 12 accumulations), chunks of 16,
-    over the row splits of gram_splits (csrc/api.cu), each split weighted by its row-blocks."""
+    over the row splits of gram_splits (csrc/gram_tc.cu), each split weighted by its row-blocks."""
     total_rb = -(-rows // 64)
     splits, _ = _gram_splits(tiles, rows, ntaps)
     rb_per = -(-total_rb // splits)
