@@ -1,6 +1,7 @@
 """TEST INFRASTRUCTURE ONLY — the launch recorder and the per-launch checks that the segmenters'
 launch-by-launch tests (tests/test_gpu_segmenter_layers.py, tests/test_gpu_semseg_layers.py) share;
-tests/test_gpu_backward_layers.py records the StyledConv backward with it (`autograd=True`).
+tests/test_gpu_backward_layers.py records the StyledConv backward with it (`autograd=True`), and
+tests/test_gpu_proggan_layers.py the ProgGAN generator.
 
 `observe` runs a forward with `torch.empty` / `torch.empty_like` and `_cabi.call` wrapped: every
 tensor the run allocates and every launch (entry point and arguments, in order) is recorded, and
@@ -64,12 +65,28 @@ _IO = {
     'rw_torgb_mod_bwd': (3, None, (9, 10, 11)),
     'rw_upfirdn2d': (0, None, (15,)),
     'rw_fused_bias_act': (0, None, (10,)),
+    # the ProgGAN generator's leaves and fused blocks, and the rewriter's rank projection
+    # (tests/test_gpu_proggan_layers.py)
+    'rw_project_rank': (0, None, (8,)),
+    'rw_pixel_norm_nchw': (0, None, (6,)),
+    'rw_nearest_up2': (0, None, (4,)),
+    'rw_pixel_norm_nchw_bwd': (1, None, (7,)),
+    'rw_nearest_up2_bwd': (0, None, (4,)),
+    'rw_proggan_input_fwd': (0, None, (7,)),
+    'rw_proggan_input_bwd': (2, None, (6, 7)),
+    'rw_narrow_conv3x3_dgrad': (0, None, (7,)),
+    'rw_narrow_conv3x3_wgrad': (1, None, (7,)),
+    'rw_torgb1x1': (0, None, (7,)),
+    'rw_torgb1x1_dgrad': (0, None, (7,)),
+    'rw_torgb1x1_wgrad': (1, None, (7,)),
+    'rw_proggan_output_block': (0, None, (10,)),
 }
 # the map passes' (C, hi, lo, ldc, coff) argument indices
 _SLICE = {'rw_seg_map': (3, 12, 13, 14, 15), 'rw_seg_map_phase': (4, 14, 15, 16, 17)}
 # operands a launch overwrites in place (snapshotted before it) and workspace arguments
 _INPLACE = {'rw_dgrad_finish': (0,)}
-_WORKSPACE = {'rw_conv_wgrad': 9, 'rw_conv_up_wgrad': 9, 'rw_torgb_mod_bwd': 12}
+_WORKSPACE = {'rw_conv_wgrad': 9, 'rw_conv_up_wgrad': 9, 'rw_torgb_mod_bwd': 12,
+              'rw_narrow_conv3x3_wgrad': 8, 'rw_torgb1x1_wgrad': 8}
 
 
 # ------------------------------------------------------------------ observation
@@ -537,15 +554,21 @@ def check_stem(m, T, a, sel):
 
 def check_conv3x3(m, T, a, sel, where):
     """rw_conv3x3_bias_act on images `sel` of its batch against the exact-operand reference plus
-    the bias (family 'conv3x3')"""
+    the bias, then, with act set, LeakyReLU 0.2 times the gain (family 'conv3x3').  The activation
+    is 1-Lipschitz times the gain, so S is the pre-activation one times the gain (a gain of 0
+    selects sqrt(2), as in the kernel)."""
     B, Cin, Cout, H, W = a[7:12]
+    act, gain = a[5], float(a[6]) or 2.0 ** 0.5
     wh, wl = (T(p, Cout, 3, 3, Cin).permute(0, 3, 1, 2).double() for p in (a[2], a[3]))
     b = T(a[4], Cout).double()[None, :, None, None]
     out = T(a[12], B, Cout, H, W)
     for i in sel:
         xh, xl = (nchw(T(p), B, H, W, Cin)[i:i + 1].double() for p in (a[0], a[1]))
         ref, S = three(lambda x, w: F.conv2d(x, w, padding=1), (xh, xl), (wh, wl))
-        m.add('conv3x3', err_u(out[i:i + 1], ref + b, S + b.abs()), '%s (K %d)' % (where, 9 * Cin))
+        ref, S = ref + b, S + b.abs()
+        if act:
+            ref, S = torch.where(ref > 0, ref, 0.2 * ref) * gain, S * abs(gain)
+        m.add('conv3x3', err_u(out[i:i + 1], ref, S), '%s (K %d)' % (where, 9 * Cin))
 
 
 def check_rowgemm(m, T, a, B, sel, where):

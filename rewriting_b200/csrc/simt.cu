@@ -1306,8 +1306,12 @@ int rw_add_noise(const float* x, const float* noise, long long noise_bstride,
     set_last_error("rw_add_noise: bad argument");
     return RW_ERR_BAD_ARG;
   }
+  if (B < 0 || C < 0 || HW < 0) {
+    set_last_error("add_noise: bad shape B=%d C=%d HW=%d", B, C, HW);
+    return RW_ERR_BAD_ARG;
+  }
+  if (B == 0 || C == 0 || HW == 0) return RW_OK;
   const long long total = static_cast<long long>(B) * C * HW;
-  if (total <= 0) return RW_OK;
   add_noise_kernel<<<grid_for(total, 256), 256, 0, stream>>>(x, noise, noise_bstride, noise_w, C,
                                                              HW, total, y);
   return check_cuda(cudaGetLastError(), "add_noise launch");
@@ -1412,12 +1416,11 @@ int rw_pixel_norm_nchw(const float* x, int B, int C, int H, int W, int up2, floa
     set_last_error("rw_pixel_norm_nchw: bad argument");
     return RW_ERR_BAD_ARG;
   }
-  const long long n = static_cast<long long>(B) * H * W;
-  if (n <= 0 || C < 1 || (up2 && (reinterpret_cast<uintptr_t>(out) & 7u))) {
+  if (B < 1 || C < 1 || H < 1 || W < 1 || (up2 && (reinterpret_cast<uintptr_t>(out) & 7u))) {
     set_last_error("pixel_norm_nchw: bad shape / alignment");
     return RW_ERR_BAD_ARG;
   }
-  const long long blocks = (n + 255) / 256;
+  const long long blocks = (static_cast<long long>(B) * H * W + 255) / 256;
   pixel_norm_nchw_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(x, B, C, H, W, up2, out);
   return check_cuda(cudaGetLastError(), "pixel_norm_nchw launch");
 }
@@ -1427,11 +1430,11 @@ int rw_nearest_up2(const float* x, long long planes, int H, int W, float* out, r
     set_last_error("rw_nearest_up2: bad argument");
     return RW_ERR_BAD_ARG;
   }
-  const long long n = planes * H * W;
-  if (n <= 0 || (reinterpret_cast<uintptr_t>(out) & 7u)) {
+  if (planes < 1 || H < 1 || W < 1 || (reinterpret_cast<uintptr_t>(out) & 7u)) {
     set_last_error("nearest_up2: bad shape / alignment");
     return RW_ERR_BAD_ARG;
   }
+  const long long n = planes * H * W;
   const long long blocks = (n + 255) / 256;
   nearest_up2_kernel<<<static_cast<unsigned>(blocks), 256, 0, stream>>>(x, n, H, W, out);
   return check_cuda(cudaGetLastError(), "nearest_up2 launch");
