@@ -563,6 +563,42 @@ int rw_semseg_classes(int nsizes, const float* const* logits, const int* map_hw,
                       const int* cat_label, const int* cat_mask, int B, int Ho, int Wo, float* probs,
                       long long* labels, int lchan, int lcoff, long long offset, rw_stream_t stream);
 
+/* ---- BiSeNet face parser (reference metrics/face-parsing.PyTorch): its passes off the convs ----
+ * The same rules as the segmenter passes above (status, no allocation, no atomics, refusal before
+ * launch, image b's results independent of the rest of the batch); the 3x3 and 1x1 convs run on
+ * rw_conv3x3_bias_act and rw_rowgemm, the max pool and the map passes on rw_seg_maxpool / rw_seg_map.
+ * Nearest resizes use torch's index rule without scales: src = min(floor(dst * (float)(in / out)),
+ * in - 1), the scale rounded to fp32 and the product formed in fp32.
+ * rw_face_stem: images as for rw_seg_input (fp32 NCHW [B,3,H,W] in [-1, 1], or uint8 NHWC decoded as
+ *   (u / 255 - 0.5) / 0.5), nearest-resized to S x S on the read, then the 7x7 / stride-2 / pad-3
+ *   conv 3 -> 64 with w [64,3,7,7] (the folded batch norm), + bias [64] and ReLU, summed over
+ *   (channel, row, column) in order in fp32: out [B,64,ceil(S/2),ceil(S/2)].  S 2..8192.
+ * rw_face_attention: the global average pool of x [B,C,H,W] (the sum, then a division by H*W),
+ *   then layer 1: v1 = act1(w1 . pool + b1) with w1 [n1,C]; when w2 is not NULL, layer 2:
+ *   v = act2(w2 . v1 + b2) with w2 [n2,n1].  Biases may be NULL; act 0 none, 1 ReLU, 2 sigmoid
+ *   1 / (1 + exp(-v)).  out [B,n1] or [B,n2].  C, n1, n2 <= 1024.
+ * rw_face_fuse: v = a * s[b,c], + a when plus_a = 1, + add (add_mode 0: none, add NULL; 1: add a
+ *   [B,C] vector broadcast over the map; 2: add a [B,C,H,W] map), each step one IEEE fp32
+ *   operation; a [B,C,H,W], s [B,C].  The result nearest-resized to Ho x Wo is written as fp32
+ *   out [B,C,Ho,Wo] and / or bf16 hi/lo planes [B*(Ho+1)*(Wo+1)][ldc] in channels coff..coff+C-1
+ *   (the rules of rw_seg_map's planes).  C % 64 == 0.
+ * rw_face_labels: logits as padded rows [B*(h+1)*(w+1)][ld] (the rw_rowgemm output, classes
+ *   0..ncls-1, ncls 1..64, no bias); per output pixel (y, x) of Ho x Wo, the pixel (Y, X) of the
+ *   S x S map that the nearest resize S -> Ho x Wo picks, each class's bilinear value there with
+ *   align_corners=True (scale (h-1)/(S-1) in fp32, as torch computes it), and its first argmax (a
+ *   NaN wins, as numpy's argmax): labels int64 [B,1,Ho,Wo]; up [B,ncls,Ho,Wo] the values, when
+ *   not NULL. */
+int rw_face_stem(const void* im, int u8, int B, int H, int W, int S, const float* w,
+                 const float* bias, float* out, rw_stream_t stream);
+int rw_face_attention(const float* x, int B, int C, int H, int W, const float* w1, const float* b1,
+                      int n1, int act1, const float* w2, const float* b2, int n2, int act2,
+                      float* out, rw_stream_t stream);
+int rw_face_fuse(const float* a, const float* s, int plus_a, const float* add, int add_mode, int B,
+                 int C, int H, int W, int Ho, int Wo, float* out, void* out_hi, void* out_lo,
+                 int ldc, int coff, rw_stream_t stream);
+int rw_face_labels(const float* logits, int B, int h, int w, int ld, int ncls, int S, int Ho, int Wo,
+                   long long* labels, float* up, rw_stream_t stream);
+
 /* ---- dissection: unit / label intersection counts (GAN dissection, utils/quickdissect) ----
  * Both calls up-sample a layer's activations act [B,U,h,w] fp32 to H x W as torch's grid_sample
  * with align_corners=True and padding_mode='zeros' does over an axis-affine grid: output (y, x)

@@ -105,6 +105,13 @@ SIGNATURES = {
     'rw_seg_avgpool': (c_int, [c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p]),
     'rw_semseg_classes': (c_int, [c_int, c_p, c_p, c_p, c_int, c_int, c_int, c_p, c_p, c_p, c_p, c_int,
                                   c_int, c_int, c_p, c_p, c_int, c_int, c_ll, c_p]),
+    'rw_face_stem': (c_int, [c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p, c_p, c_p]),
+    'rw_face_attention': (c_int, [c_p, c_int, c_int, c_int, c_int, c_p, c_p, c_int, c_int, c_p, c_p,
+                                  c_int, c_int, c_p, c_p]),
+    'rw_face_fuse': (c_int, [c_p, c_p, c_int, c_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int,
+                             c_p, c_p, c_p, c_int, c_int, c_p]),
+    'rw_face_labels': (c_int, [c_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_p, c_p,
+                               c_p]),
     'rw_upsample_bilinear': (c_int, [c_p, c_int, c_int, c_int, c_int, c_int, c_int, c_d, c_d, c_d,
                                      c_d, c_p, c_p]),
     'rw_dissect_counts': (c_int, [c_p, c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int,

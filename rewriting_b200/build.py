@@ -13,7 +13,7 @@ CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'librw_b200.so')
 SOURCES = ['api.cu', 'conv_tc.cu', 'upconv_tc.cu', 'gram_tc.cu', 'simt.cu', 'bwd.cu', 'rewrite.cu',
            'insert_wide.cu', 'proggan.cu', 'vgg.cu', 'lpips.cu', 'gen_bwd.cu',
-           'seg.cu', 'dissect.cu']
+           'seg.cu', 'dissect.cu', 'faceparse.cu']
 NVCC_FLAGS = [
     '-gencode', 'arch=compute_90a,code=sm_90a',
     '-lineinfo', '-O3', '-std=c++17',

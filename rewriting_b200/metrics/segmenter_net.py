@@ -25,6 +25,11 @@ the conv's own zero padding.  `rw_seg_map_phase` writes the planes in that order
 so only the map passes where d changes reshuffle, and conv_tc is unchanged.  Its PPM average-pools
 with `rw_seg_avgpool` and its class maps come from `rw_semseg_classes`.  The deep-supervision branch
 is not run at inference.
+
+The BiSeNet face parser (`FaceParserNet`, reference metrics/face-parsing.PyTorch) shares the folding
+and the conv helpers.  Its 7x7 / stride-2 stem, the attention vectors, the attention products with
+their nearest 2x up-sampling and the class pass are csrc/faceparse.cu's; its ResNet-18 runs its
+stride-2 convs at stride 1 and subsamples them, as above.
 """
 import ctypes
 
@@ -536,6 +541,256 @@ class SemanticNet(_FoldedNet):
                    ops._p(probs), ops._p(labels), 0 if labels is None else labels.shape[1], lcoff,
                    int(offset), ops._stream())
         return probs
+
+
+FACE_SIZE = 512
+FACE_CLASSES = 19
+FACE_PLANES = (64, 128, 256, 512)
+ACT_NONE, ACT_RELU, ACT_SIGMOID = 0, 1, 2
+
+
+class FaceParserNet(_FoldedNet):
+    """The folded BiSeNet face parser (reference metrics/face-parsing.PyTorch/model.py with its
+    ResNet-18, 19 classes) of one state dict on one device.  Only `feat_out` is computed: the
+    conv_out16 / conv_out32 heads are never read by segment_batch, so their keys are accepted and
+    ignored.  Every batch norm is folded once here."""
+
+    def __init__(self, state_dict, device):
+        super().__init__(device)
+        sd = _strip(state_dict)
+        self.check_shapes(sd)
+        conv_bn = self.conv_bn
+        r = 'cp.resnet.'
+        self.stem = conv_bn(sd, r + 'conv1.weight', r + 'bn1.', 'stem')
+        self.layers = []
+        for li in range(len(FACE_PLANES)):
+            blocks = []
+            for bi in range(2):
+                pre = r + 'layer%d.%d.' % (li + 1, bi)
+                ds = None
+                if li > 0 and bi == 0:
+                    ds = conv_bn(sd, pre + 'downsample.0.weight', pre + 'downsample.1.', '1x1')
+                blocks.append({'stride': 2 if (li > 0 and bi == 0) else 1,
+                               'c1': conv_bn(sd, pre + 'conv1.weight', pre + 'bn1.', '3x3'),
+                               'c2': conv_bn(sd, pre + 'conv2.weight', pre + 'bn2.', '3x3'),
+                               'ds': ds})
+            self.layers.append(blocks)
+        self.conv_avg = self._vec(sd, 'cp.conv_avg.conv.weight', 'cp.conv_avg.bn.')
+        self.arm = {}
+        for name in ('arm16', 'arm32'):
+            self.arm[name] = (conv_bn(sd, 'cp.%s.conv.conv.weight' % name, 'cp.%s.conv.bn.' % name, '3x3'),
+                              self._vec(sd, 'cp.%s.conv_atten.weight' % name, 'cp.%s.bn_atten.' % name))
+        self.head32 = conv_bn(sd, 'cp.conv_head32.conv.weight', 'cp.conv_head32.bn.', '3x3')
+        self.head16 = conv_bn(sd, 'cp.conv_head16.conv.weight', 'cp.conv_head16.bn.', '3x3')
+        self.ffm = conv_bn(sd, 'ffm.convblk.conv.weight', 'ffm.convblk.bn.', '1x1')
+        self.ffm_att = [self._vec(sd, 'ffm.conv%d.weight' % i, None) for i in (1, 2)]
+        self.out_conv = conv_bn(sd, 'conv_out.conv.conv.weight', 'conv_out.conv.bn.', '3x3')
+        w = torch.as_tensor(_get(sd, 'conv_out.conv_out.weight')).detach().float()
+        self.n_class = w.shape[0]
+        self.cls = _Conv('1x1', w, w.new_zeros(w.shape[0]), self.device,
+                         npad=(self.n_class + 63) // 64 * 64)
+
+    @staticmethod
+    def expected_shapes(n_class):
+        """{key: shape} of every state-dict entry the network reads (`module.` stripped)."""
+        s = {}
+
+        def conv(k, o, i, ks):
+            s[k] = (o, i, ks, ks)
+
+        def bn(p, n):
+            for q in ('weight', 'bias', 'running_mean', 'running_var'):
+                s[p + q] = (n,)
+        r = 'cp.resnet.'
+        conv(r + 'conv1.weight', 64, 3, 7)
+        bn(r + 'bn1.', 64)
+        cin = 64
+        for li, p in enumerate(FACE_PLANES):
+            for bi in range(2):
+                pre = r + 'layer%d.%d.' % (li + 1, bi)
+                conv(pre + 'conv1.weight', p, cin, 3)
+                bn(pre + 'bn1.', p)
+                conv(pre + 'conv2.weight', p, p, 3)
+                bn(pre + 'bn2.', p)
+                if li > 0 and bi == 0:
+                    conv(pre + 'downsample.0.weight', p, cin, 1)
+                    bn(pre + 'downsample.1.', p)
+                cin = p
+        conv('cp.conv_avg.conv.weight', 128, 512, 1)
+        bn('cp.conv_avg.bn.', 128)
+        for name, c in (('arm16', 256), ('arm32', 512)):
+            conv('cp.%s.conv.conv.weight' % name, 128, c, 3)
+            bn('cp.%s.conv.bn.' % name, 128)
+            conv('cp.%s.conv_atten.weight' % name, 128, 128, 1)
+            bn('cp.%s.bn_atten.' % name, 128)
+        for name in ('conv_head32', 'conv_head16'):
+            conv('cp.%s.conv.weight' % name, 128, 128, 3)
+            bn('cp.%s.bn.' % name, 128)
+        conv('ffm.convblk.conv.weight', 256, 256, 1)
+        bn('ffm.convblk.bn.', 256)
+        conv('ffm.conv1.weight', 64, 256, 1)
+        conv('ffm.conv2.weight', 256, 64, 1)
+        conv('conv_out.conv.conv.weight', 256, 256, 3)
+        bn('conv_out.conv.bn.', 256)
+        conv('conv_out.conv_out.weight', n_class, 256, 1)
+        return s
+
+    @classmethod
+    def check_shapes(cls, sd):
+        """Refuses (RwError), on the host, a state dict that lacks a key the network reads or
+        holds it in another shape: BiSeNet over ResNet-18 with a feat_out head of 1..64 classes."""
+        w = sd.get('conv_out.conv_out.weight')
+        n = int(w.shape[0]) if isinstance(w, torch.Tensor) and w.dim() == 4 else 0
+        if not 1 <= n <= 64:
+            _fail('face parser: conv_out.conv_out.weight is missing or not [1..64, 256, 1, 1]')
+        for k, shape in cls.expected_shapes(n).items():
+            if k not in sd:
+                _fail('face parser: the state dict has no %s' % k)
+            if tuple(torch.as_tensor(sd[k]).shape) != shape:
+                _fail('face parser: %s has shape %s, BiSeNet has %s'
+                      % (k, tuple(torch.as_tensor(sd[k]).shape), shape))
+
+    def _vec(self, sd, wkey, bnkey):
+        """(weight [n, k], bias [n] or None) on the device of a 1x1 conv applied to a pooled vector,
+        with its batch norm folded when bnkey is given."""
+        w = _get(sd, wkey)
+        if bnkey is None:
+            w, b = torch.as_tensor(w).detach().float(), None
+        else:
+            w, b = fold_bn(w, _bn(sd, bnkey))
+            b = b.to(self.device).contiguous()
+        return w.reshape(w.shape[0], -1).to(self.device).contiguous(), b
+
+    # ------------------------------------------------------------------ layers
+    def _attention(self, x, layers):
+        """rw_face_attention: [B, n] from x [B,C,H,W] through one or two (weight, bias, act)."""
+        B, C, H, W = x.shape
+        (w1, b1, a1) = layers[0]
+        w2, b2, a2 = layers[1] if len(layers) > 1 else (None, None, ACT_NONE)
+        n = (w2 if w2 is not None else w1).shape[0]
+        out = torch.empty((B, n), dtype=torch.float32, device=x.device)
+        _cabi.call('rw_face_attention', ops._p(x), B, C, H, W, ops._p(w1), ops._p(b1), w1.shape[0],
+                   a1, ops._p(w2), ops._p(b2), 0 if w2 is None else w2.shape[0], a2, ops._p(out),
+                   ops._stream())
+        return out
+
+    def _fuse(self, a, s, Ho, Wo, plus_a=False, add=None, planes=None, ldc=None, coff=0, fp32=False):
+        """rw_face_fuse: a * s (+ a) (+ add) nearest-resized to Ho x Wo; returns the fp32 output
+        when `fp32`, else None."""
+        B, C, H, W = a.shape
+        mode = 0 if add is None else (1 if add.dim() == 2 else 2)
+        out = torch.empty((B, C, Ho, Wo), dtype=torch.float32, device=a.device) if fp32 else None
+        hi, lo = planes if planes is not None else (None, None)
+        _cabi.call('rw_face_fuse', ops._p(a), ops._p(s), 1 if plus_a else 0, ops._p(add), mode, B, C,
+                   H, W, Ho, Wo, ops._p(out), ops._p(hi), ops._p(lo), ldc or C, coff, ops._stream())
+        return out
+
+    def stem_forward(self, images, u8, B, H, W):
+        """(planes, fp32, H, W) of layer1's input: the images resized to 512^2, the 7x7 / stride-2
+        conv with bias and ReLU, and the max pool."""
+        d = images.device
+        S = FACE_SIZE
+        h = (S + 1) // 2
+        a = torch.empty((B, 64, h, h), dtype=torch.float32, device=d)
+        _cabi.call('rw_face_stem', ops._p(images), int(u8), B, H, W, S, ops._p(self.stem.w),
+                   ops._p(self.stem.bias), ops._p(a), ops._stream())
+        ho = (h - 1) // 2 + 1
+        xf = torch.empty((B, 64, ho, ho), dtype=torch.float32, device=d)
+        _cabi.call('rw_seg_maxpool', ops._p(a), B, 64, h, h, ops._p(xf), ops._stream())
+        del a
+        X = _planes(B, 64, ho, ho, d)
+        seg_map(xf, False, B, 64, ho, ho, planes=X)
+        return X, xf, ho, ho
+
+    def _basic(self, blk, X, xf, B, H, W):
+        """(planes, fp32, H, W) of a BasicBlock's output from its input planes X / fp32 xf."""
+        c1, c2, ds = blk['c1'], blk['c2'], blk['ds']
+        dev = xf.device
+        a = self._conv3x3(c1, X, B, H, W)
+        if blk['stride'] == 2:
+            Ho, Wo = (H + 1) // 2, (W + 1) // 2
+            P1 = _planes(B, c1.cout, Ho, Wo, dev)
+            seg_map(a, False, B, c1.cout, H, W, mode=1, relu=True, planes=P1)
+        else:
+            Ho, Wo = H, W
+            P1 = self._relu_planes(a, B, c1.cout, H, W)[0]
+        del a
+        a = self._conv3x3(c2, P1, B, Ho, Wo)
+        if ds is not None:
+            Xs = X
+            if blk['stride'] == 2:
+                Xs = _planes(B, ds.cin, Ho, Wo, dev)
+                seg_map(xf, False, B, ds.cin, H, W, mode=1, planes=Xs)
+            r = seg_map(self._conv1x1(ds, Xs, B, Ho, Wo), True, B, ds.cout, Ho, Wo, bias=ds.bias,
+                        fp32=True)
+        else:
+            r = xf
+        Y = _planes(B, c2.cout, Ho, Wo, dev)
+        y = seg_map(a, False, B, c2.cout, Ho, Wo, res=r, relu=True, planes=Y, fp32=True)
+        return Y, y, Ho, Wo
+
+    def encoder(self, images, u8, B, H, W):
+        """[(planes, fp32, H, W)] of feat8, feat16 and feat32 (layers 2, 3 and 4)."""
+        X, xf, h, w = self.stem_forward(images, u8, B, H, W)
+        taps = []
+        for blocks in self.layers:
+            for blk in blocks:
+                X, xf, h, w = self._basic(blk, X, xf, B, h, w)
+            taps.append((X, xf, h, w))
+        return taps[1:]
+
+    def _arm(self, name, X, B, h, w):
+        """an attention refinement module: (feat, its attention vector) from the input planes X"""
+        cv, (aw, ab) = self.arm[name]
+        feat = seg_map(self._conv3x3(cv, X, B, h, w), False, B, cv.cout, h, w, relu=True, fp32=True)
+        return feat, self._attention(feat, [(aw, ab, ACT_SIGMOID)])
+
+    def head(self, taps):
+        """(logits as padded rows [B*(h+1)*(w+1)][n_class padded to 64], (h, w)) of the context
+        path, the feature fusion module and conv_out from the encoder's taps."""
+        (X8, f8, h8, w8), (X16, _, h16, w16), (X32, f32, h32, w32) = taps
+        B = f8.shape[0]
+        d = f8.device
+        avg = self._attention(f32, [(self.conv_avg[0], self.conv_avg[1], ACT_RELU)])
+        feat, att = self._arm('arm32', X32, B, h32, w32)
+        P = _planes(B, 128, h16, w16, d)
+        self._fuse(feat, att, h16, w16, add=avg, planes=P)
+        up32 = seg_map(self._conv3x3(self.head32, P, B, h16, w16), False, B, 128, h16, w16, relu=True,
+                       fp32=True)
+        feat, att = self._arm('arm16', X16, B, h16, w16)
+        P = _planes(B, 128, h8, w8, d)
+        self._fuse(feat, att, h8, w8, add=up32, planes=P)
+        del up32, feat
+        Pc = _planes(B, 256, h8, w8, d)
+        seg_map(f8, False, B, 128, h8, w8, planes=Pc, ldc=256, coff=0)
+        seg_map(self._conv3x3(self.head16, P, B, h8, w8), False, B, 128, h8, w8, relu=True, planes=Pc,
+                ldc=256, coff=128)
+        del P
+        feat = seg_map(self._conv1x1(self.ffm, Pc, B, h8, w8), True, B, 256, h8, w8, bias=self.ffm.bias,
+                       relu=True, fp32=True)
+        del Pc
+        att = self._attention(feat, [(self.ffm_att[0][0], None, ACT_RELU),
+                                     (self.ffm_att[1][0], None, ACT_SIGMOID)])
+        P = _planes(B, 256, h8, w8, d)
+        self._fuse(feat, att, h8, w8, plus_a=True, planes=P)
+        del feat
+        Ph = self._relu_planes(self._conv3x3(self.out_conv, P, B, h8, w8), B, 256, h8, w8)[0]
+        return self._conv1x1(self.cls, Ph, B, h8, w8), (h8, w8)
+
+    def logits(self, images, u8, B, H, W):
+        """(padded rows, (h, w)): the conv_out output at 1/8 of 512^2, as the row-GEMM leaves it."""
+        return self.head(self.encoder(images, u8, B, H, W))
+
+    def labels(self, rows, hw, B, Ho, Wo, want_up=False):
+        """rw_face_labels: (labels int64 [B,1,Ho,Wo], the up-sampled logits [B,n_class,Ho,Wo] or
+        None)."""
+        d = rows.device
+        labels = torch.empty((B, 1, Ho, Wo), dtype=torch.int64, device=d)
+        up = (torch.empty((B, self.n_class, Ho, Wo), dtype=torch.float32, device=d) if want_up
+              else None)
+        _cabi.call('rw_face_labels', ops._p(rows), B, hw[0], hw[1], rows.shape[1], self.n_class,
+                   FACE_SIZE, Ho, Wo, ops._p(labels), ops._p(up), ops._stream())
+        return labels, up
 
 
 def input_pass_norm(images, u8, size, mean, stdev, bgr):
